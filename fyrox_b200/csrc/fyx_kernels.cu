@@ -1005,12 +1005,12 @@ __device__ __forceinline__ void skin_fill_palette(float4 *s_pal, const float *pa
     }
 }
 
-// four vertices (one thread's group) from registers to the two output streams
+// four vertices (one thread's group) from registers to their packed xyz outputs, 3 float4 per stream
 template <int S, int LOG2C>
-__device__ __forceinline__ void skin_quad(const float4 *s_pal, const uint32_t lane, const float4 x4, const float4 y4, const float4 z4,
-                                          const float4 nx4, const float4 ny4, const float4 nz4, const float4 w0, const float4 w1,
-                                          const float4 w2, const float4 w3, const uint4 iq, float4 *po, float4 *no,
-                                          const PackedConsts kc)
+__device__ __forceinline__ void skin_quad_regs(const float4 *s_pal, const uint32_t lane, const float4 x4, const float4 y4, const float4 z4,
+                                               const float4 nx4, const float4 ny4, const float4 nz4, const float4 w0, const float4 w1,
+                                               const float4 w2, const float4 w3, const uint4 iq, float4 (&po)[3], float4 (&no)[3],
+                                               const PackedConsts kc)
 {
     constexpr int C = 1 << LOG2C;
     constexpr int PL = S * C;
@@ -1047,12 +1047,27 @@ __device__ __forceinline__ void skin_quad(const float4 *s_pal, const uint32_t la
         ox[v] = acc_p.x; oy[v] = acc_p.y; oz[v] = acc_z.x;
         mx[v] = acc_n.x; my[v] = acc_n.y; mz[v] = acc_z.y;
     }
-    st_stream(po + 0, make_float4(ox[0], oy[0], oz[0], ox[1]));
-    st_stream(po + 1, make_float4(oy[1], oz[1], ox[2], oy[2]));
-    st_stream(po + 2, make_float4(oz[2], ox[3], oy[3], oz[3]));
-    st_stream(no + 0, make_float4(mx[0], my[0], mz[0], mx[1]));
-    st_stream(no + 1, make_float4(my[1], mz[1], mx[2], my[2]));
-    st_stream(no + 2, make_float4(mz[2], mx[3], my[3], mz[3]));
+    po[0] = make_float4(ox[0], oy[0], oz[0], ox[1]);
+    po[1] = make_float4(oy[1], oz[1], ox[2], oy[2]);
+    po[2] = make_float4(oz[2], ox[3], oy[3], oz[3]);
+    no[0] = make_float4(mx[0], my[0], mz[0], mx[1]);
+    no[1] = make_float4(my[1], mz[1], mx[2], my[2]);
+    no[2] = make_float4(mz[2], mx[3], my[3], mz[3]);
+}
+
+// the same, stored straight to the two output streams (3 + 3 STG.128 with a 48-byte stride between lanes)
+template <int S, int LOG2C>
+__device__ __forceinline__ void skin_quad(const float4 *s_pal, const uint32_t lane, const float4 x4, const float4 y4, const float4 z4,
+                                          const float4 nx4, const float4 ny4, const float4 nz4, const float4 w0, const float4 w1,
+                                          const float4 w2, const float4 w3, const uint4 iq, float4 *po, float4 *no,
+                                          const PackedConsts kc)
+{
+    float4 p[3], n[3];
+    skin_quad_regs<S, LOG2C>(s_pal, lane, x4, y4, z4, nx4, ny4, nz4, w0, w1, w2, w3, iq, p, n, kc);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) st_stream(po + j, p[j]);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) st_stream(no + j, n[j]);
 }
 
 // two vertices (half of a four-vertex group) per thread: 22 input registers instead of 44 — k_skin2 trades wider loads for
@@ -1189,31 +1204,117 @@ void launch_bs_layout(cudaStream_t s, uint32_t n_verts, uint32_t n_shapes, uint3
                                                                                                         reinterpret_cast<uint16_t *>(d_dst), bs_blocks);
 }
 
-// One CTA per tile, inputs loaded straight into registers (LDG.128, L1-bypassing).
-template <int S, int LOG2C, int MINB, bool BS>
+// The 32 groups of a warp are 128 consecutive vertices, i.e. 1 536 contiguous bytes of each output stream.  Lane l puts its
+// three float4 at stage[3l + j] (a quarter-warp's 128-bit stores land in the distinct 16-byte bank groups 3l + j mod 8) and
+// the warp reads them back as stage[l + 32j], so each STG.128 writes 512 contiguous bytes: 6 full-line store instructions per
+// warp and group instead of 6 that each cover half of 48 sectors.  n_f4 = float4 of the warp's valid groups (3 per group).
+__device__ __forceinline__ void store_lines(float4 *stage, const uint32_t lane, const bool valid, const float4 (&p)[3], const float4 (&n)[3],
+                                            float4 *po, float4 *no, const uint32_t n_f4)
+{
+    if (valid) {
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            stage[3 * lane + j] = p[j];
+            stage[96 + 3 * lane + j] = n[j];
+        }
+    }
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        const uint32_t i = lane + 32u * j;
+        if (i < n_f4) {
+            st_stream(po + i, stage[i]);
+            st_stream(no + i, stage[96 + i]);
+        }
+    }
+    __syncwarp(); // every lane has read the stage before the next group overwrites it
+}
+
+__device__ __forceinline__ void cp_async16(float4 *dst, const float4 *src)
+{
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+
+constexpr int kSkinStageF4 = 2 * 96;        // per warp: 128 skinned positions + 128 normals
+constexpr int kSkinRingF4 = kVblkRows * 32; // per warp: the next group of every lane, 11 rows x 32 lanes (5 632 B)
+// shared memory of k_skin: palette planes, output stages, and with PREFETCH the input ring
+template <int S, int LOG2C, bool PREFETCH> constexpr size_t skin_smem_bytes()
+{
+    return sizeof(float4) * ((size_t)3 * S * (1 << LOG2C) + (kBlock / 32) * (kSkinStageF4 + (PREFETCH ? kSkinRingF4 : 0)));
+}
+
+// One CTA per tile; a warp skins 32 consecutive groups (128 vertices) per step and writes them as full lines (store_lines).
+// PREFETCH: while group i is computed, group i + 1 of the same lane is already on its way into the warp's shared ring by
+// 11 cp.async.cg 16-byte copies; lane l only ever reads the 16-byte pieces it copied itself, so cp.async.wait_group is the
+// whole synchronisation (no mbarrier, no __syncwarp, no bank conflicts: a row of the ring is 32 consecutive float4).  The
+// first copies are issued before griddepcontrol.wait (the vertex blocks are static).  Without PREFETCH the inputs are loaded
+// straight into registers (LDG.128, L1-bypassing): the form for palettes too large to leave room for the ring at 2 CTAs/SM.
+template <int S, int LOG2C, int MINB, bool BS, bool PREFETCH>
 __global__ void __launch_bounds__(kBlock, MINB) k_skin(const SkinArrays sk, const SkinTile *__restrict__ tiles, const uint32_t n_tiles,
                                                      const float one, const float negzero)
 {
+    constexpr int PAL = 3 * S * (1 << LOG2C);
     extern __shared__ float4 smem[];
     float4 *const s_pal = smem;
     PackedConsts kc;
     kc.one = make_float2(one, one);
     kc.negzero = make_float2(negzero, negzero);
     const SkinTile T = tiles[blockIdx.x];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    float4 *const stage = smem + PAL + warp * kSkinStageF4;
+    float4 *const ring = smem + PAL + (kBlock / 32) * kSkinStageF4 + warp * kSkinRingF4 + lane; // this lane's column
+    const uint32_t zero = __float_as_uint(negzero) << 1; // 0, but not a constant the compiler can fold
+    auto prefetch = [&](const uint32_t q, const uint32_t dep) {
+        if (q < T.n_quads) {
+            const size_t quad = (size_t)T.quad_start + q;
+            const float4 *row = sk.vblk + (quad >> 5) * kVblkStride + (quad & 31);
+#pragma unroll
+            for (int r = 0; r < kVblkRows; ++r) cp_async16(ring + r * 32 + dep, row + r * 32);
+        }
+        cp_async_commit();
+    };
+    if (PREFETCH) prefetch(threadIdx.x, 0);
     pdl_wait(); // the palettes come from k_palette
     skin_fill_palette<S, LOG2C>(s_pal, sk.palette, T.bone_off, T.n_bones);
     __syncthreads();
-    const uint32_t lane = threadIdx.x & 31u;
-    for (uint32_t q = threadIdx.x; q < T.n_quads; q += kBlock) {
+    for (uint32_t q0 = warp * 32; q0 < T.n_quads; q0 += kBlock) {
+        const uint32_t q = q0 + lane;
+        const bool valid = q < T.n_quads;
         const size_t quad = (size_t)T.quad_start + q;
-        const float4 *row = sk.vblk + (quad >> 5) * kVblkStride + (quad & 31); // block, then this group's column
-        float4 x4 = ld_stream(row + 0 * 32), y4 = ld_stream(row + 1 * 32), z4 = ld_stream(row + 2 * 32);
-        float4 nx4 = ld_stream(row + 3 * 32), ny4 = ld_stream(row + 4 * 32), nz4 = ld_stream(row + 5 * 32);
-        const float4 w0 = ld_stream(row + 6 * 32), w1 = ld_stream(row + 7 * 32), w2 = ld_stream(row + 8 * 32), w3 = ld_stream(row + 9 * 32);
-        const uint4 iq = ld_stream(reinterpret_cast<const uint4 *>(row + 10 * 32));
-        if (BS && T.n_shapes) apply_blend_shapes(sk, T, q, x4, y4, z4, nx4, ny4, nz4);
-        skin_quad<S, LOG2C>(s_pal, lane, x4, y4, z4, nx4, ny4, nz4, w0, w1, w2, w3, iq, reinterpret_cast<float4 *>(sk.opos) + 3 * quad,
-                            reinterpret_cast<float4 *>(sk.onrm) + 3 * quad, kc);
+        float4 x4, y4, z4, nx4, ny4, nz4, w0, w1, w2, w3;
+        uint4 iq;
+        if (PREFETCH) {
+            cp_async_wait_all();
+            if (valid) {
+                x4 = ring[0 * 32]; y4 = ring[1 * 32]; z4 = ring[2 * 32];
+                nx4 = ring[3 * 32]; ny4 = ring[4 * 32]; nz4 = ring[5 * 32];
+                w0 = ring[6 * 32]; w1 = ring[7 * 32]; w2 = ring[8 * 32]; w3 = ring[9 * 32];
+                iq = *reinterpret_cast<const uint4 *>(ring + 10 * 32);
+            }
+            // the next copies overwrite the slots just read: their address depends on a value of every one of those 11 reads,
+            // so no copy can be issued before the reads have completed
+            const uint32_t dep = valid ? ((__float_as_uint(x4.x) ^ __float_as_uint(y4.x) ^ __float_as_uint(z4.x) ^ __float_as_uint(nx4.x) ^
+                                           __float_as_uint(ny4.x) ^ __float_as_uint(nz4.x) ^ __float_as_uint(w0.x) ^ __float_as_uint(w1.x) ^
+                                           __float_as_uint(w2.x) ^ __float_as_uint(w3.x) ^ iq.x) & zero)
+                                       : 0u;
+            prefetch(q + kBlock, dep);
+        } else if (valid) {
+            const float4 *row = sk.vblk + (quad >> 5) * kVblkStride + (quad & 31); // block, then this group's column
+            x4 = ld_stream(row + 0 * 32); y4 = ld_stream(row + 1 * 32); z4 = ld_stream(row + 2 * 32);
+            nx4 = ld_stream(row + 3 * 32); ny4 = ld_stream(row + 4 * 32); nz4 = ld_stream(row + 5 * 32);
+            w0 = ld_stream(row + 6 * 32); w1 = ld_stream(row + 7 * 32); w2 = ld_stream(row + 8 * 32); w3 = ld_stream(row + 9 * 32);
+            iq = ld_stream(reinterpret_cast<const uint4 *>(row + 10 * 32));
+        }
+        float4 p[3], n[3];
+        if (valid) {
+            if (BS && T.n_shapes) apply_blend_shapes(sk, T, q, x4, y4, z4, nx4, ny4, nz4);
+            skin_quad_regs<S, LOG2C>(s_pal, lane, x4, y4, z4, nx4, ny4, nz4, w0, w1, w2, w3, iq, p, n, kc);
+        }
+        const size_t f0 = 3 * ((size_t)T.quad_start + q0); // the warp's first float4 in each output stream
+        store_lines(stage, lane, valid, p, n, reinterpret_cast<float4 *>(sk.opos) + f0, reinterpret_cast<float4 *>(sk.onrm) + f0,
+                    3u * min(32u, T.n_quads - q0));
     }
 }
 
@@ -1787,20 +1888,22 @@ void launch_palette(cudaStream_t s, const NodeArrays &a, const SkinArrays &sk)
     launch_pdl(k_palette, grid_for(sk.n_entries), kBlock, 0, s, a, sk);
 }
 
-template <int S, int LOG2C, int MINB, bool BS> static void launch_skin_t2(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles)
+template <int S, int LOG2C, int MINB, bool BS, bool PREFETCH>
+static void launch_skin_t2(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles)
 {
-    constexpr size_t smem_pal = (size_t)3 * S * (1 << LOG2C) * sizeof(float4);
+    constexpr size_t smem = skin_smem_bytes<S, LOG2C, PREFETCH>();
     static bool init = false;
     if (!init) {
-        cudaFuncSetAttribute(k_skin<S, LOG2C, MINB, BS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pal);
+        cudaFuncSetAttribute(k_skin<S, LOG2C, MINB, BS, PREFETCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         init = true;
     }
-    launch_pdl(k_skin<S, LOG2C, MINB, BS>, n_tiles, kBlock, smem_pal, s, sk, tiles, n_tiles, 1.0f, -0.0f);
+    launch_pdl(k_skin<S, LOG2C, MINB, BS, PREFETCH>, n_tiles, kBlock, smem, s, sk, tiles, n_tiles, 1.0f, -0.0f);
 }
-template <int S, int LOG2C, int MINB> static void launch_skin_t(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles, bool bs)
+template <int S, int LOG2C, int MINB, bool PREFETCH>
+static void launch_skin_t(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles, bool bs)
 {
-    if (bs) launch_skin_t2<S, LOG2C, MINB, true>(s, sk, tiles, n_tiles);
-    else launch_skin_t2<S, LOG2C, MINB, false>(s, sk, tiles, n_tiles);
+    if (bs) launch_skin_t2<S, LOG2C, MINB, true, PREFETCH>(s, sk, tiles, n_tiles);
+    else launch_skin_t2<S, LOG2C, MINB, false, PREFETCH>(s, sk, tiles, n_tiles);
 }
 
 template <int S, int LOG2C, int STAGES, int MINB> static void launch_skin_tma_t(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles)
@@ -1854,13 +1957,14 @@ void launch_skin(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, ui
         else launch_skin2_t<65, 3, 6>(s, sk, tiles, n_tiles);
         return;
     }
-    // 3 CTAs/SM (<= 85 registers): capping at 64 registers for 4 CTAs/SM spills (inherited from the B200 tuning, not re-measured on H100)
+    // <= 64 bones: the prefetching form, 2 CTAs/SM (<= 128 registers; 25 KB palette + 24 KB output stages + 44 KB ring per CTA).
+    // Larger palettes leave no room for the ring at 2 CTAs/SM: loads into registers, 3 CTAs/SM (<= 85 registers).
     if (max_bones <= 64) {       // 8 copies: 25 KB of palette planes
-        launch_skin_t<65, 3, 3>(s, sk, tiles, n_tiles, blend_shapes);
+        launch_skin_t<65, 3, 2, true>(s, sk, tiles, n_tiles, blend_shapes);
     } else if (max_bones <= 128) { // 8 copies: 50 KB
-        launch_skin_t<129, 3, 3>(s, sk, tiles, n_tiles, blend_shapes);
+        launch_skin_t<129, 3, 3, false>(s, sk, tiles, n_tiles, blend_shapes);
     } else {                       // 4 copies (2-way worst case): 49 KB
-        launch_skin_t<257, 2, 3>(s, sk, tiles, n_tiles, blend_shapes);
+        launch_skin_t<257, 2, 3, false>(s, sk, tiles, n_tiles, blend_shapes);
     }
 }
 
