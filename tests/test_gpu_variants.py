@@ -32,8 +32,11 @@ def test_cull_variants_match_the_oracle(variant):
 @pytest.mark.timeout(1000)
 @pytest.mark.parametrize("variant", ["tma2", "tma3", "pair5"])  # TMA rings (2 / 3 stages); two vertices per thread
 def test_tma_skinning_variants_match_the_oracle(variant):
-    """k_skin_tma: vertex blocks staged by cp.async.bulk + mbarrier rings (fyx_kernels.cu)."""
-    _run({"FYX_SKIN_VARIANT": variant}, ["test_gpu_parity.py", "test_gpu_fullsize.py"], "skin or render_prep")
+    """k_skin_tma: vertex blocks staged by cp.async.bulk + mbarrier rings; k_skin2: two vertices per thread (fyx_kernels.cu).
+    The variants replace launches of <= 64 bones without blend shapes; test_gpu_skinning_paths.py also runs every other
+    band and the blend-shape launches under the same setting."""
+    _run({"FYX_SKIN_VARIANT": variant}, ["test_gpu_parity.py", "test_gpu_fullsize.py", "test_gpu_skinning_paths.py"],
+         "skin or render_prep or skinning_paths")
 
 
 @pytest.mark.timeout(1000)
@@ -49,4 +52,5 @@ def test_subforest_kernel_on_and_off_match_the_oracle(mode):
 def test_fold_in_stream_order_matches_the_oracle():
     """FYX_SIDE_FOLD=0: asynchronous frames run the skinned-mesh fold in order on the main stream instead of beside the palette /
     skinning kernels (the default, exercised by every pipelined test of the normal run)."""
-    _run({"FYX_SIDE_FOLD": "0"}, ["test_gpu_parity.py", "test_gpu_fuzz.py"], "pipelined or render_prep or random_call or skin")
+    _run({"FYX_SIDE_FOLD": "0"}, ["test_gpu_parity.py", "test_gpu_fuzz.py", "test_gpu_skinning_paths.py"],
+         "pipelined or render_prep or random_call or skin or skinning_paths")
