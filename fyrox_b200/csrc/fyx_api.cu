@@ -121,7 +121,6 @@ struct fyx_ctx {
     uint32_t n_nodes = 0, n_slots = 0, root = FYX_NONE, n_renderable = 0;
     std::vector<uint32_t> slot_of_node, node_of_slot, level_off;
     NodeArrays a{};
-    DevBuf b_vis;
     DevBuf b_parent, b_flags, b_mask, b_gidx, b_L[3], b_G[3], b_la[3], b_wa[3], b_slot_of_node;
     bool have_topology = false, updated_once = false;
     SubforestPlan sf{};  // deep levels walked by one launch (fyx_internal.h); n_ctas = 0: one launch per level everywhere
@@ -390,7 +389,6 @@ void rebuild_node_arrays(fyx_ctx *c)
     a.flags = c->b_flags.as<uint32_t>();
     a.mask = c->b_mask.as<uint32_t>();
     a.gidx = c->b_gidx.as<uint32_t>();
-    a.vis = c->b_vis.as<uint8_t>();
     for (int i = 0; i < 3; ++i) {
         a.L[i] = c->b_L[i].as<float4>();
         a.G[i] = c->b_G[i].as<float4>();
@@ -403,7 +401,6 @@ void rebuild_node_arrays(fyx_ctx *c)
 void to_dev_frustum(const fyx_frustum &f, uint32_t cam_mask, uint32_t pass_flags, FrustumDev &d)
 {
     for (int p = 0; p < 6; ++p) d.plane[p] = make_float4(f.planes[p][0], f.planes[p][1], f.planes[p][2], f.planes[p][3]);
-    for (int i = 0; i < 8; ++i) d.corner[i] = make_float4(f.corners[i][0], f.corners[i][1], f.corners[i][2], 0.0f);
     for (int q = 0; q < 3; ++q)
         for (int k = 0; k < 4; ++k) d.pn[q][k] = make_float2(f.planes[2 * q][k], f.planes[2 * q + 1][k]);
     // distinct corner coordinates per axis (bit-pattern equality, so -0/+0 and NaNs stay separate entries:
@@ -471,12 +468,8 @@ int32_t prepare_cull(fyx_ctx *c, uint32_t nf, const fyx_frustum *fr, const uint3
     c->cp.counts = V.d_counts;
     c->cp.one = 1.0f;
     c->cp.negzero = -0.0f;
-    c->cp.shadow_bits = 0u;
-    c->cp.cam_same = 1u;
     for (uint32_t f = 0; f < nf; ++f) {
         to_dev_frustum(fr[f], cam_mask ? cam_mask[f] : 0xFFFFFFFFu, pass_flags ? pass_flags[f] : 0u, c->cp.f[f]);
-        if (c->cp.f[f].pass_flags & FYX_PASS_SHADOW) c->cp.shadow_bits |= 1u << f;
-        if (c->cp.f[f].cam_mask != c->cp.f[0].cam_mask) c->cp.cam_same = 0u;
         // worst case every alive node is visible (fyx_set_flags may turn any of them renderable)
         int32_t rc = dev_ensure(c, V.b_vis[f], sizeof(uint32_t) * std::max<size_t>(c->n_slots, 1));
         if (rc) return rc;
@@ -519,10 +512,6 @@ int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cu
     }
     if (c->sf.n_ctas) { // the deep levels (small sub-trees: skeletons) in one launch
         launch_update_subforest(c->stream, c->a, c->sf, all, cull);
-        c->launches++;
-    }
-    if (cull && cull_defers_compaction(cull->nf)) { // the level kernels stored visible bits: build the lists now
-        launch_compact_vis(c->stream, c->a, *cull);
         c->launches++;
     }
     if (c->fold.n) {
@@ -701,7 +690,7 @@ extern "C" void fyx_destroy(fyx_ctx *c)
     fyx_comm_destroy_internal(c);
     inst_free(c);
     anim_free(c);
-    DevBuf *bufs[] = {&c->b_vis, &c->b_parent, &c->b_flags, &c->b_mask, &c->b_gidx, &c->b_slot_of_node, &c->d_stage, &c->b_statics, &c->b_trs, &c->b_vblk,
+    DevBuf *bufs[] = {&c->b_parent, &c->b_flags, &c->b_mask, &c->b_gidx, &c->b_slot_of_node, &c->d_stage, &c->b_statics, &c->b_trs, &c->b_vblk,
                       &c->b_ms_range, &c->b_ms_bundle, &c->b_ms_skin, &c->b_prune, &c->b_sf_rng, &c->b_opos, &c->b_onrm, &c->b_bs, &c->b_bs_w, &c->b_surf_of_slot, &c->b_surf_bones, &c->b_palette, &c->b_bone_slot, &c->b_tiles, &c->b_fold_node,
                       &c->b_fold_begin, &c->b_fold_bone, &c->b_fold_stale_idx, &c->b_late_slot, &c->b_stale_pos, &c->b_counts_packed, &c->b_counts_all};
     for (DevBuf *b : bufs) dev_free(*b);
@@ -1096,8 +1085,6 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     if ((rc = dev_ensure(c, c->b_flags, n * 4))) return rc;
     if ((rc = dev_ensure(c, c->b_mask, n * 4))) return rc;
     if ((rc = dev_ensure(c, c->b_gidx, n * 4))) return rc;
-    if ((rc = dev_ensure(c, c->b_vis, (n + 15) & ~size_t(7)))) return rc;
-    CU(cudaMemset(c->b_vis.p, 0, c->b_vis.bytes));
     if ((rc = dev_ensure(c, c->b_slot_of_node, std::max<size_t>(capacity, 1) * 4))) return rc;
     for (int k = 0; k < 3; ++k) {
         if ((rc = dev_ensure(c, c->b_L[k], n * sizeof(float4)))) return rc;

@@ -31,7 +31,6 @@ struct NodeArrays {
     uint32_t *flags;
     uint32_t *mask;
     uint32_t *gidx;
-    uint8_t *vis; // per slot: bit f = visible in frustum f of the current cull (deferred compaction, k_compact_vis)
     float4 *L[3];
     float4 *G[3];
     float2 *la[3];
@@ -45,8 +44,6 @@ struct CullParams {
     uint32_t *out_slot[FYX_MAX_FRUSTA]; // the same entries as HBM slots (nullptr unless fyx_enable_instances)
     uint32_t *counts;              // counts[f * kCountStride]
     float one, negzero;            // 1.0f, -0.0f: run-time operands of the unfusable packed FMAs (fyx_math.cuh)
-    uint32_t shadow_bits;          // bit f: frustum f is a shadow pass (FYX_PASS_SHADOW)
-    uint32_t cam_same;             // non-zero: every frustum of the call has the same camera render mask (f[0].cam_mask)
 };
 
 struct SkinArrays {
@@ -170,9 +167,6 @@ struct SubforestPlan {
     uint32_t n_ctas = 0, n_levels = 0, first_level = 0; // deep levels = [first_level, first_level + n_levels)
     const uint2 *rng = nullptr;                        // [cta][level] = slot range (begin, end)
 };
-// deferred compaction: the level kernels only store each node's visible bits; this pass turns the bit column into the lists
-void launch_compact_vis(cudaStream_t s, const NodeArrays &a, const CullParams &cp);
-bool cull_defers_compaction(int nf);
 void launch_update_subforest(cudaStream_t s, const NodeArrays &a, const SubforestPlan &sf, bool update_all, const CullParams *cull);
 
 // ---- launchers (fyx_kernels.cu) ----

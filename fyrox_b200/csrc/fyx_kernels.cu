@@ -3,9 +3,6 @@
 // All kernels are HBM-bandwidth-bound streaming kernels over SoA planes (no tensor cores: 4x4 f32
 // work at ~0.3-1 flop/B).  Arithmetic follows fyx_math.cuh (one rounding per op, reference order).
 // Each kernel names the reference code it replaces (paths relative to the Fyrox tree).
-#include <cstdlib>
-#include <cstring>
-
 #include <cuda_fp16.h>
 
 #include "fyx_internal.h"
@@ -76,114 +73,6 @@ static void launch_pdl(void (*kernel)(Params...), unsigned grid, unsigned block,
 }
 
 // ------------------------------------------------------------------------------------------------
-// Warp-level pre-reject of whole frusta (the 6-frusta cull is instruction-issue-bound, not HBM-bound).
-//
-// Siblings sit in adjacent slots, so the 32 boxes of a warp are neighbours in the world and most frusta of a
-// multi-frustum call (five of six cube faces, typically) contain none of them.  The warp reduces its boxes to
-// their union U and tests U ONCE, with the work spread over the lanes: lane l < 3*nf evaluates plane pair
-// l%3 of frustum l/3 on U's max-corner, lane c (two rounds) tests frustum corner c against U.  Frustum f is
-// dead for the warp iff some plane rejects U and no corner of f lies in U; then every participating lane's
-// own test is false too, bit for bit:
-//   * cloud test: for a lane box B ⊆ U the operand picked per axis (min for a negative normal component, max
-//     otherwise) is never further along the normal than U's, products by the same constant and sums are
-//     monotone under round-to-nearest, so s_B <= s_U <= 0 on that plane — the lane's max-corner (hence all
-//     eight corners, frustum.rs:205-219) is behind it;
-//   * fallback (frustum.rs:236-242): a corner outside U on some axis (exact compares) is outside B on it.
-// Participating lanes = candidates with frustum culling on and a tame box (finite, ordered: the premise of
-// the max-corner form); everything else keeps its own per-lane test.  CPU check of the claim on random and
-// adversarial warps: tests/test_cull_trick_cpu.py.
-// ------------------------------------------------------------------------------------------------
-struct PrefTable {
-    float4 e[FYX_MAX_FRUSTA * 3][5];      // per (frustum, plane pair): pn[0..3] (2 float4), vsel[3][2] (6 u32), pad: 80 B stride = conflict-free LDS.128
-    float4 corner[FYX_MAX_FRUSTA * 8];
-};
-
-__device__ __forceinline__ void pref_fill(PrefTable &T, const CullParams &cp, const int nf)
-{
-    const int t = threadIdx.x;
-    if (t < 3 * nf) {
-        const int f = t / 3, q = t % 3;
-        const FrustumDev &F = cp.f[f];
-        T.e[t][0] = make_float4(F.pn[q][0].x, F.pn[q][0].y, F.pn[q][1].x, F.pn[q][1].y);
-        T.e[t][1] = make_float4(F.pn[q][2].x, F.pn[q][2].y, F.pn[q][3].x, F.pn[q][3].y);
-        T.e[t][2] = make_float4(__uint_as_float(F.vsel[q][0][0]), __uint_as_float(F.vsel[q][0][1]), __uint_as_float(F.vsel[q][1][0]),
-                                __uint_as_float(F.vsel[q][1][1]));
-        T.e[t][3] = make_float4(__uint_as_float(F.vsel[q][2][0]), __uint_as_float(F.vsel[q][2][1]), 0.f, 0.f);
-    }
-    const int c = t - 64;
-    if (c >= 0 && c < 8 * nf) T.corner[c] = cp.f[c >> 3].corner[c & 7];
-}
-
-// sm_90's redux.sync reduces integers only: the warp min / max of non-NaN floats is taken on their order-preserving
-// s32 image (negative floats get their magnitude bits flipped; the map is its own inverse, and -0 orders below +0).
-__device__ __forceinline__ int32_t f32_order_key(const float v)
-{
-    const int32_t i = __float_as_int(v);
-    return i ^ ((i >> 31) & 0x7FFFFFFF);
-}
-__device__ __forceinline__ float warp_min_f32(const float v)
-{
-    const int32_t k = __reduce_min_sync(0xFFFFFFFFu, f32_order_key(v));
-    return __int_as_float(k ^ ((k >> 31) & 0x7FFFFFFF));
-}
-__device__ __forceinline__ float warp_max_f32(const float v)
-{
-    const int32_t k = __reduce_max_sync(0xFFFFFFFFu, f32_order_key(v));
-    return __int_as_float(k ^ ((k >> 31) & 0x7FFFFFFF));
-}
-
-// Must be called by all 32 lanes.  part: this lane's box takes part in the union.  Returns the frusta that are NOT
-// proven dead for the participating lanes (bit f).
-template <int NFT>
-__device__ __forceinline__ uint32_t warp_live_frusta(const bool part, const float2 wx, const float2 wy, const float2 wz, const int nf_rt,
-                                                     const PrefTable &T, const PackedConsts &kc)
-{
-    const int nf = (NFT > 0) ? NFT : nf_rt;
-    if (!__any_sync(0xFFFFFFFFu, part)) return 0u; // nobody needs a geometric test
-    const float inf = __int_as_float(0x7f800000);
-    const float ulx = warp_min_f32(part ? wx.x : inf), uhx = warp_max_f32(part ? wx.y : -inf);
-    const float uly = warp_min_f32(part ? wy.x : inf), uhy = warp_max_f32(part ? wy.y : -inf);
-    const float ulz = warp_min_f32(part ? wz.x : inf), uhz = warp_max_f32(part ? wz.y : -inf);
-    const int lane = threadIdx.x & 31;
-    bool rej = false;
-    if (lane < 3 * nf) {
-        const float4 a = T.e[lane][0], b = T.e[lane][1], s0 = T.e[lane][2], s1 = T.e[lane][3];
-        const uint32_t xl = __float_as_uint(ulx), xh = __float_as_uint(uhx), yl = __float_as_uint(uly), yh = __float_as_uint(uhy),
-                       zl = __float_as_uint(ulz), zh = __float_as_uint(uhz);
-        const float2 vx = make_float2(pick(xl, xh, __float_as_uint(s0.x)), pick(xl, xh, __float_as_uint(s0.y)));
-        const float2 vy = make_float2(pick(yl, yh, __float_as_uint(s0.z)), pick(yl, yh, __float_as_uint(s0.w)));
-        const float2 vz = make_float2(pick(zl, zh, __float_as_uint(s1.x)), pick(zl, zh, __float_as_uint(s1.y)));
-        const float2 s = add2(add2(add2(mul2(make_float2(a.x, a.y), vx, kc), mul2(make_float2(a.z, a.w), vy, kc), kc),
-                                   mul2(make_float2(b.x, b.y), vz, kc), kc), make_float2(b.z, b.w), kc);
-        rej = (s.x <= 0.0f) | (s.y <= 0.0f);
-    }
-    const uint32_t rb = __ballot_sync(0xFFFFFFFFu, rej);
-    uint32_t live = 0u;
-    constexpr int kRounds = (NFT > 0) ? (8 * NFT + 31) / 32 : (8 * (int)FYX_MAX_FRUSTA + 31) / 32;
-#pragma unroll
-    for (int r = 0; r < kRounds; ++r) {
-        if (NFT == 0 && r * 4 >= nf) break;
-        const int c = lane + 32 * r;
-        bool in = false;
-        if (c < 8 * nf) {
-            const float4 k = T.corner[c];
-            in = (k.x >= ulx) & (k.x <= uhx) & (k.y >= uly) & (k.y <= uhy) & (k.z >= ulz) & (k.z <= uhz);
-        }
-        const uint32_t cb = __ballot_sync(0xFFFFFFFFu, in);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int f = 4 * r + j;
-            if (f < nf) {
-                const bool cloud_fail = ((rb >> (3 * f)) & 7u) != 0u;
-                const bool corner_in = ((cb >> (8 * j)) & 0xFFu) != 0u;
-                live |= (!cloud_fail || corner_in) ? (1u << f) : 0u;
-            }
-        }
-    }
-    return live;
-}
-
-// ------------------------------------------------------------------------------------------------
 // NodeTrait::should_be_rendered (scene/node/mod.rs:231-256) + the shadow-pass cast_shadows test of
 // Mesh::collect_render_data (scene/mesh/mod.rs:696-698) + reachability from Graph::root
 // (iterate_recursive, renderer/bundle.rs:988-1004), for every frustum of the call.  Bit f of the
@@ -191,7 +80,8 @@ __device__ __forceinline__ uint32_t warp_live_frusta(const bool part, const floa
 // ------------------------------------------------------------------------------------------------
 // NFT: number of frusta known at compile time (the loop is unrolled and cp.f[f] becomes constant-bank operands of the
 // arithmetic instead of ~35 indexed parameter loads per frustum), 0 = run-time count.
-// live: frusta whose geometric test this lane still has to run (all ones without the warp-level pre-reject).
+// live: frusta whose geometric test this lane has to run.  Every caller passes all ones; the mask stays because without it
+// ptxas allocates k_fold_bones differently (same results, different instructions).
 constexpr uint32_t kNeedBits = FYX_NODE_ALIVE | FYX_NODE_RENDERABLE | FYX_NODE_REACHABLE | FYX_NODE_GLOBAL_VISIBILITY | FYX_NODE_GLOBAL_ENABLED;
 
 template <int NFT>
@@ -204,8 +94,6 @@ __device__ __forceinline__ uint32_t cull_bits(const uint32_t nf, const uint32_t 
         bool ok = (mask & cp.f[f].cam_mask) != 0u;
         ok &= !((cp.f[f].pass_flags & FYX_PASS_SHADOW) && !(nf & FYX_NODE_CAST_SHADOWS));
         if (ok && (nf & FYX_NODE_FRUSTUM_CULLING)) {
-            // a frustum proven dead for the warp's union box needs no test — unless this lane's box is not tame (it took
-            // no part in the union)
             if (((live >> f) & 1u) || !tame) ok = frustum_intersects_aabb(cp.f[f], wx, wy, wz, kc, tame);
             else ok = false;
         }
@@ -221,135 +109,25 @@ __device__ __forceinline__ uint32_t cull_bits(const uint32_t nf, const uint32_t 
 }
 
 // Per-warp part of the cull, called by all 32 lanes: cand = this lane holds a node that may be emitted at all.
-// PRE: warp-level pre-reject on.
-template <int NFT, bool PRE>
+template <int NFT>
 __device__ __forceinline__ uint32_t cull_warp(const bool cand, const uint32_t nf, const uint32_t mask, const float2 wx, const float2 wy,
-                                              const float2 wz, const CullParams &cp, const PrefTable *T)
+                                              const float2 wz, const CullParams &cp)
 {
     PackedConsts kc;
     kc.one = make_float2(cp.one, cp.one);
     kc.negzero = make_float2(cp.negzero, cp.negzero);
     const bool ok = cand && (nf & kNeedBits) == kNeedBits;
     const bool tame = ok && aabb_is_tame(wx, wy, wz);
-    uint32_t live = 0xFFFFFFFFu;
-    if (PRE) live = warp_live_frusta<NFT>(tame && (nf & FYX_NODE_FRUSTUM_CULLING), wx, wy, wz, cp.nf, *T, kc);
-    return ok ? cull_bits<NFT>(nf, mask, wx, wy, wz, cp, kc, tame, live) : 0u;
-}
-
-// ------------------------------------------------------------------------------------------------
-// The same predicate in warp-convergent form (VAR bit 5), called by all 32 lanes.  The per-lane form above runs the
-// geometric test inside `if (ok && culling)`: every frustum costs a divergence region (BSSY/BSYNC, an activemask per
-// vote) and ~12 instructions of mask / pass / flag tests.  Here
-//   * the cheap tests produce one bit mask of eligible frusta per lane (per call: shadow passes as a bit mask, the
-//     camera masks compared once when they are all equal);
-//   * the plane tests of frustum f run for the WHOLE warp whenever some lane needs them (the other lanes' values are
-//     ignored: same issue slots either way), so every vote uses the full mask and every branch is warp-uniform;
-//   * the corner-in-box fallback runs only for lanes a plane rejected without the margin of `pm` (fyx_math.cuh).
-// Lanes whose box is not tame (never in practice) take the literal per-lane test.  Same booleans as cull_bits.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool corner_in_box(const FrustumDev &f, const float2 x, const float2 y, const float2 z)
-{
-    uint32_t alive = 0xFFu;
-    const float2 box[3] = {x, y, z};
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        const float lo = box[a].x, hi = box[a].y;
-        const float4 v0 = f.ax_val[a][0];
-        uint32_t m = 0u;
-        m |= ((v0.x >= lo) & (v0.x <= hi)) ? f.ax_mask[a][0] : 0u;
-        m |= ((v0.y >= lo) & (v0.y <= hi)) ? f.ax_mask[a][1] : 0u;
-        m |= ((v0.z >= lo) & (v0.z <= hi)) ? f.ax_mask[a][2] : 0u;
-        m |= ((v0.w >= lo) & (v0.w <= hi)) ? f.ax_mask[a][3] : 0u;
-        if (((f.n_ax >> (8 * a)) & 0xFFu) > 4u) {
-            const float4 v1 = f.ax_val[a][1];
-            m |= ((v1.x >= lo) & (v1.x <= hi)) ? f.ax_mask[a][4] : 0u;
-            m |= ((v1.y >= lo) & (v1.y <= hi)) ? f.ax_mask[a][5] : 0u;
-            m |= ((v1.z >= lo) & (v1.z <= hi)) ? f.ax_mask[a][6] : 0u;
-            m |= ((v1.w >= lo) & (v1.w <= hi)) ? f.ax_mask[a][7] : 0u;
-        }
-        alive &= m;
-    }
-    return alive != 0u;
-}
-
-template <int NFT>
-__device__ __forceinline__ uint32_t cull_warp_conv(const bool cand, const uint32_t nf, const uint32_t mask, const float2 wx, const float2 wy,
-                                                   const float2 wz, const CullParams &cp)
-{
-    constexpr uint32_t kFull = 0xFFFFFFFFu;
-    PackedConsts kc;
-    kc.one = make_float2(cp.one, cp.one);
-    kc.negzero = make_float2(cp.negzero, cp.negzero);
-    const int nfr = (NFT > 0) ? NFT : cp.nf;
-    const uint32_t all = (nfr >= 32) ? kFull : ((1u << nfr) - 1u);
-    const bool ok = cand && (nf & kNeedBits) == kNeedBits;
-    // eligible frusta of this lane: render mask ∩ camera mask, shadow passes only for shadow casters
-    uint32_t elig;
-    if (cp.cam_same) {
-        elig = (mask & cp.f[0].cam_mask) ? all : 0u;
-    } else {
-        elig = 0u;
-        if (NFT > 0) {
-#pragma unroll
-            for (int f = 0; f < NFT; ++f) elig |= (mask & cp.f[f].cam_mask) ? (1u << f) : 0u;
-        } else {
-            for (int f = 0; f < nfr; ++f) elig |= (mask & cp.f[f].cam_mask) ? (1u << f) : 0u;
-        }
-    }
-    if (!(nf & FYX_NODE_CAST_SHADOWS)) elig &= ~cp.shadow_bits;
-    if (!ok) elig = 0u;
-    const bool geo = (nf & FYX_NODE_FRUSTUM_CULLING) != 0u;
-    uint32_t want = geo ? elig : 0u; // frusta whose geometric test this lane needs
-    if (!__any_sync(kFull, want != 0u)) return elig;
-    uint32_t bits = geo ? 0u : elig;
-    const bool tame = aabb_is_tame(wx, wy, wz);
-    if (__any_sync(kFull, want != 0u && !tame)) { // literal per-lane path for boxes outside the max-corner form's premise
-        if (want != 0u && !tame) {
-            for (int f = 0; f < nfr; ++f)
-                if (((want >> f) & 1u) && frustum_intersects_aabb(cp.f[f], wx, wy, wz, kc, false)) bits |= 1u << f;
-            want = 0u;
-        }
-    }
-    const uint32_t xl = __float_as_uint(wx.x), xh = __float_as_uint(wx.y), yl = __float_as_uint(wy.x), yh = __float_as_uint(wy.y),
-                   zl = __float_as_uint(wz.x), zh = __float_as_uint(wz.y);
-    auto one = [&](const int f) {
-        const bool act = ((want >> f) & 1u) != 0u;
-        if (!__any_sync(kFull, act)) return;
-        const FrustumDev &F = cp.f[f];
-        bool cloud = act, strong = false;
-#pragma unroll
-        for (int q = 0; q < 3; ++q) {
-            const float2 vx = make_float2(pick(xl, xh, F.vsel[q][0][0]), pick(xl, xh, F.vsel[q][0][1]));
-            const float2 vy = make_float2(pick(yl, yh, F.vsel[q][1][0]), pick(yl, yh, F.vsel[q][1][1]));
-            const float2 vz = make_float2(pick(zl, zh, F.vsel[q][2][0]), pick(zl, zh, F.vsel[q][2][1]));
-            const float2 s = add2(add2(add2(mul2(F.pn[q][0], vx, kc), mul2(F.pn[q][1], vy, kc), kc), mul2(F.pn[q][2], vz, kc), kc), F.pn[q][3], kc);
-            cloud &= !(s.x <= 0.0f) & !(s.y <= 0.0f);
-            strong |= (s.x < F.pm[q].x) | (s.y < F.pm[q].y);
-            if (q < 2 && !__any_sync(kFull, cloud)) break; // every lane that wanted this frustum is rejected already
-        }
-        bool res = cloud;
-        const bool fb = act && !cloud && !strong; // rejected by a plane it (nearly) touches: the reference's corner loop decides
-        if (__any_sync(kFull, fb)) {
-            if (fb) res = corner_in_box(F, wx, wy, wz);
-        }
-        bits |= res ? (1u << f) : 0u;
-    };
-    if (NFT > 0) {
-#pragma unroll
-        for (int f = 0; f < NFT; ++f) one(f);
-    } else {
-        for (int f = 0; f < nfr; ++f) one(f);
-    }
-    return bits;
+    return ok ? cull_bits<NFT>(nf, mask, wx, wy, wz, cp, kc, tame, 0xFFFFFFFFu) : 0u;
 }
 
 // ------------------------------------------------------------------------------------------------
 // Compaction of the visible node indices.  Replaces the Vec pushes of RenderDataBundleStorage::push
 // (renderer/bundle.rs:1248-1278).  Order inside a list is unspecified.  Two forms:
-//  * CTA-wide: warp ballot + popc rank, per-warp counts in shared memory, one atomicAdd per (CTA, frustum);
-//  * warp-wide: one atomicAdd per (warp, frustum that has a visible lane) — no shared memory, no barriers, and
-//    frusta nobody in the warp is visible in cost nothing (the 6-frusta kernel is issue-bound: ~180 -> ~30
-//    instructions per warp); the counters sit on their own 128 B lines.
+//  * CTA-wide (the level and cull kernels): warp ballot + popc rank, per-warp counts in shared memory, one atomicAdd per
+//    (CTA, frustum);
+//  * warp-wide (k_fold_bones, whose cull runs in warp 0 only): one atomicAdd per (warp, frustum that has a visible lane);
+//    the counters sit on their own 128 B lines.
 // Both must be called by every thread of the CTA / warp.
 // ------------------------------------------------------------------------------------------------
 template <int NFT>
@@ -494,23 +272,12 @@ __device__ __forceinline__ void update_node(const NodeArrays &a, const uint32_t 
     }
 }
 
-// VAR: bit 0 = warp-level pre-reject of whole frusta, bit 1 = warp-wide compaction (else CTA-wide), bit 2 = FYX_UPDATE_ALL
-// specialisation (own columns, render mask and list index loaded up front)
-// bit 4 = compiled for 8 resident CTAs per SM (<= 32 registers: the 40 the kernel wants limit it to 48 of 64 warps, and it is
-// latency-bound); bit 5 = warp-convergent predicate (cull_warp_conv; replaces bit 0)
-template <int NFT, int VAR>
-__global__ void __launch_bounds__(kBlock, (VAR & 16) ? 8 : 6) k_update_level(const NodeArrays a, const uint32_t lo, const uint32_t hi,
-                                                         const uint32_t update_all, const CullParams cp)
+// NFT < 0: no fused cull.  UA: FYX_UPDATE_ALL (update_node; the render mask and list index are loaded up front too).
+template <int NFT, bool UA>
+__global__ void __launch_bounds__(kBlock, 6) k_update_level(const NodeArrays a, const uint32_t lo, const uint32_t hi, const uint32_t update_all,
+                                                            const CullParams cp)
 {
     pdl_trigger();
-    constexpr bool PRE = (NFT >= 0) && (VAR & 1);
-    constexpr bool UA = (VAR & 4) != 0;
-    __shared__ __align__(16) unsigned char s_pref[PRE ? sizeof(PrefTable) : 16];
-    PrefTable *T = reinterpret_cast<PrefTable *>(s_pref);
-    if (PRE) {
-        pref_fill(*T, cp, NFT > 0 ? NFT : cp.nf);
-        __syncthreads();
-    }
     const uint32_t slot = lo + blockIdx.x * kBlock + threadIdx.x;
     uint32_t nf = 0u;
     float2 wx = make_float2(0.f, 0.f), wy = wx, wz = wx;
@@ -518,22 +285,16 @@ __global__ void __launch_bounds__(kBlock, (VAR & 16) ? 8 : 6) k_update_level(con
     uint32_t mask = 0u, gi_early = 0u;
     if (UA && (NFT >= 0) && valid) { // static columns: no reason to wait for anything
         mask = a.mask[slot];
-        if (!(VAR & 8)) gi_early = a.gidx[slot];
+        gi_early = a.gidx[slot];
     }
     if (valid) update_node<(NFT >= 0), UA>(a, slot, update_all, nf, wx, wy, wz);
     else pdl_wait();
     if (NFT >= 0) {
         const bool cand = valid && !(nf & F_SKINNED);
         if (!UA) mask = cand ? a.mask[slot] : 0u;
-        const uint32_t vis_bits = (VAR & 32) ? cull_warp_conv<(NFT > 0 ? NFT : 0)>(cand, nf, mask, wx, wy, wz, cp)
-                                             : cull_warp<(NFT > 0 ? NFT : 0), PRE>(cand, nf, mask, wx, wy, wz, cp, T);
-        if (VAR & 8) { // deferred compaction: one byte per node now, the lists are built by k_compact_vis after the last level
-            if (valid) a.vis[slot] = (uint8_t)vis_bits;
-            return;
-        }
+        const uint32_t vis_bits = cull_warp<(NFT > 0 ? NFT : 0)>(cand, nf, mask, wx, wy, wz, cp);
         const uint32_t gi = UA ? gi_early : (vis_bits ? a.gidx[slot] : 0u);
-        if (VAR & 2) compact_emit_warp(vis_bits, gi, slot, cp);
-        else compact_emit<(NFT > 0 ? NFT : 0)>(vis_bits, gi, slot, cp);
+        compact_emit<(NFT > 0 ? NFT : 0)>(vis_bits, gi, slot, cp);
     }
 }
 
@@ -544,7 +305,7 @@ __global__ void __launch_bounds__(kBlock, (VAR & 16) ? 8 : 6) k_update_level(con
 // memory for the children.  Same arithmetic, flags, change tracking and fused cull as k_update_level; what it removes
 // is a kernel launch per level for levels of a few thousand nodes (C3: six skeleton levels of 10 k - 320 k nodes).
 // ------------------------------------------------------------------------------------------------
-template <int NFT, bool UA, bool DEFER>
+template <int NFT, bool UA>
 __global__ void __launch_bounds__(kBlock) k_update_subforest(const NodeArrays a, const uint2 *__restrict__ rng, const int n_levels,
                                                              const uint32_t update_all, const CullParams cp)
 {
@@ -638,82 +399,14 @@ __global__ void __launch_bounds__(kBlock) k_update_subforest(const NodeArrays a,
             if (NFT >= 0) {
                 const bool cand = valid && !(nf & F_SKINNED);
                 const uint32_t mask = cand ? a.mask[slot] : 0u;
-                const uint32_t vis_bits = cull_warp<(NFT > 0 ? NFT : 0), false>(cand, nf, mask, wx, wy, wz, cp, nullptr);
-                if (DEFER) {
-                    if (valid) a.vis[slot] = (uint8_t)vis_bits;
-                } else {
-                    const uint32_t gi = vis_bits ? a.gidx[slot] : 0u;
-                    compact_emit<(NFT > 0 ? NFT : 0)>(vis_bits, gi, slot, cp);
-                }
+                const uint32_t vis_bits = cull_warp<(NFT > 0 ? NFT : 0)>(cand, nf, mask, wx, wy, wz, cp);
+                const uint32_t gi = vis_bits ? a.gidx[slot] : 0u;
+                compact_emit<(NFT > 0 ? NFT : 0)>(vis_bits, gi, slot, cp);
             }
         }
         __syncthreads(); // this level's rows are complete (and the previous level's are no longer read)
         prevA = r.x;
         prevB = r.y;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Deferred compaction.  With the cull fused into the level kernels, the compaction (ballots, shared-memory prefix, one
-// atomic per CTA and frustum, three CTA-wide barriers) sat at the end of a 900-instruction thread and every warp of a CTA
-// waited for the slowest one.  Here the level kernels store ONE byte per node (its visible bits) and this small pass —
-// 1 B read per node, gidx only where something is visible — turns the byte column into the lists: a thread takes 8
-// consecutive slots, a warp 256, one atomicAdd per (warp, frustum with anything visible).  Skinned meshes are emitted by
-// k_fold_bones (their byte is 0).  Order inside a list stays unspecified.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBlock) k_compact_vis(const NodeArrays a, const CullParams cp)
-{
-    pdl_trigger();
-    pdl_wait();
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint64_t first = ((uint64_t)blockIdx.x * kBlock + threadIdx.x) * 8u;
-    unsigned long long v = 0ull;
-    if (first + 8u <= a.cap) {
-        v = *reinterpret_cast<const unsigned long long *>(a.vis + first); // the column is 256-byte aligned: 8-byte loads are
-    } else if (first < a.cap) {
-        for (uint32_t j = 0; j < 8u && first + j < a.cap; ++j) v |= (unsigned long long)a.vis[first + j] << (8u * j);
-    }
-    uint32_t frusta = 0u; // frusta this thread has entries for
-    {
-        unsigned long long t = v;
-        t |= t >> 32;
-        t |= t >> 16;
-        t |= t >> 8;
-        frusta = (uint32_t)(t & 0xFFu);
-    }
-    uint32_t m = __reduce_or_sync(0xFFFFFFFFu, frusta);
-    if (!m) return;
-    uint32_t gi[8];
-    if (v) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) gi[j] = (first + j < a.cap) ? a.gidx[first + j] : 0u;
-    }
-    while (m) {
-        const int f = __ffs(m) - 1;
-        m &= m - 1u;
-        const unsigned long long sel = (v >> f) & 0x0101010101010101ull; // byte j = node j visible in f
-        const uint32_t cnt = (uint32_t)__popcll(sel);
-        uint32_t incl = cnt; // inclusive warp scan
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
-            if (lane >= (uint32_t)d) incl += t;
-        }
-        const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-        uint32_t base = 0u;
-        if (lane == 0) base = atomicAdd(cp.counts + f * kCountStride, total);
-        base = __shfl_sync(0xFFFFFFFFu, base, 0) + incl - cnt;
-        if (cnt) {
-            uint32_t k = 0;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                if ((sel >> (8 * j)) & 1ull) {
-                    cp.out[f][base + k] = gi[j];
-                    if (cp.out_slot[f]) cp.out_slot[f][base + k] = (uint32_t)(first + j);
-                    ++k;
-                }
-            }
-        }
     }
 }
 
@@ -724,17 +417,10 @@ __global__ void __launch_bounds__(kBlock) k_compact_vis(const NodeArrays a, cons
 // prune != nullptr: one launch per hierarchy level [lo, hi) — a node is hidden for the frusta in which an ancestor pruned the
 // DFS: a statically batched mesh that is rendered (RdcControlFlow::Break, scene/mesh/mod.rs:725; renderer/bundle.rs:996-1001)
 // or, through lodp, a LOD object out of range.  prune[slot] = frusta hidden for the node's children.
-template <int NFT, int VAR>
+template <int NFT>
 __global__ void __launch_bounds__(kBlock) k_cull(const NodeArrays a, const CullParams cp, const uint32_t *lodp, const uint32_t lo, const uint32_t hi,
                                                  uint32_t *prune)
 {
-    constexpr bool PRE = (VAR & 1) != 0;
-    __shared__ __align__(16) unsigned char s_pref[PRE ? sizeof(PrefTable) : 16];
-    PrefTable *T = reinterpret_cast<PrefTable *>(s_pref);
-    if (PRE) {
-        pref_fill(*T, cp, NFT > 0 ? NFT : cp.nf);
-        __syncthreads();
-    }
     const uint32_t slot = lo + blockIdx.x * kBlock + threadIdx.x;
     const bool valid = slot < hi;
     uint32_t nf = 0u, mask = 0u;
@@ -746,7 +432,7 @@ __global__ void __launch_bounds__(kBlock) k_cull(const NodeArrays a, const CullP
         wy = ld_stream(a.wa[1] + slot);
         wz = ld_stream(a.wa[2] + slot);
     }
-    uint32_t vis_bits = (VAR & 32) ? cull_warp_conv<NFT>(valid, nf, mask, wx, wy, wz, cp) : cull_warp<NFT, PRE>(valid, nf, mask, wx, wy, wz, cp, T);
+    uint32_t vis_bits = cull_warp<NFT>(valid, nf, mask, wx, wy, wz, cp);
     uint32_t hidden = 0u;
     if (valid && (lodp || prune)) {
         if (lodp) hidden = lodp[slot]; // frusta whose LOD filter hides the node or one of its ancestors
@@ -758,8 +444,7 @@ __global__ void __launch_bounds__(kBlock) k_cull(const NodeArrays a, const CullP
         if (prune) prune[slot] = hidden | ((nf & FYX_NODE_STATIC_BATCH) ? vis_bits : 0u);
     }
     const uint32_t gi = vis_bits ? a.gidx[slot] : 0u;
-    if (VAR & 2) compact_emit_warp(vis_bits, gi, slot, cp);
-    else compact_emit<NFT>(vis_bits, gi, slot, cp);
+    compact_emit<NFT>(vis_bits, gi, slot, cp);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1055,95 +740,6 @@ __device__ __forceinline__ void skin_quad_regs(const float4 *s_pal, const uint32
     no[2] = make_float4(mz[2], mx[3], my[3], mz[3]);
 }
 
-// the same, stored straight to the two output streams (3 + 3 STG.128 with a 48-byte stride between lanes)
-template <int S, int LOG2C>
-__device__ __forceinline__ void skin_quad(const float4 *s_pal, const uint32_t lane, const float4 x4, const float4 y4, const float4 z4,
-                                          const float4 nx4, const float4 ny4, const float4 nz4, const float4 w0, const float4 w1,
-                                          const float4 w2, const float4 w3, const uint4 iq, float4 *po, float4 *no,
-                                          const PackedConsts kc)
-{
-    float4 p[3], n[3];
-    skin_quad_regs<S, LOG2C>(s_pal, lane, x4, y4, z4, nx4, ny4, nz4, w0, w1, w2, w3, iq, p, n, kc);
-#pragma unroll
-    for (int j = 0; j < 3; ++j) st_stream(po + j, p[j]);
-#pragma unroll
-    for (int j = 0; j < 3; ++j) st_stream(no + j, n[j]);
-}
-
-// two vertices (half of a four-vertex group) per thread: 22 input registers instead of 44 — k_skin2 trades wider loads for
-// more resident warps (k_skin sits at 24 warps per SM with 80 registers and is bound by load latency, not by bandwidth)
-template <int S, int LOG2C>
-__device__ __forceinline__ void skin_pair(const float4 *s_pal, const uint32_t lane, const float2 x2, const float2 y2, const float2 z2, const float2 nx2,
-                                          const float2 ny2, const float2 nz2, const float2 w0, const float2 w1, const float2 w2, const float2 w3,
-                                          const uint2 iq, float2 *po, float2 *no, const PackedConsts kc)
-{
-    constexpr int C = 1 << LOG2C;
-    constexpr int PL = S * C;
-    const float px[2] = {x2.x, x2.y}, py[2] = {y2.x, y2.y}, pz[2] = {z2.x, z2.y};
-    const float nx[2] = {nx2.x, nx2.y}, ny[2] = {ny2.x, ny2.y}, nz[2] = {nz2.x, nz2.y};
-    const float wk2[2][4] = {{w0.x, w1.x, w2.x, w3.x}, {w0.y, w1.y, w2.y, w3.y}};
-    const uint32_t iv[2] = {iq.x, iq.y};
-    float ox[2], oy[2], oz[2], mx[2], my[2], mz[2];
-#pragma unroll
-    for (int v = 0; v < 2; ++v) {
-        const float2 pxx = make_float2(px[v], px[v]), pyy = make_float2(py[v], py[v]), pzz = make_float2(pz[v], pz[v]);
-        const float2 nxx = make_float2(nx[v], nx[v]), nyy = make_float2(ny[v], ny[v]), nzz = make_float2(nz[v], nz[v]);
-        const float2 pnx = make_float2(px[v], nx[v]), pny = make_float2(py[v], ny[v]), pnz = make_float2(pz[v], nz[v]);
-        float2 acc_p = make_float2(0.0f, 0.0f), acc_n = make_float2(0.0f, 0.0f), acc_z = make_float2(0.0f, 0.0f);
-        const float *wk = wk2[v];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t bone = (iv[v] >> (8 * k)) & 0xFFu;
-            const float4 *row = s_pal + (((lane - bone) & (uint32_t)(C - 1)) * S + bone);
-            const float4 A = row[0], B = row[PL], Z = row[2 * PL];
-            const float2 ww = make_float2(wk[k], wk[k]);
-            const float2 t = add2(add2(add2(mul2(lo2(A), pxx, kc), mul2(hi2(A), pyy, kc), kc), mul2(lo2(B), pzz, kc), kc), hi2(B), kc);
-            acc_p = add2(acc_p, mul2(t, ww, kc), kc);
-            const float2 r = add2(add2(mul2(lo2(A), nxx, kc), mul2(hi2(A), nyy, kc), kc), mul2(lo2(B), nzz, kc), kc);
-            acc_n = add2(acc_n, mul2(r, ww, kc), kc);
-            float2 z = add2(add2(mul2(pnx, make_float2(Z.x, Z.x), kc), mul2(pny, make_float2(Z.y, Z.y), kc), kc), mul2(pnz, make_float2(Z.z, Z.z), kc), kc);
-            z.x = FYX_ADD(z.x, Z.w);
-            acc_z = add2(acc_z, mul2(z, ww, kc), kc);
-        }
-        ox[v] = acc_p.x; oy[v] = acc_p.y; oz[v] = acc_z.x;
-        mx[v] = acc_n.x; my[v] = acc_n.y; mz[v] = acc_z.y;
-    }
-    st_stream(po + 0, make_float2(ox[0], oy[0]));
-    st_stream(po + 1, make_float2(oz[0], ox[1]));
-    st_stream(po + 2, make_float2(oy[1], oz[1]));
-    st_stream(no + 0, make_float2(mx[0], my[0]));
-    st_stream(no + 1, make_float2(mz[0], mx[1]));
-    st_stream(no + 2, make_float2(my[1], mz[1]));
-}
-
-template <int S, int LOG2C, int MINB>
-__global__ void __launch_bounds__(kBlock, MINB) k_skin2(const SkinArrays sk, const SkinTile *__restrict__ tiles, const uint32_t n_tiles, const float one,
-                                                      const float negzero)
-{
-    extern __shared__ float4 smem[];
-    float4 *const s_pal = smem;
-    PackedConsts kc;
-    kc.one = make_float2(one, one);
-    kc.negzero = make_float2(negzero, negzero);
-    const SkinTile T = tiles[blockIdx.x];
-    pdl_wait(); // the palettes come from k_palette
-    skin_fill_palette<S, LOG2C>(s_pal, sk.palette, T.bone_off, T.n_bones);
-    __syncthreads();
-    const uint32_t lane = threadIdx.x & 31u;
-    for (uint32_t h = threadIdx.x; h < 2u * T.n_quads; h += kBlock) {
-        const size_t quad = (size_t)T.quad_start + (h >> 1);
-        const float2 *row = reinterpret_cast<const float2 *>(sk.vblk + (quad >> 5) * kVblkStride + (quad & 31)) + (h & 1u);
-        const float2 x2 = ld_stream(row + 0 * 64), y2 = ld_stream(row + 1 * 64), z2 = ld_stream(row + 2 * 64);
-        const float2 nx2 = ld_stream(row + 3 * 64), ny2 = ld_stream(row + 4 * 64), nz2 = ld_stream(row + 5 * 64);
-        const float2 w0 = ld_stream(row + 6 * 64), w1 = ld_stream(row + 7 * 64), w2 = ld_stream(row + 8 * 64), w3 = ld_stream(row + 9 * 64);
-        const float2 iqf = ld_stream(row + 10 * 64);
-        const uint2 iq = make_uint2(__float_as_uint(iqf.x), __float_as_uint(iqf.y));
-        const size_t pair = 2 * quad + (h & 1u); // index of the vertex pair: 6 floats = 3 float2 per stream
-        skin_pair<S, LOG2C>(s_pal, lane, x2, y2, z2, nx2, ny2, nz2, w0, w1, w2, w3, iq, reinterpret_cast<float2 *>(sk.opos) + 3 * pair,
-                            reinterpret_cast<float2 *>(sk.onrm) + 3 * pair, kc);
-    }
-}
-
 // N4: blend shapes ahead of the skinning (standard.shader:167-173): for i in 0..blendShapesCount:
 //   inputPosition.xyz += offsets.position * weight;  inputNormal += offsets.normal * weight
 // in shape order, offsets = the f16 texels of BlendShapesContainer::from_lists (scene/mesh/surface.rs:92-218, exact in
@@ -1315,110 +911,6 @@ __global__ void __launch_bounds__(kBlock, MINB) k_skin(const SkinArrays sk, cons
         const size_t f0 = 3 * ((size_t)T.quad_start + q0); // the warp's first float4 in each output stream
         store_lines(stage, lane, valid, p, n, reinterpret_cast<float4 *>(sk.opos) + f0, reinterpret_cast<float4 *>(sk.onrm) + f0,
                     3u * min(32u, T.n_quads - q0));
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_skin with TMA bulk staging (the experiment BASELINE.json's north_star names; a tested variant, not the default).
-// The vertex input is already laid out for it: a block of 128 vertices is 5 632 contiguous bytes (11 rows x 512 B).
-// Every WARP owns a ring of STAGES block buffers in shared memory and its own mbarriers: lane 0 issues one 1-D
-// cp.async.bulk (global -> shared, completion counted in bytes on the mbarrier) per block, the warp waits on the
-// barrier's phase parity, reads its 11 rows with conflict-free LDS.128 (lane l owns group l of the block), computes,
-// stores, and refills the buffer with the block STAGES ahead.  The vertex blocks are static, so the first copies are
-// issued BEFORE griddepcontrol.wait (they overlap k_palette's tail); the palette planes are then filled as in k_skin.
-// Selected with FYX_SKIN_VARIANT=tma2 (4 palette copies, 2 stages, 2 CTAs/SM) or tma3 (8 copies, 3 stages, 1 CTA/SM).
-// ------------------------------------------------------------------------------------------------
-constexpr uint32_t kVblkBytes = kVblkStride * sizeof(float4); // 5632
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(const uint32_t bar, const uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(const uint32_t bar, const uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(const uint32_t bar, const uint32_t parity)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE_%=;\n"
-        "bra WAIT_%=;\n"
-        "DONE_%=:\n"
-        "}\n" ::"r"(bar),
-        "r"(parity)
-        : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(const uint32_t dst, const void *src, const uint32_t bytes, const uint32_t bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
-                 : "memory");
-}
-
-template <int S, int LOG2C, int STAGES, int MINB>
-__global__ void __launch_bounds__(kBlock, MINB) k_skin_tma(const SkinArrays sk, const SkinTile *__restrict__ tiles, const uint32_t n_tiles,
-                                                         const float one, const float negzero)
-{
-    constexpr int C = 1 << LOG2C;
-    constexpr int W = kBlock / 32;
-    constexpr uint32_t kPalBytes = (3u * S * C * sizeof(float4) + 127u) & ~127u;
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    float4 *const s_pal = reinterpret_cast<float4 *>(smem_raw);
-    unsigned char *const ring = smem_raw + kPalBytes;
-    uint64_t *const bars = reinterpret_cast<uint64_t *>(ring + (size_t)W * STAGES * kVblkBytes);
-    PackedConsts kc;
-    kc.one = make_float2(one, one);
-    kc.negzero = make_float2(negzero, negzero);
-    const SkinTile T = tiles[blockIdx.x];
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    const uint32_t b0 = T.quad_start >> 5, b1 = (T.quad_start + T.n_quads + 31u) >> 5; // blocks [b0, b1) hold the tile
-    const uint32_t q_lo = T.quad_start, q_hi = T.quad_start + T.n_quads;
-    unsigned char *const my_ring = ring + (size_t)warp * STAGES * kVblkBytes;
-    const uint32_t my_bar = smem_u32(bars + warp * STAGES);
-    if (lane == 0) {
-#pragma unroll
-        for (int st = 0; st < STAGES; ++st) mbar_init(my_bar + 8u * st, 1u);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    // prologue: the first STAGES blocks of this warp (static data: does not wait for the predecessor kernel)
-    if (lane == 0) {
-#pragma unroll
-        for (int st = 0; st < STAGES; ++st) {
-            const uint32_t b = b0 + warp + (uint32_t)st * W;
-            if (b < b1) {
-                mbar_expect_tx(my_bar + 8u * st, kVblkBytes);
-                bulk_g2s(smem_u32(my_ring + (size_t)st * kVblkBytes), sk.vblk + (size_t)b * kVblkStride, kVblkBytes, my_bar + 8u * st);
-            }
-        }
-    }
-    pdl_wait(); // the palettes come from k_palette
-    skin_fill_palette<S, LOG2C>(s_pal, sk.palette, T.bone_off, T.n_bones);
-    __syncthreads();
-    uint32_t j = 0;
-    for (uint32_t b = b0 + warp; b < b1; b += W, ++j) {
-        const uint32_t st = j % STAGES, parity = (j / STAGES) & 1u;
-        mbar_wait(my_bar + 8u * st, parity);
-        const float4 *row = reinterpret_cast<const float4 *>(my_ring + (size_t)st * kVblkBytes) + lane;
-        const size_t quad = ((size_t)b << 5) + lane;
-        if (quad >= q_lo && quad < q_hi) {
-            const float4 x4 = row[0 * 32], y4 = row[1 * 32], z4 = row[2 * 32];
-            const float4 nx4 = row[3 * 32], ny4 = row[4 * 32], nz4 = row[5 * 32];
-            const float4 w0 = row[6 * 32], w1 = row[7 * 32], w2 = row[8 * 32], w3 = row[9 * 32];
-            const uint4 iq = *reinterpret_cast<const uint4 *>(row + 10 * 32);
-            skin_quad<S, LOG2C>(s_pal, lane, x4, y4, z4, nx4, ny4, nz4, w0, w1, w2, w3, iq, reinterpret_cast<float4 *>(sk.opos) + 3 * quad,
-                                reinterpret_cast<float4 *>(sk.onrm) + 3 * quad, kc);
-        }
-        __syncwarp(); // every lane has read the buffer before it is refilled
-        const uint32_t nb = b + (uint32_t)STAGES * W;
-        if (lane == 0 && nb < b1) {
-            mbar_expect_tx(my_bar + 8u * st, kVblkBytes);
-            bulk_g2s(smem_u32(my_ring + (size_t)st * kVblkBytes), sk.vblk + (size_t)nb * kVblkStride, kVblkBytes, my_bar + 8u * st);
-        }
     }
 }
 
@@ -1700,83 +1192,37 @@ __global__ void __launch_bounds__(kBlock) k_compact_gathered(const uint32_t *pad
 // ------------------------------------------------------------------------------------------------
 static inline unsigned grid_for(uint64_t n) { return (unsigned)((n + kBlock - 1) / kBlock); }
 
-// Cull variant (bit 0: warp-level pre-reject of whole frusta, bit 1: warp-wide compaction).  Default: both for
-// multi-frustum calls, compaction only for a single frustum; FYX_CULL_VARIANT=0..3 overrides (A/B measurements).
-static int cull_variant(int nf)
+// The usual frustum counts get an unrolled cull: camera, CSM cascades, cube faces.
+template <int NFT>
+static void launch_update_level_t(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, bool update_all, const CullParams &cp)
 {
-    static int forced = [] {
-        const char *e = getenv("FYX_CULL_VARIANT");
-        return (e && *e) ? atoi(e) & 63 : -1;
-    }();
-    if (forced >= 0) return forced;
-    (void)nf;
-    return 4; // A/B on H100 in DESIGN.md §4: CTA-wide compaction, no pre-reject, FYX_UPDATE_ALL specialisation, 6 CTAs/SM
+    if (update_all) launch_pdl(k_update_level<NFT, true>, grid_for(hi - lo), kBlock, 0, s, a, lo, hi, 1u, cp);
+    else launch_pdl(k_update_level<NFT, false>, grid_for(hi - lo), kBlock, 0, s, a, lo, hi, 0u, cp);
 }
-
-// bit 3 of the variant: the level kernels store visible bits, k_compact_vis builds the lists (bit 1 is then meaningless)
-bool cull_defers_compaction(int nf) { return (cull_variant(nf) & 8) != 0; }
-
-#define FYX_DISPATCH_VAR(KERNEL, NF, VAR, ...)                                   \
-    switch (VAR) {                                                               \
-    case 0: launch_pdl(KERNEL<NF, 0>, __VA_ARGS__); break;                       \
-    case 1: launch_pdl(KERNEL<NF, 1>, __VA_ARGS__); break;                       \
-    case 2: launch_pdl(KERNEL<NF, 2>, __VA_ARGS__); break;                       \
-    case 3: launch_pdl(KERNEL<NF, 3>, __VA_ARGS__); break;                       \
-    case 4: launch_pdl(KERNEL<NF, 4>, __VA_ARGS__); break;                       \
-    case 5: launch_pdl(KERNEL<NF, 5>, __VA_ARGS__); break;                       \
-    case 6: launch_pdl(KERNEL<NF, 6>, __VA_ARGS__); break;                       \
-    case 7: launch_pdl(KERNEL<NF, 7>, __VA_ARGS__); break;                       \
-    case 8: launch_pdl(KERNEL<NF, 8>, __VA_ARGS__); break;                       \
-    case 9: launch_pdl(KERNEL<NF, 9>, __VA_ARGS__); break;                       \
-    case 12: launch_pdl(KERNEL<NF, 12>, __VA_ARGS__); break;                     \
-    case 13: launch_pdl(KERNEL<NF, 13>, __VA_ARGS__); break;                     \
-    case 20: launch_pdl(KERNEL<NF, 20>, __VA_ARGS__); break;                     \
-    case 21: launch_pdl(KERNEL<NF, 21>, __VA_ARGS__); break;                     \
-    case 28: launch_pdl(KERNEL<NF, 28>, __VA_ARGS__); break;                     \
-    case 32: launch_pdl(KERNEL<NF, 32>, __VA_ARGS__); break;                     \
-    case 34: launch_pdl(KERNEL<NF, 34>, __VA_ARGS__); break;                     \
-    case 36: launch_pdl(KERNEL<NF, 36>, __VA_ARGS__); break;                     \
-    case 38: launch_pdl(KERNEL<NF, 38>, __VA_ARGS__); break;                     \
-    case 52: launch_pdl(KERNEL<NF, 52>, __VA_ARGS__); break;                     \
-    default: launch_pdl(KERNEL<NF, 54>, __VA_ARGS__); break;                     \
-    }
 
 void launch_update_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, bool update_all, const CullParams *cull)
 {
     if (hi <= lo) return;
-    if (cull) {
-        const unsigned g = grid_for(hi - lo);
-        const uint32_t ua = update_all ? 1u : 0u;
-        int var = (cull_variant(cull->nf) & 3) | ((update_all && (cull_variant(cull->nf) & 4)) ? 4 : 0);
-        if (cull_variant(cull->nf) & 8) var = (var & 5) | 8; // deferred compaction: 8, 9, 12, 13
-        if ((cull_variant(cull->nf) & 16) && update_all) // 32-register builds: 20 (= 4 | 16), 21 (+ pre-reject), 28 (= 12 | 16)
-            var = (cull_variant(cull->nf) & 8) ? 28 : ((cull_variant(cull->nf) & 1) ? 21 : 20);
-        if (cull_variant(cull->nf) & 32) // warp-convergent predicate: 32, 34 (+ warp compaction); FYX_UPDATE_ALL: 36, 38, 52, 54
-            var = 32 | (cull_variant(cull->nf) & 2) | (update_all ? ((cull_variant(cull->nf) & 16) ? 20 : (cull_variant(cull->nf) & 4)) : 0);
-        switch (cull->nf) { // the usual frustum counts get an unrolled cull: camera, CSM cascades, cube faces
-        case 1: FYX_DISPATCH_VAR(k_update_level, 1, var, g, kBlock, 0, s, a, lo, hi, ua, *cull); break;
-        case 2: FYX_DISPATCH_VAR(k_update_level, 2, var, g, kBlock, 0, s, a, lo, hi, ua, *cull); break;
-        case 3: FYX_DISPATCH_VAR(k_update_level, 3, var, g, kBlock, 0, s, a, lo, hi, ua, *cull); break;
-        case 4: FYX_DISPATCH_VAR(k_update_level, 4, var, g, kBlock, 0, s, a, lo, hi, ua, *cull); break;
-        case 6: FYX_DISPATCH_VAR(k_update_level, 6, var, g, kBlock, 0, s, a, lo, hi, ua, *cull); break;
-        default: FYX_DISPATCH_VAR(k_update_level, 0, var, g, kBlock, 0, s, a, lo, hi, ua, *cull); break;
-        }
-    } else {
+    if (!cull) {
         CullParams none;
         none.nf = 0;
-        if (update_all && (cull_variant(0) & 16)) launch_pdl(k_update_level<-1, 20>, grid_for(hi - lo), kBlock, 0, s, a, lo, hi, 1u, none);
-        else if (update_all && (cull_variant(0) & 4)) launch_pdl(k_update_level<-1, 4>, grid_for(hi - lo), kBlock, 0, s, a, lo, hi, 1u, none);
-        else launch_pdl(k_update_level<-1, 0>, grid_for(hi - lo), kBlock, 0, s, a, lo, hi, update_all ? 1u : 0u, none);
+        launch_update_level_t<-1>(s, a, lo, hi, update_all, none);
+        return;
+    }
+    switch (cull->nf) {
+    case 1: launch_update_level_t<1>(s, a, lo, hi, update_all, *cull); break;
+    case 2: launch_update_level_t<2>(s, a, lo, hi, update_all, *cull); break;
+    case 3: launch_update_level_t<3>(s, a, lo, hi, update_all, *cull); break;
+    case 4: launch_update_level_t<4>(s, a, lo, hi, update_all, *cull); break;
+    case 6: launch_update_level_t<6>(s, a, lo, hi, update_all, *cull); break;
+    default: launch_update_level_t<0>(s, a, lo, hi, update_all, *cull); break;
     }
 }
 
 template <int NFT> static void launch_subforest_t(cudaStream_t s, const NodeArrays &a, const SubforestPlan &sf, bool ua, const CullParams &cp)
 {
-    const bool defer = NFT >= 0 && cull_defers_compaction(cp.nf);
-    if (ua && defer) launch_pdl(k_update_subforest<NFT, true, true>, sf.n_ctas, kBlock, 0, s, a, sf.rng, (int)sf.n_levels, 1u, cp);
-    else if (ua) launch_pdl(k_update_subforest<NFT, true, false>, sf.n_ctas, kBlock, 0, s, a, sf.rng, (int)sf.n_levels, 1u, cp);
-    else if (defer) launch_pdl(k_update_subforest<NFT, false, true>, sf.n_ctas, kBlock, 0, s, a, sf.rng, (int)sf.n_levels, 0u, cp);
-    else launch_pdl(k_update_subforest<NFT, false, false>, sf.n_ctas, kBlock, 0, s, a, sf.rng, (int)sf.n_levels, 0u, cp);
+    if (ua) launch_pdl(k_update_subforest<NFT, true>, sf.n_ctas, kBlock, 0, s, a, sf.rng, (int)sf.n_levels, 1u, cp);
+    else launch_pdl(k_update_subforest<NFT, false>, sf.n_ctas, kBlock, 0, s, a, sf.rng, (int)sf.n_levels, 0u, cp);
 }
 
 void launch_update_subforest(cudaStream_t s, const NodeArrays &a, const SubforestPlan &sf, bool update_all, const CullParams *cull)
@@ -1793,12 +1239,6 @@ void launch_update_subforest(cudaStream_t s, const NodeArrays &a, const Subfores
     case 6: launch_subforest_t<6>(s, a, sf, update_all, *cull); break;
     default: launch_subforest_t<0>(s, a, sf, update_all, *cull); break;
     }
-}
-
-void launch_compact_vis(cudaStream_t s, const NodeArrays &a, const CullParams &cp)
-{
-    if (!a.cap || !cp.nf) return;
-    launch_pdl(k_compact_vis, grid_for(((uint64_t)a.cap + 7) / 8), kBlock, 0, s, a, cp);
 }
 
 // Reflection-probe selection of from_graph (renderer/bundle.rs:918-925): the last ReflectionProbe in pool order whose world box
@@ -1829,31 +1269,17 @@ void launch_cull_lights(cudaStream_t s, const NodeArrays &a, const CullParams &c
     k_cull_lights<<<grid_for(a.cap), kBlock, 0, s>>>(a, cp, d_out_ptrs, counts);
 }
 
-template <int NF> static void launch_cull_t(cudaStream_t s, unsigned g, int var, const NodeArrays &a, const CullParams &cp, const uint32_t *lodp, uint32_t lo,
-                                            uint32_t hi, uint32_t *prune)
-{
-    switch (var) {
-    case 0: k_cull<NF, 0><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 1: k_cull<NF, 1><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 2: k_cull<NF, 2><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 3: k_cull<NF, 3><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 32: k_cull<NF, 32><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    default: k_cull<NF, 34><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    }
-}
-
 void launch_cull_range(cudaStream_t s, const NodeArrays &a, const CullParams &cp, const uint32_t *lodp, uint32_t lo, uint32_t hi, uint32_t *prune)
 {
     if (hi <= lo) return;
     const unsigned g = grid_for(hi - lo);
-    const int var = (cull_variant(cp.nf) & 32) ? (32 | (cull_variant(cp.nf) & 2)) : (cull_variant(cp.nf) & 3);
     switch (cp.nf) {
-    case 1: launch_cull_t<1>(s, g, var, a, cp, lodp, lo, hi, prune); break;
-    case 2: launch_cull_t<2>(s, g, var, a, cp, lodp, lo, hi, prune); break;
-    case 3: launch_cull_t<3>(s, g, var, a, cp, lodp, lo, hi, prune); break;
-    case 4: launch_cull_t<4>(s, g, var, a, cp, lodp, lo, hi, prune); break;
-    case 6: launch_cull_t<6>(s, g, var, a, cp, lodp, lo, hi, prune); break;
-    default: launch_cull_t<0>(s, g, var, a, cp, lodp, lo, hi, prune); break;
+    case 1: k_cull<1><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
+    case 2: k_cull<2><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
+    case 3: k_cull<3><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
+    case 4: k_cull<4><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
+    case 6: k_cull<6><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
+    default: k_cull<0><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
     }
 }
 
@@ -1906,57 +1332,9 @@ static void launch_skin_t(cudaStream_t s, const SkinArrays &sk, const SkinTile *
     else launch_skin_t2<S, LOG2C, MINB, false, PREFETCH>(s, sk, tiles, n_tiles);
 }
 
-template <int S, int LOG2C, int STAGES, int MINB> static void launch_skin_tma_t(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles)
-{
-    constexpr size_t pal = ((size_t)3 * S * (1 << LOG2C) * sizeof(float4) + 127) & ~size_t(127);
-    constexpr size_t smem = pal + (size_t)(kBlock / 32) * STAGES * kVblkBytes + (size_t)(kBlock / 32) * STAGES * 8;
-    static bool init = false;
-    if (!init) {
-        cudaFuncSetAttribute(k_skin_tma<S, LOG2C, STAGES, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        init = true;
-    }
-    launch_pdl(k_skin_tma<S, LOG2C, STAGES, MINB>, n_tiles, kBlock, smem, s, sk, tiles, n_tiles, 1.0f, -0.0f);
-}
-
-template <int S, int LOG2C, int MINB> static void launch_skin2_t(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles)
-{
-    constexpr size_t smem_pal = (size_t)3 * S * (1 << LOG2C) * sizeof(float4);
-    static bool init = false;
-    if (!init) {
-        cudaFuncSetAttribute(k_skin2<S, LOG2C, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_pal);
-        init = true;
-    }
-    launch_pdl(k_skin2<S, LOG2C, MINB>, n_tiles, kBlock, smem_pal, s, sk, tiles, n_tiles, 1.0f, -0.0f);
-}
-
-// 0 = LDG straight into registers (default), 2 = TMA bulk ring (2 stages, 4 palette copies, 2 CTAs/SM), 3 = (3 stages, 8 copies, 1 CTA/SM)
-static int skin_variant()
-{
-    static int v = [] {
-        const char *e = getenv("FYX_SKIN_VARIANT");
-        if (!e || !*e) return 0;
-        if (!strcmp(e, "tma2")) return 2;
-        if (!strcmp(e, "tma3")) return 3;
-        if (!strcmp(e, "pair4")) return 14; // two vertices per thread, compiled for 4 / 5 / 6 CTAs per SM
-        if (!strcmp(e, "pair5")) return 15;
-        if (!strcmp(e, "pair6")) return 16;
-        return 0;
-    }();
-    return v;
-}
-
 void launch_skin(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, uint32_t n_tiles, uint32_t max_bones, bool blend_shapes)
 {
     if (!n_tiles) return;
-    const int var = skin_variant();
-    if (var && max_bones <= 64 && !blend_shapes) { // the experiments cover the benchmarked palette size
-        if (var == 2) launch_skin_tma_t<65, 2, 2, 2>(s, sk, tiles, n_tiles);
-        else if (var == 3) launch_skin_tma_t<65, 3, 3, 1>(s, sk, tiles, n_tiles);
-        else if (var == 14) launch_skin2_t<65, 3, 4>(s, sk, tiles, n_tiles);
-        else if (var == 15) launch_skin2_t<65, 3, 5>(s, sk, tiles, n_tiles);
-        else launch_skin2_t<65, 3, 6>(s, sk, tiles, n_tiles);
-        return;
-    }
     // <= 64 bones: the prefetching form, 2 CTAs/SM (<= 128 registers; 25 KB palette + 24 KB output stages + 44 KB ring per CTA).
     // Larger palettes leave no room for the ring at 2 CTAs/SM: loads into registers, 3 CTAs/SM (<= 85 registers).
     if (max_bones <= 64) {       // 8 copies: 25 KB of palette planes

@@ -109,7 +109,6 @@ struct FrustumDev {
     // mask of the corners that have it
     float4 ax_val[3][2];
     uint32_t ax_mask[3][8]; // per distinct coordinate: the 8-bit mask of the frustum corners that have it
-    float4 corner[8];       // the corners themselves (frustum.rs:70-79 order), for the warp-level pre-reject
     // pm[q] = for planes (2q, 2q+1): the smallest s = ((nx*cx + ny*cy) + nz*cz) + d over the frustum's OWN eight corners,
     // evaluated on the host in exactly the kernels' arithmetic (NaN if any of them is NaN).  A box whose max-corner s on a
     // plane is below it cannot contain a frustum corner (see frustum_intersects_aabb): the fallback is skipped.

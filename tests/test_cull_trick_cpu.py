@@ -107,67 +107,6 @@ def test_corner_in_box_through_distinct_coordinate_masks():
         assert np.array_equal(alive != 0, want), trial
 
 
-def test_warp_union_pre_reject_never_hides_a_visible_box():
-    """The multi-frustum kernels first test the UNION of a warp's 32 boxes against every frustum (fyx_kernels.cu,
-    warp_live_frusta): a frustum is skipped for the whole warp iff some plane rejects the union's max-corner AND no frustum
-    corner lies inside the union.  Claim: then the reference predicate (8-corner cloud loop, then corner-in-box) is false for
-    every box of the warp.  Checked in numpy float32 on clustered warps placed around random / adversarial frusta — boxes that
-    touch planes, degenerate boxes, zeros of both signs, bounds equal to corner coordinates."""
-    rng = np.random.default_rng(99)
-    warps, W = 20000, 32
-    skipped = visible_total = 0
-    with np.errstate(over="ignore", under="ignore", invalid="ignore"):
-        for trial in range(12):
-            special = trial >= 8
-            # a "frustum": 6 planes + 8 corners (any planes / corners do: the claim does not depend on them being consistent)
-            if special:
-                n = special_values(rng, 18).reshape(6, 3)
-                d = special_values(rng, 6)
-                corners = special_values(rng, 24).reshape(8, 3)
-            else:
-                n = rng.normal(size=(6, 3)).astype(f32)
-                n /= np.linalg.norm(n, axis=1, keepdims=True).astype(f32)
-                d = (rng.normal(size=6) * 30).astype(f32)
-                corners = (rng.normal(size=(8, 3)) * 40).astype(f32)
-            centre = (rng.normal(size=(warps, 1, 3)) * 40).astype(f32)
-            a = centre + (rng.normal(size=(warps, W, 3)) * 4).astype(f32)
-            b = a + np.abs(rng.normal(size=(warps, W, 3)) * 2).astype(f32) * (rng.random((warps, W, 3)) > 0.1)  # some degenerate axes
-            if special:
-                sv = special_values(rng, warps * W * 3).reshape(warps, W, 3)
-                snap = rng.random((warps, W, 3)) < 0.3
-                a = np.where(snap, sv, a)
-                snap2 = rng.random((warps, W, 3)) < 0.2
-                b = np.where(snap2, corners[rng.integers(0, 8, (warps, W)), :], b)
-            lo, hi = np.minimum(a, b), np.maximum(a, b)
-            part = rng.random((warps, W)) < 0.9  # lanes that take part in the union (culling on, tame)
-            part[:, 0] = True
-            ulo = np.where(part[..., None], lo, np.inf).min(axis=1)
-            uhi = np.where(part[..., None], hi, -np.inf).max(axis=1)
-            # union: max-corner per plane, corner-in-union
-            cloud_fail = np.zeros(warps, bool)
-            for p in range(6):
-                npl = np.broadcast_to(n[p], (warps, 3))
-                cloud_fail |= trick_all_behind(npl, np.full(warps, d[p], f32), ulo, uhi)
-            corner_in = np.zeros(warps, bool)
-            for c in range(8):
-                corner_in |= ((corners[c] >= ulo) & (corners[c] <= uhi)).all(1)
-            dead = cloud_fail & ~corner_in
-            # reference predicate per box
-            L, H = lo.reshape(-1, 3), hi.reshape(-1, 3)
-            cloud = np.ones(len(L), bool)
-            for p in range(6):
-                cloud &= ~literal_all_behind(np.broadcast_to(n[p], (len(L), 3)), np.full(len(L), d[p], f32), L, H)
-            inside = np.zeros(len(L), bool)
-            for c in range(8):
-                inside |= ((corners[c] >= L) & (corners[c] <= H)).all(1)
-            vis = (cloud | inside).reshape(warps, W)
-            bad = dead[:, None] & part & vis
-            assert not bad.any(), (trial, int(bad.sum()))
-            skipped += int(dead.sum())
-            visible_total += int(vis.sum())
-    assert skipped > 10000 and visible_total > 10000  # both outcomes are exercised
-
-
 def test_cube_face_frusta_share_planes_and_what_sharing_would_buy():
     """VERDICT r01 item 4(ii) asked whether plane evaluations can be shared between the frusta of one call.  Facts this test pins
     for the benchmark's six cube-face frusta (camera.cube_frusta): the 24 side planes are 6 unoriented planes — every side

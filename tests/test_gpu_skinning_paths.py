@@ -120,7 +120,7 @@ def test_tile_splits_and_warp_tails(max_bones, blend):
     """Every vertex count around a warp (128 vertices), a 1024-vertex step and the 8192-vertex tile, up to five tiles;
     the order puts tile starts at many offsets mod 32 and mod 128 groups.  With `blend`, every other surface has blend
     shapes, so shape records are read across tile boundaries (local_quad0 != 0), 128 shapes on a two-tile surface
-    (without, the <= 64 launch is also the one the FYX_SKIN_VARIANT forms take over)."""
+    (without, every launch takes the form compiled without blend shapes)."""
     rng = np.random.default_rng(max_bones + blend)
     counts = [COUNTS[i] for i in rng.permutation(len(COUNTS))]
     specs = []

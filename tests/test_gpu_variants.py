@@ -1,6 +1,5 @@
-"""Kernel variants that are selected through the environment when the library first launches them (A/B switches kept for
-measurement: FYX_CULL_VARIANT, FYX_SKIN_VARIANT) get the same bit-exact parity tests as the defaults, each in its own
-process."""
+"""Paths that the environment can force when the library first launches them (FYX_SUBFOREST, FYX_SIDE_FOLD) get the same
+bit-exact parity tests as the defaults, each in its own process."""
 import os
 import subprocess
 import sys
@@ -18,25 +17,6 @@ def _run(env, tests, k):
                        capture_output=True, text=True, env=e, timeout=900)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
     assert " passed" in r.stdout
-
-
-@pytest.mark.timeout(1000)
-@pytest.mark.parametrize("variant", ["0", "3", "13", "20", "34", "52"])
-def test_cull_variants_match_the_oracle(variant):
-    """bit 0: warp-union pre-reject of whole frusta, bit 1: warp-wide compaction, bit 2: FYX_UPDATE_ALL specialisation, bit 3: deferred compaction (k_compact_vis), bit 4: 32-register build, bit 5: warp-convergent predicate
-    (fyx_kernels.cu; the default is 4).  Four variants exercise every bit; the others differ only in combinations."""
-    _run({"FYX_CULL_VARIANT": variant}, ["test_gpu_parity.py", "test_gpu_drawprep.py"],
-         "cull or render_prep or pipelined or k7 or lod or light or instances or bundle")
-
-
-@pytest.mark.timeout(1000)
-@pytest.mark.parametrize("variant", ["tma2", "tma3", "pair5"])  # TMA rings (2 / 3 stages); two vertices per thread
-def test_tma_skinning_variants_match_the_oracle(variant):
-    """k_skin_tma: vertex blocks staged by cp.async.bulk + mbarrier rings; k_skin2: two vertices per thread (fyx_kernels.cu).
-    The variants replace launches of <= 64 bones without blend shapes; test_gpu_skinning_paths.py also runs every other
-    band and the blend-shape launches under the same setting."""
-    _run({"FYX_SKIN_VARIANT": variant}, ["test_gpu_parity.py", "test_gpu_fullsize.py", "test_gpu_skinning_paths.py"],
-         "skin or render_prep or skinning_paths")
 
 
 @pytest.mark.timeout(1000)

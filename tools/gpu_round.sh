@@ -52,7 +52,7 @@ timeout 200 python tools/drawprep_bench.py > $OUT/${TAG}_drawprep.json 2> $OUT/$
 cat $OUT/${TAG}_drawprep.json
 
 if [ "$MODE" != "quick" ]; then
-    K='regex:k_update_level|k_update_subforest|k_compact_vis|k_fold|k_palette|k_skin|k_snapshot|k_cull|k_scatter_trs|k_anim|k_inst|k_lod|k_peer'
+    K='regex:k_update_level|k_update_subforest|k_fold|k_palette|k_skin|k_snapshot|k_cull|k_scatter_trs|k_anim|k_inst|k_lod|k_peer'
     B="--no-c5 --no-parity --no-cpu-baseline --no-device-animation"
     log "ncu launch list of the default bench workload (C4)"
     timeout 400 ncu --metrics gpu__time_duration.sum --clock-control none -k "$K" --csv --log-file $OUT/${TAG}_launches_C4.csv \

@@ -6,7 +6,7 @@ OUT=gpurun_out
 TAG=r02r
 mkdir -p $OUT
 echo "[v14] variant test"; timeout 900 python -m pytest tests/test_gpu_variants.py -m gpu -q -x -k "fold_in_stream" 2>&1 | tail -3
-K='regex:k_update_level|k_update_subforest|k_compact_vis|k_fold|k_palette|k_skin|k_snapshot|k_cull|k_scatter_trs'
+K='regex:k_update_level|k_update_subforest|k_fold|k_palette|k_skin|k_snapshot|k_cull|k_scatter_trs'
 B="--no-c5 --no-parity --no-cpu-baseline --no-device-animation"
 echo "[v14] launch list"
 timeout 400 ncu --metrics gpu__time_duration.sum --clock-control none -k "$K" --csv --log-file $OUT/${TAG}_launches_C4.csv \

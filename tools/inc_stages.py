@@ -2,7 +2,7 @@
 """Stage times (CUDA events of synchronous frames, fyx_get_timings) of the C4 frame in its two update modes, with the changed
 bones uploaded every frame: FYX_UPDATE_ALL (every node recomputed) vs FYX_UPDATE_INCREMENTAL (static + skeletons: only the bones
 change, clean sub-trees keep matrices and boxes, everything is culled again) — and the pipelined end-to-end time of both.
-usage: python tools/inc_stages.py [units]   (FYX_CULL_VARIANT etc. from the environment)"""
+usage: python tools/inc_stages.py [units]"""
 import json
 import os
 import sys
@@ -35,7 +35,7 @@ def main():
         pm.array[:] = full_trs.array[:, 3:7]
         full_trs.free()
         anim.append((pi, pm))
-    out = {"units": units, "variant": os.environ.get("FYX_CULL_VARIANT", "default")}
+    out = {"units": units}
     for name, flags in (("all_dirty", fb.UPDATE_ALL), ("incremental", fb.UPDATE_INCREMENTAL)):
         acc = {}
         n = 12
