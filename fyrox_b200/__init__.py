@@ -7,7 +7,7 @@ the mirror of the reference's host interface (`scene`), and the synthetic scene 
 """
 from . import _lib  # noqa: F401
 from ._lib import (  # noqa: F401
-    FYX_NONE, NODE_ALIVE, NODE_LIGHT, NODE_STATIC_BATCH, NODE_REFLECTION_PROBE, NODE_CAST_SHADOWS, NODE_DEFAULT, NODE_ENABLED, NODE_FRUSTUM_CULLING, NODE_GLOBAL_ENABLED,
+    FYX_NONE, LIGHT_DIRECTIONAL, LIGHT_POINT, LIGHT_SPOT, LIGHT_UNKNOWN, NODE_ALIVE, NODE_LIGHT, NODE_STATIC_BATCH, NODE_REFLECTION_PROBE, NODE_CAST_SHADOWS, NODE_DEFAULT, NODE_ENABLED, NODE_FRUSTUM_CULLING, NODE_GLOBAL_ENABLED,
     NODE_GLOBAL_VISIBILITY, NODE_REACHABLE, NODE_RENDERABLE, NODE_VISIBILITY, PASS_SHADOW, UPDATE_ALL, UPDATE_INCREMENTAL,
 )
 from .context import (  # noqa: F401

@@ -162,6 +162,23 @@ class fyx_instances(C.Structure):
     ]
 
 
+LIGHT_UNKNOWN, LIGHT_SPOT, LIGHT_POINT, LIGHT_DIRECTIONAL = 0, 1, 2, 3
+
+
+class fyx_light_source(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("full_cone_angle", C.c_float), ("distance_or_radius", C.c_float)]
+
+
+class fyx_shadow_settings(C.Structure):
+    _fields_ = [("spot_shadows_distance", C.c_float), ("point_shadows_distance", C.c_float), ("spot_shadows_enabled", C.c_uint32),
+                ("point_shadows_enabled", C.c_uint32)]
+
+
+class fyx_shadow_map(C.Structure):
+    _fields_ = [("light", C.c_uint32), ("face", C.c_uint32), ("cascade", C.c_uint32), ("first", C.c_uint32), ("count", C.c_uint32),
+                ("view_projection", C.c_float * 16)]
+
+
 # every symbol include/fyrox_b200.h declares: name -> (restype, argtypes)
 ctx_p = C.c_void_p
 SYMBOLS = {
@@ -200,6 +217,10 @@ SYMBOLS = {
     "fyx_cull_lights": (C.c_int32, [ctx_p]),
     "fyx_select_reflection_probes": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
     "fyx_get_visible_lights": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(u32p), u32p]),
+    "fyx_set_light_sources": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "fyx_cull_shadow_casters": (C.c_int32, [ctx_p, C.c_uint32, f32p, C.POINTER(fyx_shadow_settings)]),
+    "fyx_get_shadow_maps": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p)]),
+    "fyx_get_shadow_maps_device": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p)]),
     "fyx_build_palettes": (C.c_int32, [ctx_p]),
     "fyx_skin": (C.c_int32, [ctx_p]),
     "fyx_render_prep": (C.c_int32, [ctx_p, C.POINTER(fyx_frame_desc)]),

@@ -329,6 +329,46 @@ class Context:
             return np.empty(0, dtype=np.uint32)
         return np.ctypeslib.as_array(p, shape=(n.value,)).copy()
 
+    # ---- N4 (shadow casters) ----
+    LIGHT_SOURCE_DTYPE = np.dtype([("kind", "<u4"), ("full_cone_angle", "<f4"), ("distance_or_radius", "<f4")])
+    SHADOW_MAP_DTYPE = np.dtype([("light", "<u4"), ("face", "<u4"), ("cascade", "<u4"), ("first", "<u4"), ("count", "<u4"),
+                                 ("view_projection", "<f4", 16)])
+
+    def set_light_sources(self, sources, idx=None):
+        """One record per light node (LIGHT_SOURCE_DTYPE: kind, full_cone_angle, distance_or_radius); kind LIGHT_UNKNOWN removes it."""
+        src = np.ascontiguousarray(sources, dtype=self.LIGHT_SOURCE_DTYPE)
+        ix = _u32(idx)
+        self._chk(self._lib.fyx_set_light_sources(self._h, src.size, _ptr(ix), src.ctypes.data_as(C.c_void_p)))
+
+    def cull_shadow_casters(self, camera_frustum: int, camera_translation, spot_shadows_distance: float = 10.0, point_shadows_distance: float = 10.0,
+                            spot_shadows_enabled: bool = True, point_shadows_enabled: bool = True):
+        """The spot and point shadow maps the deferred light renderer draws for frustum `camera_frustum` of the last cull, and
+        their visible sets (renderer/light.rs:509-606, 695-763).  Defaults are QualitySettings::default() (renderer/settings.rs)."""
+        t = _f32(camera_translation)
+        st = L.fyx_shadow_settings(float(spot_shadows_distance), float(point_shadows_distance), int(bool(spot_shadows_enabled)),
+                                   int(bool(point_shadows_enabled)))
+        self._chk(self._lib.fyx_cull_shadow_casters(self._h, camera_frustum, t.ctypes.data_as(L.f32p), C.byref(st)))
+
+    def get_shadow_maps(self, copy: bool = True):
+        """(maps, entries): maps is a SHADOW_MAP_DTYPE array; map k's visible set is entries[first:first + count].
+        copy=False returns views of the library's pinned buffers, valid until the next cull_shadow_casters."""
+        pm, pe = C.c_void_p(), C.c_void_p()
+        n = C.c_uint32()
+        self._chk(self._lib.fyx_get_shadow_maps(self._h, C.byref(pm), C.byref(n), C.byref(pe)))
+        if not n.value:
+            return np.empty(0, self.SHADOW_MAP_DTYPE), np.empty(0, np.uint32)
+        maps = np.frombuffer((C.c_char * (n.value * self.SHADOW_MAP_DTYPE.itemsize)).from_address(pm.value), self.SHADOW_MAP_DTYPE)
+        total = int(maps["first"][-1]) + int(maps["count"][-1])
+        entries = np.ctypeslib.as_array(C.cast(pe.value, L.u32p), shape=(max(total, 1),))[:total]
+        return (maps.copy(), entries.copy()) if copy else (maps, entries)
+
+    def get_shadow_maps_device(self):
+        """(device pointer of the map table, number of maps, device pointer of the entries)."""
+        pm, pe = C.c_void_p(), C.c_void_p()
+        n = C.c_uint32()
+        self._chk(self._lib.fyx_get_shadow_maps_device(self._h, C.byref(pm), C.byref(n), C.byref(pe)))
+        return pm.value, n.value, pe.value
+
     # ---- N2: animation sampling on the device ----
     KEY_DTYPE = np.dtype([("location", "<f4"), ("value", "<f4"), ("kind", "<u4"), ("left_tangent", "<f4"), ("right_tangent", "<f4")])
     TRACK_DTYPE = np.dtype([("target_node", "<u4"), ("binding", "<u4"), ("value_kind", "<u4"), ("enabled", "<u4"), ("n_curves", "<u4"),

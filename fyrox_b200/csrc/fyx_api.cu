@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 
+#include "fyx_frustum.cuh"
 #include "fyx_hostseg.hpp"
 #include "fyx_internal.h"
 
@@ -217,6 +218,18 @@ struct fyx_ctx {
     uint32_t light_nf = 0;
     bool lights_valid = false;
 
+    // N4 shadow casters (fyx_drawprep.inl): light-source records by node index, their device table by pool order, the maps
+    std::vector<fyx_light_source> light_src; // kind FYX_LIGHT_UNKNOWN = no record
+    std::vector<float> light_m22;
+    bool light_table_dirty = false;
+    uint32_t n_light_table = 0;
+    DevBuf b_light_table, b_sh_scratch, b_sh_frusta, b_sh_maps, b_sh_counts, b_sh_warp_any, b_sh_small, b_sh_entries;
+    uint32_t *h_sh_small = nullptr; // pinned: n_maps, total
+    void *h_sh_maps = nullptr, *h_sh_entries = nullptr;
+    size_t h_sh_maps_cap = 0, h_sh_entries_cap = 0;
+    uint32_t sh_n_maps = 0, sh_total = 0;
+    bool sh_valid = false, sh_on_host = false;
+
     // N3 draw-prep (fyx_drawprep.inl)
     bool instances_enabled = false, have_bundles = false, rank_on_device = false;
     uint32_t n_bundle_ids = 1;
@@ -394,65 +407,6 @@ void rebuild_node_arrays(fyx_ctx *c)
         a.G[i] = c->b_G[i].as<float4>();
         a.la[i] = c->b_la[i].as<float2>();
         a.wa[i] = c->b_wa[i].as<float2>();
-    }
-}
-
-// Frustum → kernel parameter form
-void to_dev_frustum(const fyx_frustum &f, uint32_t cam_mask, uint32_t pass_flags, FrustumDev &d)
-{
-    for (int p = 0; p < 6; ++p) d.plane[p] = make_float4(f.planes[p][0], f.planes[p][1], f.planes[p][2], f.planes[p][3]);
-    for (int q = 0; q < 3; ++q)
-        for (int k = 0; k < 4; ++k) d.pn[q][k] = make_float2(f.planes[2 * q][k], f.planes[2 * q + 1][k]);
-    // distinct corner coordinates per axis (bit-pattern equality, so -0/+0 and NaNs stay separate entries:
-    // each entry is compared exactly like the corner it came from)
-    d.n_ax = 0;
-    for (int k = 0; k < 3; ++k) {
-        int n = 0;
-        uint32_t masks[8] = {0};
-        float vals[8];
-        for (int j = 0; j < 8; ++j) d.ax_mask[k][j] = 0;
-        for (int i = 0; i < 8; ++i) {
-            const float v = f.corners[i][k];
-            uint32_t vb, ub;
-            memcpy(&vb, &v, 4);
-            int j = 0;
-            for (; j < n; ++j) {
-                memcpy(&ub, &vals[j], 4);
-                if (ub == vb) break;
-            }
-            if (j == n) {
-                vals[n] = v;
-                ++n;
-            }
-            masks[j] |= 1u << i;
-        }
-        for (int j = n; j < 8; ++j) vals[j] = std::nanf(""); // never inside any box
-        d.ax_val[k][0] = make_float4(vals[0], vals[1], vals[2], vals[3]);
-        d.ax_val[k][1] = make_float4(vals[4], vals[5], vals[6], vals[7]);
-        for (int j = 0; j < n; ++j) d.ax_mask[k][j] = masks[j];
-        d.n_ax |= (uint32_t)n << (8 * k);
-    }
-    d.cam_mask = cam_mask;
-    d.pass_flags = pass_flags;
-    for (int p = 0; p < 6; ++p)
-        for (int k = 0; k < 3; ++k) d.vsel[p >> 1][k][p & 1] = (f.planes[p][k] < 0.0f) ? 0x3210u : 0x7654u;
-    // smallest plane value over the frustum's own corners, one rounding per operation in the kernels' order (the volatile
-    // temporaries keep the host compiler from contracting anything)
-    for (int p = 0; p < 6; ++p) {
-        float m = std::numeric_limits<float>::infinity();
-        for (int i = 0; i < 8; ++i) {
-            volatile float a = f.planes[p][0] * f.corners[i][0];
-            volatile float b = f.planes[p][1] * f.corners[i][1];
-            volatile float ab = a + b;
-            volatile float e = f.planes[p][2] * f.corners[i][2];
-            volatile float abe = ab + e;
-            volatile float sv = abe + f.planes[p][3];
-            const float v = sv;
-            if (std::isnan(v) || std::isnan(m)) m = std::nanf("");
-            else if (v < m) m = v;
-        }
-        if (p & 1) d.pm[p >> 1].y = m;
-        else d.pm[p >> 1].x = m;
     }
 }
 
@@ -771,59 +725,10 @@ extern "C" uint64_t fyx_kernel_launch_count(const fyx_ctx *c) { return c ? c->la
 // --------------------------------------------------------------------------------------------
 // host-side math (tiny, per frustum).  Built with -ffp-contract=off.
 // --------------------------------------------------------------------------------------------
-namespace {
-inline float h_dot3(const float *u, const float *v) { return (u[0] * v[0] + u[1] * v[1]) + u[2] * v[2]; }
-inline void h_cross(const float *u, const float *v, float *o)
-{
-    o[0] = u[1] * v[2] - u[2] * v[1];
-    o[1] = u[2] * v[0] - u[0] * v[2];
-    o[2] = u[0] * v[1] - u[1] * v[0];
-}
-// Plane::from_abcd — fyrox-math/src/plane.rs:63-75
-bool h_plane(float a, float b, float c_, float d, float *out)
-{
-    const float n[3] = {a, b, c_};
-    const float len = std::sqrt(h_dot3(n, n));
-    if (len == 0.0f) return false;
-    const float coeff = 1.0f / len;
-    out[0] = a * coeff;
-    out[1] = b * coeff;
-    out[2] = c_ * coeff;
-    out[3] = d * coeff;
-    return true;
-}
-// Plane::intersection_point — plane.rs:94-102
-void h_isect(const float *a, const float *b, const float *c_, float *out)
-{
-    float bc[3], ca[3], ab[3];
-    h_cross(b, c_, bc);
-    const float f = -1.0f / h_dot3(a, bc);
-    h_cross(c_, a, ca);
-    h_cross(a, b, ab);
-    for (int i = 0; i < 3; ++i) out[i] = ((bc[i] * a[3] + ca[i] * b[3]) + ab[i] * c_[3]) * f;
-}
-} // namespace
-
 extern "C" int32_t fyx_frustum_from_view_projection_matrix(const float m[16], fyx_frustum *out)
 {
     if (!m || !out) return FYX_ERR_INVALID_ARGUMENT;
-    float(*p)[4] = out->planes; // frustum.rs:55-68; m[] is nalgebra's linear (column-major) index
-    if (!h_plane(m[3] + m[0], m[7] + m[4], m[11] + m[8], m[15] + m[12], p[0])) return FYX_ERR_INVALID_ARGUMENT;
-    if (!h_plane(m[3] - m[0], m[7] - m[4], m[11] - m[8], m[15] - m[12], p[1])) return FYX_ERR_INVALID_ARGUMENT;
-    if (!h_plane(m[3] - m[1], m[7] - m[5], m[11] - m[9], m[15] - m[13], p[2])) return FYX_ERR_INVALID_ARGUMENT;
-    if (!h_plane(m[3] + m[1], m[7] + m[5], m[11] + m[9], m[15] + m[13], p[3])) return FYX_ERR_INVALID_ARGUMENT;
-    if (!h_plane(m[3] - m[2], m[7] - m[6], m[11] - m[10], m[15] - m[14], p[4])) return FYX_ERR_INVALID_ARGUMENT;
-    if (!h_plane(m[3] + m[2], m[7] + m[6], m[11] + m[10], m[15] + m[14], p[5])) return FYX_ERR_INVALID_ARGUMENT;
-    enum { L = 0, R = 1, T = 2, B = 3, F = 4, N = 5 }; // frustum.rs:70-79
-    h_isect(p[L], p[T], p[F], out->corners[0]);
-    h_isect(p[L], p[B], p[F], out->corners[1]);
-    h_isect(p[R], p[B], p[F], out->corners[2]);
-    h_isect(p[R], p[T], p[F], out->corners[3]);
-    h_isect(p[L], p[T], p[N], out->corners[4]);
-    h_isect(p[L], p[B], p[N], out->corners[5]);
-    h_isect(p[R], p[B], p[N], out->corners[6]);
-    h_isect(p[R], p[T], p[N], out->corners[7]);
-    return FYX_OK;
+    return frustum_from_view_projection(m, *out) ? FYX_OK : FYX_ERR_INVALID_ARGUMENT;
 }
 
 extern "C" void fyx_frustum_default(fyx_frustum *out)
@@ -840,19 +745,7 @@ extern "C" void fyx_frustum_default(fyx_frustum *out)
     fyx_frustum_from_view_projection_matrix(m, out);
 }
 
-extern "C" void fyx_mat4_mul(const float a[16], const float b[16], float out[16])
-{
-    float r[16];
-    for (int j = 0; j < 4; ++j)
-        for (int i = 0; i < 4; ++i) {
-            float y = a[i] * b[j * 4];
-            y = y + a[4 + i] * b[j * 4 + 1];
-            y = y + a[8 + i] * b[j * 4 + 2];
-            y = y + a[12 + i] * b[j * 4 + 3];
-            r[j * 4 + i] = y;
-        }
-    memcpy(out, r, sizeof r);
-}
+extern "C" void fyx_mat4_mul(const float a[16], const float b[16], float out[16]) { mat4_mul(a, b, out); }
 
 // --------------------------------------------------------------------------------------------
 // scene description
@@ -1081,6 +974,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
         }
         dev_free(b_map);
     }
+    c->light_table_dirty = true; // the light-source records stay with their node indices; their slots are looked up again
     if ((rc = dev_ensure(c, c->b_parent, n * 4))) return rc;
     if ((rc = dev_ensure(c, c->b_flags, n * 4))) return rc;
     if ((rc = dev_ensure(c, c->b_mask, n * 4))) return rc;

@@ -183,6 +183,36 @@ struct LodParams {
 void launch_lod_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, const float2 *range, uint32_t *lodp, const LodParams &lp);
 void launch_select_probes(cudaStream_t s, const NodeArrays &a, const LodParams &obs, uint32_t *best /* [nf], cleared to 0 by the caller: node index + 1 */);
 void launch_cull_lights(cudaStream_t s, const NodeArrays &a, const CullParams &cp, uint32_t *const *d_out_ptrs, uint32_t *counts);
+
+// N4 shadow casters (fyx_cull_shadow_casters): one record per light node, in pool order
+struct ShadowLightDev {
+    uint32_t slot;
+    uint32_t kind; // FYX_LIGHT_*
+    float m22;     // 1 / tan(fovy / 2), evaluated on the host
+    float distance_or_radius;
+};
+struct ShadowParams {
+    const ShadowLightDev *lights;
+    uint32_t n_lights;
+    FrustumDev cam;      // the camera frustum of the last cull (planes + cam_mask)
+    FrustumDev fallback; // Frustum::default(): from_view_projection_matrix(..).unwrap_or_default() (renderer/bundle.rs:893-896)
+    float cam_t[3];
+    float spot_distance, point_distance;
+    uint32_t spot_enabled, point_enabled;
+    const fyx_trs *trs; // the node's last TRS record per slot; nullptr = none sent (identity scale)
+    // outputs of pass 1 (map table), read by the node pass
+    fyx_frustum *scratch; // [max maps] the map frusta as planes + corners
+    FrustumDev *frusta;   // [max maps]
+    fyx_shadow_map *maps; // [max maps]
+    uint32_t *n_maps;     // one u32
+    // node pass: per-map counts (each on its own 128 B line), then the lists
+    uint32_t *counts;     // [max maps * kCountStride]
+    uint32_t *warp_any;   // [warps]: the warp's nodes are in at least one map (written by the count pass, read by the emit pass)
+    uint32_t *total;      // one u32: entries of all maps
+    uint32_t *entries;    // [total], sized by the host from the count pass
+};
+void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp); // map table + frusta, count pass, scan
+void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);
 void launch_fold_bones(cudaStream_t s, const NodeArrays &a, const FoldArrays &fa, const CullParams *cull);
 void launch_snapshot_bones(cudaStream_t s, const NodeArrays &a, uint32_t n_late, const uint32_t *late_slot, float4 *stale_pos);
 void launch_palette(cudaStream_t s, const NodeArrays &a, const SkinArrays &sk);

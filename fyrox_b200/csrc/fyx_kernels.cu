@@ -5,6 +5,7 @@
 // Each kernel names the reference code it replaces (paths relative to the Fyrox tree).
 #include <cuda_fp16.h>
 
+#include "fyx_frustum.cuh"
 #include "fyx_internal.h"
 #include "fyx_trs.cuh"
 
@@ -1461,6 +1462,278 @@ void launch_compact_gathered(cudaStream_t s, const uint32_t *pad, uint32_t maxc,
 {
     if (!maxc || nranks <= 0) return;
     k_compact_gathered<<<grid_for((uint64_t)maxc * nranks), kBlock, 0, s>>>(pad, maxc, counts_all, nranks, f, dst);
+}
+
+// ------------------------------------------------------------------------------------------------
+// N4 shadow casters (fyx_cull_shadow_casters): the shadow-map loop of the deferred light renderer (renderer/light.rs:509-606,
+// 695-763) and, for every map, the cull of RenderDataBundleStorage::from_graph in its shadow pass (renderer/shadow/spot.rs:142,
+// shadow/point.rs:162-180).  Pass 1 (one CTA) builds the map table; pass 2 reads every node once and counts its entries in
+// every map; a one-CTA scan places the lists; pass 3 re-tests the warps that had an entry and writes the lists.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kShadowNeed = kNeedBits | FYX_NODE_CAST_SHADOWS;
+
+// Vector3::try_normalize(f32::EPSILON).unwrap_or(fallback): norm <= eps ⇒ the fallback, else each component / norm
+__device__ __forceinline__ void try_normalize(const float *v, const float *fallback, float *out)
+{
+    const float n = sqrtf(dot3(v, v));
+    if (n <= 1.1920929e-07f) {
+        out[0] = fallback[0]; out[1] = fallback[1]; out[2] = fallback[2];
+    } else {
+        out[0] = v[0] / n; out[1] = v[1] / n; out[2] = v[2] / n;
+    }
+}
+
+// renderer/utils.rs:49-75, CubeMapFaceDescriptor::cube_faces(): look and up of the six faces
+__constant__ float c_face_look[6][3] = {{1.f, 0.f, 0.f}, {-1.f, 0.f, 0.f}, {0.f, 1.f, 0.f}, {0.f, -1.f, 0.f}, {0.f, 0.f, 1.f}, {0.f, 0.f, -1.f}};
+__constant__ float c_face_up[6][3] = {{0.f, -1.f, 0.f}, {0.f, -1.f, 0.f}, {0.f, 0.f, 1.f}, {0.f, 0.f, -1.f}, {0.f, -1.f, 0.f}, {0.f, -1.f, 0.f}};
+
+// one map: view_projection = P · V, its frustum (Frustum::default if the matrix has none, renderer/bundle.rs:893-896)
+__device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uint32_t m, const uint32_t light, const uint32_t face, const uint32_t cascade,
+                               const float *P, const float *eye, const float *target, const float *up)
+{
+    float V[16], VP[16];
+    look_at_rh(eye, target, up, V);
+    mat4_mul(P, V, VP);
+    fyx_shadow_map &o = sp.maps[m];
+    o.light = light;
+    o.face = face;
+    o.cascade = cascade;
+    o.first = 0u;
+    o.count = 0u;
+    for (int k = 0; k < 16; ++k) o.view_projection[k] = VP[k];
+    if (frustum_from_view_projection(VP, sp.scratch[m])) to_dev_frustum(sp.scratch[m], sp.cam.cam_mask, FYX_PASS_SHADOW, sp.frusta[m]);
+    else sp.frusta[m] = sp.fallback;
+}
+
+__global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, const ShadowParams sp)
+{
+    __shared__ uint32_t s_warp[kBlock / 32];
+    __shared__ uint32_t s_base;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    pdl_trigger(); // the node pass loads its columns meanwhile
+    if (tid == 0) s_base = 0u;
+    PackedConsts kc;
+    kc.one = make_float2(1.0f, 1.0f);
+    kc.negzero = make_float2(-0.0f, -0.0f);
+    for (uint32_t base = 0; base < sp.n_lights; base += kBlock) {
+        const uint32_t i = base + tid;
+        uint32_t n_maps = 0u, cascade = 0u, slot = 0u, kind = FYX_LIGHT_UNKNOWN;
+        float pos[3] = {0.f, 0.f, 0.f}, upv[3] = {0.f, 0.f, 0.f}, lookv[3] = {0.f, 0.f, 0.f}, radius = 0.f, m22 = 0.f;
+        if (i < sp.n_lights) {
+            const ShadowLightDev L = sp.lights[i];
+            slot = L.slot;
+            kind = L.kind;
+            m22 = L.m22;
+            const uint32_t nf = a.flags[slot];
+            // in the camera's light list (renderer/bundle.rs:926-974, as k_cull_lights)
+            constexpr uint32_t need = FYX_NODE_ALIVE | FYX_NODE_LIGHT | FYX_NODE_GLOBAL_VISIBILITY | FYX_NODE_GLOBAL_ENABLED;
+            bool ok = (nf & need) == need && (kind == FYX_LIGHT_SPOT || kind == FYX_LIGHT_POINT);
+            if (ok) {
+                const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
+                ok = frustum_intersects_aabb(sp.cam, wx, wy, wz, kc, aabb_is_tame(wx, wy, wz));
+            }
+            if (ok) {
+                const float4 r0 = a.G[0][slot], r1 = a.G[1][slot], r2 = a.G[2][slot];
+                pos[0] = r0.w; pos[1] = r1.w; pos[2] = r2.w;    // global_position
+                upv[0] = r0.y; upv[1] = r1.y; upv[2] = r2.y;    // up_vector: column 1
+                lookv[0] = r0.z; lookv[1] = r1.z; lookv[2] = r2.z; // look_vector: column 2
+                // light.rs:510: (light.position - observer.position.translation).norm()
+                const float d[3] = {FYX_SUB(pos[0], sp.cam_t[0]), FYX_SUB(pos[1], sp.cam_t[1]), FYX_SUB(pos[2], sp.cam_t[2])};
+                const float dist = sqrtf(dot3(d, d));
+                const bool spot = kind == FYX_LIGHT_SPOT;
+                const float sd = spot ? sp.spot_distance : sp.point_distance;
+                // light.rs:529-532, 547-549: cast_shadows && distance_to_camera <= shadows_distance && enabled
+                ok = (nf & FYX_NODE_CAST_SHADOWS) && dist <= sd && (spot ? sp.spot_enabled : sp.point_enabled);
+                // light.rs:570-572: max(local scale) * raw radius
+                float sx = 1.f, sy = 1.f, sz = 1.f;
+                if (sp.trs) {
+                    sx = sp.trs[slot].scale[0];
+                    sy = sp.trs[slot].scale[1];
+                    sz = sp.trs[slot].scale[2];
+                }
+                radius = FYX_MUL(fmaxf(fmaxf(sx, sy), sz), L.distance_or_radius);
+                // light.rs:585-587, Frustum::is_intersects_sphere (fyrox-math/src/frustum.rs:336-347)
+                bool sphere = true;
+                for (int p = 0; p < 6; ++p) {
+                    const float4 pl = sp.cam.plane[p];
+                    const float n[3] = {pl.x, pl.y, pl.z};
+                    const float dd = FYX_ADD(dot3(n, pos), pl.w);
+                    if (dd < -radius) { sphere = false; break; }
+                    if (fabsf(dd) < radius) break;
+                }
+                ok = ok && sphere;
+                // light.rs:589-602 (a distance equal to b1 is neither < b1 nor > b1: cascade 2)
+                const float b1 = FYX_MUL(sd, 0.2f), b2 = FYX_MUL(sd, 0.4f);
+                const float e[3] = {FYX_SUB(sp.cam_t[0], pos[0]), FYX_SUB(sp.cam_t[1], pos[1]), FYX_SUB(sp.cam_t[2], pos[2])};
+                const float metric = sqrtf(dot3(e, e));
+                cascade = (dist < b1 || metric <= radius) ? 0u : (dist > b1 && dist < b2) ? 1u : 2u;
+                n_maps = ok ? (spot ? 1u : 6u) : 0u;
+            }
+        }
+        // ordered compaction: maps in light (pool) order
+        uint32_t incl = n_maps;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= (uint32_t)o) incl += v;
+        }
+        if (lane == 31u) s_warp[warp] = incl;
+        __syncthreads();
+        uint32_t first = s_base + incl - n_maps;
+        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
+        if (n_maps) {
+            const uint32_t light = a.gidx[slot];
+            float P[16];
+            perspective_square(m22, 0.01f, radius, P); // z_near 0.01, z_far light_radius (light.rs:702-704, point.rs:167-170)
+            if (kind == FYX_LIGHT_SPOT) {
+                // light.rs:706-722: look_at_rh(pos, pos - emit_direction, look_vector normalised)
+                const float zdir[3] = {0.f, 0.f, 1.f}, ydir[3] = {0.f, 1.f, 0.f};
+                float emit[3], up[3];
+                try_normalize(upv, zdir, emit);
+                try_normalize(lookv, ydir, up);
+                const float target[3] = {FYX_SUB(pos[0], emit[0]), FYX_SUB(pos[1], emit[1]), FYX_SUB(pos[2], emit[2])};
+                shadow_map_out(sp, first, light, 0u, cascade, P, pos, target, up);
+            } else {
+                // shadow/point.rs:172-180: one map per cube face
+#pragma unroll 1
+                for (uint32_t k = 0; k < 6u; ++k) {
+                    const float target[3] = {FYX_ADD(pos[0], c_face_look[k][0]), FYX_ADD(pos[1], c_face_look[k][1]), FYX_ADD(pos[2], c_face_look[k][2])};
+                    const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
+                    shadow_map_out(sp, first + k, light, k, cascade, P, pos, target, up);
+                }
+            }
+        }
+        __syncthreads();
+        if (tid == kBlock - 1) s_base = first + n_maps;
+        __syncthreads();
+    }
+    if (tid == 0) *sp.n_maps = s_base;
+}
+
+// the node's part of from_graph for a shadow map, minus the frustum test: alive, renderable, reachable, globally visible and
+// enabled, cast_shadows, render mask against the camera's (every map carries the camera's mask)
+__device__ __forceinline__ bool shadow_candidate(const uint32_t nf, const uint32_t mask, const ShadowParams &sp)
+{
+    return (nf & kShadowNeed) == kShadowNeed && (mask & sp.cam.cam_mask) != 0u;
+}
+
+// pass 2: every node read once (flags, mask, box: 32 B) and tested against every map; one atomic per (warp, map) with an entry
+__global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, const ShadowParams sp)
+{
+    const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
+    const bool valid = slot < a.cap;
+    uint32_t nf = 0u, mask = 0u;
+    float2 wx = make_float2(0.f, 0.f), wy = wx, wz = wx;
+    if (valid) {
+        nf = a.flags[slot];
+        mask = a.mask[slot];
+        wx = ld_stream(a.wa[0] + slot);
+        wy = ld_stream(a.wa[1] + slot);
+        wz = ld_stream(a.wa[2] + slot);
+    }
+    pdl_trigger();
+    pdl_wait(); // the map table
+    const bool cand = valid && shadow_candidate(nf, mask, sp);
+    uint32_t any = 0u;
+    if (__any_sync(0xFFFFFFFFu, cand)) {
+        PackedConsts kc;
+        kc.one = make_float2(1.0f, 1.0f);
+        kc.negzero = make_float2(-0.0f, -0.0f);
+        const bool tame = cand && aabb_is_tame(wx, wy, wz);
+        const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
+        const FrustumDev *__restrict__ F = sp.frusta;
+        const uint32_t n_maps = *sp.n_maps;
+        for (uint32_t m = 0; m < n_maps; ++m) {
+            const bool ok = test ? frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame) : cand;
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
+            if (b && lane == 0u) atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
+            any |= b;
+        }
+    }
+    if (lane == 0u) sp.warp_any[slot >> 5] = any;
+}
+
+// the lists' places: maps[m].first / count, counts[m] becomes map m's write cursor, total = all entries
+__global__ void __launch_bounds__(1024) k_shadow_scan(const ShadowParams sp)
+{
+    __shared__ uint32_t s_warp[32];
+    __shared__ uint32_t s_base;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    pdl_wait();
+    if (tid == 0) s_base = 0u;
+    const uint32_t n = *sp.n_maps;
+    for (uint32_t base = 0; base < n; base += 1024u) {
+        const uint32_t m = base + tid;
+        const uint32_t c = m < n ? sp.counts[(size_t)m * kCountStride] : 0u;
+        uint32_t incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= (uint32_t)o) incl += v;
+        }
+        if (lane == 31u) s_warp[warp] = incl;
+        __syncthreads();
+        uint32_t first = s_base + incl - c;
+        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
+        if (m < n) {
+            sp.maps[m].first = first;
+            sp.maps[m].count = c;
+            sp.counts[(size_t)m * kCountStride] = first;
+        }
+        __syncthreads();
+        if (tid == 1023u) s_base = first + c;
+        __syncthreads();
+    }
+    if (tid == 0) *sp.total = s_base;
+}
+
+// pass 3: the warps that had an entry test again and write their node indices
+__global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const ShadowParams sp)
+{
+    const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
+    pdl_wait();
+    if (!sp.warp_any[slot >> 5]) return; // warp-uniform
+    const bool valid = slot < a.cap;
+    uint32_t nf = 0u, mask = 0u, gi = 0u;
+    float2 wx = make_float2(0.f, 0.f), wy = wx, wz = wx;
+    if (valid) {
+        nf = a.flags[slot];
+        mask = a.mask[slot];
+        wx = ld_stream(a.wa[0] + slot);
+        wy = ld_stream(a.wa[1] + slot);
+        wz = ld_stream(a.wa[2] + slot);
+        gi = a.gidx[slot];
+    }
+    const bool cand = valid && shadow_candidate(nf, mask, sp);
+    PackedConsts kc;
+    kc.one = make_float2(1.0f, 1.0f);
+    kc.negzero = make_float2(-0.0f, -0.0f);
+    const bool tame = cand && aabb_is_tame(wx, wy, wz);
+    const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
+    const FrustumDev *__restrict__ F = sp.frusta;
+    const uint32_t n_maps = *sp.n_maps;
+    const uint32_t lt = (1u << lane) - 1u;
+    for (uint32_t m = 0; m < n_maps; ++m) {
+        const bool ok = test ? frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame) : cand;
+        const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
+        if (!b) continue;
+        uint32_t at = 0u;
+        if (lane == 0u) at = atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
+        at = __shfl_sync(0xFFFFFFFFu, at, 0);
+        if (ok) sp.entries[at + __popc(b & lt)] = gi;
+    }
+}
+
+void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
+{
+    k_shadow_frusta<<<1, kBlock, 0, s>>>(a, sp);
+    if (a.cap) launch_pdl(k_shadow_count, grid_for(a.cap), kBlock, 0, s, a, sp);
+    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
+}
+
+void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
+{
+    if (a.cap) launch_pdl(k_shadow_emit, grid_for(a.cap), kBlock, 0, s, a, sp);
 }
 
 } // namespace fyx

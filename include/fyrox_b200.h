@@ -241,6 +241,62 @@ int32_t fyx_cull_lights(fyx_ctx *ctx);
 int32_t fyx_select_reflection_probes(fyx_ctx *ctx, uint32_t count, uint32_t *out_probe);
 int32_t fyx_get_visible_lights(fyx_ctx *ctx, uint32_t frustum, const uint32_t **out_idx, uint32_t *out_count);
 
+/* N4 (shadow casters) — the shadow-map loop of the deferred light renderer (renderer/light.rs:509-606, 695-763) with the
+ * per-map cull of the spot and point shadow renderers (renderer/shadow/spot.rs:142, shadow/point.rs:162-180), on the device.
+ *
+ * fyx_set_light_sources: the LightSource data of `count` light nodes (idx NULL = nodes 0..count-1) that the world
+ * transform does not give: kind, SpotLight::full_cone_angle (spot only) and SpotLight::distance / PointLight::radius.
+ * FYX_LIGHT_UNKNOWN removes the node's record.  Carried over by fyx_set_topology with the node indices.  The projection's
+ * one transcendental, m22 = 1 / tan(fovy / 2) (fovy = full_cone_angle, or FRAC_PI_2 for a point light), is evaluated here
+ * with the platform's tanf; everything the device does with the record is + − × ÷ √.
+ *
+ * fyx_cull_shadow_casters: takes frustum `camera_frustum` of the most recent cull as the camera (its planes and its
+ * cam_mask = observer.render_mask) and `camera_translation` as observer.position.translation, and produces every shadow
+ * map the reference renders for that camera, in its order: lights in pool order, 1 map per spot light, 6 per point
+ * light in CubeMapFaceDescriptor::cube_faces() order.  A light gets maps only when it is in the camera's light list
+ * (fyx_cull_lights' rule), its node has FYX_NODE_CAST_SHADOWS, distance_to_camera <= {spot,point}_shadows_distance,
+ * shadows are enabled for its kind, and the camera frustum intersects the sphere (position, light_radius), light_radius =
+ * max(local scale) * distance_or_radius with the scale of the node's last TRS record (identity without one).  Each map
+ * gets the cascade index of light.rs:592-606, view_projection = P · V (spot: look_at_rh(pos, pos − up, look); point:
+ * look_at_rh(pos, pos + face.look, face.up); z_near 0.01, z_far light_radius) and the visible set of
+ * from_graph(map frustum, cam_mask, shadow pass): alive, renderable, reachable, should_be_rendered and cast_shadows.
+ * One pass over the nodes tests every map; list memory grows with the visible entries.  Synchronous.
+ * Not modelled: directional lights and cascaded shadow maps (shadow/csm.rs: they need the camera's projection and the
+ * frame size — cull those frusta with fyx_cull and FYX_PASS_SHADOW), light occlusion queries
+ * (use_light_occlusion_culling = false), shadow alpha and other shading-only values, instance packing of the lists.
+ * Returns FYX_ERR_STATE when no cull has been made, a frame is still in flight, LOD ranges with observers are active or a
+ * node carries FYX_NODE_STATIC_BATCH (the per-map LOD filter and static-batch pruning are not modelled: the call refuses
+ * rather than give a different set), or the context is sharded (fyx_comm_init); FYX_ERR_INVALID_ARGUMENT when
+ * camera_frustum is not a frustum of the last cull. */
+#define FYX_LIGHT_UNKNOWN 0u
+#define FYX_LIGHT_SPOT 1u
+#define FYX_LIGHT_POINT 2u
+#define FYX_LIGHT_DIRECTIONAL 3u
+typedef struct fyx_light_source {
+    uint32_t kind;             /* FYX_LIGHT_* */
+    float full_cone_angle;     /* radians, spot lights only */
+    float distance_or_radius;  /* SpotLight::distance or PointLight::radius */
+} fyx_light_source;
+typedef struct fyx_shadow_settings { /* QualitySettings, renderer/settings.rs:112-191 */
+    float spot_shadows_distance;
+    float point_shadows_distance;
+    uint32_t spot_shadows_enabled;
+    uint32_t point_shadows_enabled;
+} fyx_shadow_settings;
+typedef struct fyx_shadow_map {
+    uint32_t light;            /* light node index */
+    uint32_t face;             /* 0 for a spot light, the cube face 0..5 for a point light */
+    uint32_t cascade;          /* 0, 1 or 2 */
+    uint32_t first, count;     /* the map's visible list is entries[first, first + count), order unspecified */
+    float view_projection[16]; /* column-major */
+} fyx_shadow_map;
+int32_t fyx_set_light_sources(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const fyx_light_source *src);
+int32_t fyx_cull_shadow_casters(fyx_ctx *ctx, uint32_t camera_frustum, const float camera_translation[3], const fyx_shadow_settings *settings);
+/* Result of the last fyx_cull_shadow_casters: pinned host copies ... */
+int32_t fyx_get_shadow_maps(fyx_ctx *ctx, const fyx_shadow_map **out_maps, uint32_t *out_n_maps, const uint32_t **out_entries);
+/* ... or the device arrays (*out_n_maps is a host value). */
+int32_t fyx_get_shadow_maps_device(fyx_ctx *ctx, const fyx_shadow_map **d_maps, uint32_t *out_n_maps, const uint32_t **d_entries);
+
 /* N4 (LOD filter) — the lod_filter of RenderDataBundleStorage::from_graph (renderer/bundle.rs:898-916, 988-1004): a node
  * that is an object of a LOD level is visible for an observer only while its normalised distance
  * (|observer.translation − global_position| − z_near) / (z_far − z_near) lies in the level's [begin, end]; a node that is
