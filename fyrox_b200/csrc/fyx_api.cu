@@ -7,8 +7,10 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "fyx_frustum.cuh"
@@ -24,10 +26,127 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// Owners of the context's CUDA resources.  Each is move-only and frees what it holds when it dies; a move assignment swaps,
+// so what the target held before dies with the moved-from source.  A failed allocation leaves the owner as it was.
 struct DevBuf {
     void *p = nullptr;
     size_t bytes = 0;
+    DevBuf() = default;
+    DevBuf(DevBuf &&o) noexcept { *this = std::move(o); }
+    DevBuf &operator=(DevBuf &&o) noexcept
+    {
+        std::swap(p, o.p);
+        std::swap(bytes, o.bytes);
+        return *this;
+    }
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf()
+    {
+        if (p) cudaFree(p);
+    }
+    cudaError_t alloc(size_t n)
+    {
+        DevBuf fresh;
+        const cudaError_t e = cudaMalloc(&fresh.p, n);
+        if (e != cudaSuccess) {
+            fresh.p = nullptr;
+            return e;
+        }
+        fresh.bytes = n;
+        *this = std::move(fresh);
+        return cudaSuccess;
+    }
     template <class T> T *as() const { return static_cast<T *>(p); }
+};
+
+// page-locked host memory
+struct PinnedBuf {
+    void *p = nullptr;
+    size_t bytes = 0;
+    PinnedBuf() = default;
+    PinnedBuf(PinnedBuf &&o) noexcept { *this = std::move(o); }
+    PinnedBuf &operator=(PinnedBuf &&o) noexcept
+    {
+        std::swap(p, o.p);
+        std::swap(bytes, o.bytes);
+        return *this;
+    }
+    PinnedBuf(const PinnedBuf &) = delete;
+    PinnedBuf &operator=(const PinnedBuf &) = delete;
+    ~PinnedBuf()
+    {
+        if (p) cudaFreeHost(p);
+    }
+    // at least n bytes; the contents are not kept.  The old buffer is freed first, so the caller must know that no copy
+    // still uses it.  On failure the buffer is empty.
+    cudaError_t ensure(size_t n)
+    {
+        if (n <= bytes) return cudaSuccess;
+        *this = PinnedBuf{};
+        const size_t nb = std::max<size_t>(4096, n + n / 2);
+        const cudaError_t e = cudaHostAlloc(&p, nb, cudaHostAllocDefault);
+        if (e != cudaSuccess) {
+            p = nullptr;
+            return e;
+        }
+        bytes = nb;
+        return cudaSuccess;
+    }
+    template <class T> T *as() const { return static_cast<T *>(p); }
+};
+
+struct Event {
+    cudaEvent_t h = nullptr;
+    Event() = default;
+    Event(Event &&o) noexcept { std::swap(h, o.h); }
+    Event &operator=(Event &&o) noexcept
+    {
+        std::swap(h, o.h);
+        return *this;
+    }
+    Event(const Event &) = delete;
+    Event &operator=(const Event &) = delete;
+    ~Event()
+    {
+        if (h) cudaEventDestroy(h);
+    }
+    cudaError_t create(unsigned flags)
+    {
+        Event fresh;
+        const cudaError_t e = cudaEventCreateWithFlags(&fresh.h, flags);
+        if (e == cudaSuccess) *this = std::move(fresh);
+        else fresh.h = nullptr;
+        return e;
+    }
+    operator cudaEvent_t() const { return h; }
+};
+
+struct Stream {
+    cudaStream_t h = nullptr;
+    Stream() = default;
+    Stream(Stream &&o) noexcept { std::swap(h, o.h); }
+    Stream &operator=(Stream &&o) noexcept
+    {
+        std::swap(h, o.h);
+        return *this;
+    }
+    Stream(const Stream &) = delete;
+    Stream &operator=(const Stream &) = delete;
+    ~Stream()
+    {
+        if (h) cudaStreamDestroy(h);
+    }
+    cudaError_t create(int priority = 0)
+    {
+        Stream fresh;
+        const cudaError_t e = priority ? cudaStreamCreateWithPriority(&fresh.h, cudaStreamNonBlocking, priority)
+                                       : cudaStreamCreateWithFlags(&fresh.h, cudaStreamNonBlocking);
+        if (e == cudaSuccess) *this = std::move(fresh);
+        else fresh.h = nullptr;
+        return e;
+    }
+    operator cudaStream_t() const { return h; }
 };
 
 struct Surface {
@@ -51,20 +170,18 @@ struct VisSlot {
     DevBuf b_vis[FYX_MAX_FRUSTA];
     DevBuf b_vis_slot[FYX_MAX_FRUSTA]; // the same entries as HBM slots (fyx_enable_instances)
     bool have_slots = false;
-    uint32_t *d_counts = nullptr; // kCountStride * FYX_MAX_FRUSTA, each counter on its own 128 B line
-    uint32_t *h_counts = nullptr; // pinned, FYX_MAX_FRUSTA
-    uint32_t *h_vis[FYX_MAX_FRUSTA] = {};
-    size_t h_vis_cap[FYX_MAX_FRUSTA] = {};
+    DevBuf d_counts;    // kCountStride * FYX_MAX_FRUSTA, each counter on its own 128 B line
+    PinnedBuf h_counts; // FYX_MAX_FRUSTA
+    PinnedBuf h_vis[FYX_MAX_FRUSTA];
     uint32_t nf = 0;
     bool counts_on_host = false, lists_on_host = false;
     // multi-GPU: the all-gathered lists of this frame (padded slots, packed list, host copy)
     DevBuf b_gath_pad[FYX_MAX_FRUSTA], b_gath[FYX_MAX_FRUSTA];
     uint32_t gath_count[FYX_MAX_FRUSTA] = {};
-    uint32_t *h_gath[FYX_MAX_FRUSTA] = {};
-    size_t h_gath_cap[FYX_MAX_FRUSTA] = {};
+    PinnedBuf h_gath[FYX_MAX_FRUSTA];
     bool gathered = false, gathered_on_host = false;
     bool own_only = false; // FYX_FRAME_READBACK_OWN: the host copy of this frame is the rank's own lists
-    cudaEvent_t ev_gather = nullptr, ev_counts_all = nullptr;
+    Event ev_gather, ev_counts_all;
     uint64_t epoch = 0;            // number of this gathered frame (the same on every rank)
     bool via_peer = false;         // exchanged by peer stores (fyx_peer.cu), else NCCL
     uint32_t *gath_ptr[FYX_MAX_FRUSTA] = {}; // the gathered list on the device (peer allocation or b_gath)
@@ -76,7 +193,7 @@ struct VisSlot {
     uint32_t *seg_own[FYX_MAX_FRUSTA] = {};
     bool pending = false; // written by a pipelined (async + read-back) frame that fyx_frame_wait has not collected yet
     uint64_t frame_no = 0;
-    cudaEvent_t ev_cull = nullptr, ev_counts = nullptr, ev_done = nullptr;
+    Event ev_cull, ev_counts, ev_done;
 };
 
 // N2: one animation on the host side (fyx_anim.inl)
@@ -88,14 +205,12 @@ struct AnimHost {
 // N3: packed instances of one frustum (fyx_drawprep.inl)
 struct InstOut {
     DevBuf b_node, b_sort, b_mats, b_bundles, b_surf, b_skin;
-    void *h_surf = nullptr;
-    size_t h_surf_cap = 0;
+    PinnedBuf h_surf;
     uint32_t n_visible = 0;
     DevBuf b_block_of, b_blocks; // bone-matrix blocks of the skinned instances (fyx_pack_bone_matrices)
     uint32_t n_blocks = 0;
     bool blocks_valid = false;
-    void *h[4] = {};
-    size_t h_cap[4] = {};
+    PinnedBuf h[4];
     uint32_t count = 0, n_bundles = 0;
     bool valid = false, on_host = false;
 };
@@ -103,18 +218,18 @@ struct InstOut {
 } // namespace
 
 struct PeerState {
-    void *local = nullptr;                 // this rank's exchange allocation (control block + 2 x F lists)
+    DevBuf local;                          // this rank's exchange allocation (control block + 2 x F lists)
     void *mapped[kPeerMaxRanks] = {};      // the other ranks' allocations (cudaIpcOpenMemHandle)
-    uint32_t *cta_done = nullptr;
-    uint32_t *h_counts = nullptr;          // pinned: [epoch & 1][2][rank][frustum] copy of the count table
+    DevBuf cta_done;
+    PinnedBuf h_counts;                    // [epoch & 1][2][rank][frustum] copy of the count table
     PeerParams pp{};
     bool ready = false;
 };
 
 struct fyx_ctx {
     int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = false;
+    cudaStream_t stream = nullptr; // own_stream, or the caller's stream from fyx_config (never destroyed here)
+    Stream own_stream;
     std::string err;
     uint64_t launches = 0;
 
@@ -132,12 +247,11 @@ struct fyx_ctx {
     bool have_trs = false;
 
     // error word written by kernels
-    uint32_t *d_err = nullptr;
-    uint32_t *h_err = nullptr; // pinned
+    DevBuf d_err;
+    PinnedBuf h_err;
 
     // staging (host pinned + device)
-    void *h_stage = nullptr;
-    size_t h_stage_bytes = 0;
+    PinnedBuf h_stage;
     DevBuf d_stage;
 
     // cull outputs
@@ -149,11 +263,11 @@ struct fyx_ctx {
 
     // frame pipelining (FYX_FRAME_ASYNC): uploads on their own stream into alternating staging buffers,
     // read-backs on a third stream
-    cudaStream_t copy_stream = nullptr, d2h_stream = nullptr;
-    cudaStream_t fold_stream = nullptr; // skinned-mesh fold + cull beside the palette / skinning kernels of asynchronous frames
-    cudaEvent_t ev_levels_done = nullptr, ev_fold_done = nullptr;
+    Stream copy_stream, d2h_stream;
+    Stream fold_stream; // skinned-mesh fold + cull beside the palette / skinning kernels of asynchronous frames
+    Event ev_levels_done, ev_fold_done;
     DevBuf d_stage_frame[2];
-    cudaEvent_t ev_upload[2] = {}, ev_slot_free[2] = {};
+    Event ev_upload[2], ev_slot_free[2];
     bool slot_used[2] = {false, false};
     int upload_parity = 0;
     cudaEvent_t ev_levels_prev = nullptr; // the previous frame's "level kernels + fold + cull are done" event (its ev_cull), if it recorded one
@@ -185,7 +299,7 @@ struct fyx_ctx {
     std::vector<uint8_t> skinned_node; // per node: has a skinned surface
 
     // timing
-    cudaEvent_t ev[EV_COUNT] = {};
+    Event ev[EV_COUNT];
     fyx_timings timings{};
     bool timings_pending = false; // an async frame's events have not been read yet
     bool stage_events_valid = false; // the last frame recorded the per-stage events (synchronous frames only)
@@ -213,7 +327,7 @@ struct fyx_ctx {
 
     // N4 light lists (fyx_drawprep.inl)
     DevBuf b_light[FYX_MAX_FRUSTA], b_light_ptrs, b_light_counts;
-    uint32_t *h_light_counts = nullptr; // pinned
+    PinnedBuf h_light_counts;
     std::vector<uint32_t> h_light[FYX_MAX_FRUSTA];
     uint32_t light_nf = 0;
     bool lights_valid = false;
@@ -224,9 +338,8 @@ struct fyx_ctx {
     bool light_table_dirty = false;
     uint32_t n_light_table = 0;
     DevBuf b_light_table, b_sh_scratch, b_sh_frusta, b_sh_maps, b_sh_counts, b_sh_warp_any, b_sh_small, b_sh_entries;
-    uint32_t *h_sh_small = nullptr; // pinned: n_maps, total
-    void *h_sh_maps = nullptr, *h_sh_entries = nullptr;
-    size_t h_sh_maps_cap = 0, h_sh_entries_cap = 0;
+    PinnedBuf h_sh_small; // n_maps, total
+    PinnedBuf h_sh_maps, h_sh_entries;
     uint32_t sh_n_maps = 0, sh_total = 0;
     bool sh_valid = false, sh_on_host = false;
 
@@ -234,15 +347,15 @@ struct fyx_ctx {
     bool instances_enabled = false, have_bundles = false, rank_on_device = false;
     uint32_t n_bundle_ids = 1;
     DevBuf b_bundle, b_rank_slot, b_inst_hist, b_inst_first, b_inst_offset, b_inst_tmp, b_inst_nb;
-    uint32_t *h_inst_nb = nullptr;
+    PinnedBuf h_inst_nb;
     InstOut inst[FYX_MAX_FRUSTA];
 
     // multi-GPU (fyx_comm.cu)
     void *comm = nullptr;
     int nranks = 1, rank = 0;
-    cudaStream_t comm_stream = nullptr; // the collective runs beside the palette / skinning kernels (highest priority)
+    Stream comm_stream; // the collective runs beside the palette / skinning kernels (highest priority)
     DevBuf b_counts_packed, b_counts_all;
-    uint32_t *h_counts_all = nullptr; // pinned nranks*FYX_MAX_FRUSTA
+    PinnedBuf h_counts_all; // nranks*FYX_MAX_FRUSTA
     bool want_peer = true, want_hostseg = true;
     unsigned peer_push_ctas = 96;
     bool exchange_built = false, hostseg_ready = false, hostseg_registered = false;
@@ -250,10 +363,10 @@ struct fyx_ctx {
     uint64_t exch_total_cap = 0, gather_epoch = 0;
     PeerState peer;
     HostSeg hostseg;
-    cudaEvent_t ev_x0[2] = {}, ev_x1[2] = {}; // timing of the exchange (per epoch parity)
+    Event ev_x0[2], ev_x1[2]; // timing of the exchange (per epoch parity)
     uint64_t x_epoch[2] = {0, 0};
     int x_slot[2] = {0, 0};
-    cudaEvent_t ev_gath_read[2] = {}; // private D2H copies of the gathered device lists (per epoch parity)
+    Event ev_gath_read[2]; // private D2H copies of the gathered device lists (per epoch parity)
     bool gath_read_valid[2] = {false, false};
 };
 
@@ -284,44 +397,15 @@ int32_t dev_ensure(fyx_ctx *c, DevBuf &b, size_t bytes, bool keep = false)
     if (bytes <= b.bytes) return FYX_OK;
     size_t nb = keep ? std::max(bytes, b.bytes + b.bytes / 2) : bytes;
     nb = (nb + 255) & ~size_t(255);
-    void *np = nullptr;
-    CU(cudaMalloc(&np, nb));
+    DevBuf fresh;
+    CU(fresh.alloc(nb));
     // growable tables are copied as a whole when they grow again: give their not-yet-written tail a defined value
-    if (keep) CU(cudaMemsetAsync(np, 0, nb, c->stream));
-    if (b.p) {
-        cudaError_t e = cudaSuccess;
-        if (keep && b.bytes) e = cudaMemcpyAsync(np, b.p, b.bytes, cudaMemcpyDeviceToDevice, c->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) {
-            cudaFree(np); // the old buffer stays valid
-            return fail(c, FYX_ERR_CUDA, "growing a device buffer failed: %s", cudaGetErrorString(e));
-        }
-        cudaFree(b.p);
-    }
-    b.p = np;
-    b.bytes = nb;
-    return FYX_OK;
-}
-
-void dev_free(DevBuf &b)
-{
-    if (b.p) cudaFree(b.p);
-    b.p = nullptr;
-    b.bytes = 0;
-}
-
-int32_t host_stage_ensure(fyx_ctx *c, size_t bytes)
-{
-    if (bytes <= c->h_stage_bytes) return FYX_OK;
-    if (c->h_stage) {
+    if (keep) CU(cudaMemsetAsync(fresh.p, 0, nb, c->stream));
+    if (b.p) { // the old buffer stays valid until the stream has finished with it
+        if (keep && b.bytes) CU(cudaMemcpyAsync(fresh.p, b.p, b.bytes, cudaMemcpyDeviceToDevice, c->stream));
         CU(cudaStreamSynchronize(c->stream));
-        cudaFreeHost(c->h_stage);
-        c->h_stage = nullptr;
-        c->h_stage_bytes = 0;
     }
-    size_t nb = (bytes + bytes / 4 + 4095) & ~size_t(4095);
-    CU(cudaHostAlloc(&c->h_stage, nb, cudaHostAllocDefault));
-    c->h_stage_bytes = nb;
+    b = std::move(fresh);
     return FYX_OK;
 }
 
@@ -352,17 +436,16 @@ int32_t stage_to_device(fyx_ctx *c, const void *a0, size_t n0, const void *a1, s
     for (int i = 0; i < 2; ++i)
         if (src[i] && len[i] && !(direct && is_pinned(src[i]))) need_bounce = true;
     if (need_bounce) {
-        rc = host_stage_ensure(c, total);
-        if (rc) return rc;
-        // the previous use of the bounce buffer must have drained
+        // the previous use of the bounce buffer must have drained, before it is refilled or replaced
         CU(cudaStreamSynchronize(c->stream));
+        CU(c->h_stage.ensure(total));
     }
     for (int i = 0; i < 2; ++i) {
         if (!src[i] || !len[i]) continue;
         const void *from = src[i];
         if (!(direct && is_pinned(src[i]))) {
-            memcpy(static_cast<char *>(c->h_stage) + off[i], src[i], len[i]);
-            from = static_cast<char *>(c->h_stage) + off[i];
+            memcpy(c->h_stage.as<char>() + off[i], src[i], len[i]);
+            from = c->h_stage.as<char>() + off[i];
         }
         CU(cudaMemcpyAsync(dbase + off[i], from, len[i], cudaMemcpyHostToDevice, c->stream));
     }
@@ -374,10 +457,11 @@ int32_t stage_to_device(fyx_ctx *c, const void *a0, size_t n0, const void *a1, s
 int32_t check_device_errors(fyx_ctx *c)
 {
     // called right after a stream synchronisation; h_err was copied before it
-    const uint32_t e = *c->h_err;
+    uint32_t &h_err = *c->h_err.as<uint32_t>();
+    const uint32_t e = h_err;
     if (!e) return FYX_OK;
-    *c->h_err = 0;
-    cudaMemsetAsync(c->d_err, 0, sizeof(uint32_t), c->stream);
+    h_err = 0;
+    cudaMemsetAsync(c->d_err.p, 0, sizeof(uint32_t), c->stream);
     if (e & E_NOT_AFFINE)
         return fail(c, FYX_ERR_NOT_AFFINE, "a matrix with a bottom row other than (0,0,0,1) or a non-finite entry was skipped");
     if (e & E_BAD_BONE_INDEX) return fail(c, FYX_ERR_INVALID_ARGUMENT, "a vertex references a bone index >= n_bones");
@@ -388,7 +472,7 @@ int32_t check_device_errors(fyx_ctx *c)
 
 int32_t sync_and_check(fyx_ctx *c)
 {
-    CU(cudaMemcpyAsync(c->h_err, c->d_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(c->h_err.p, c->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     CU(cudaGetLastError());
     return check_device_errors(c);
@@ -419,7 +503,7 @@ int32_t prepare_cull(fyx_ctx *c, uint32_t nf, const fyx_frustum *fr, const uint3
     if (V.pending) return fail(c, FYX_ERR_STATE, "two pipelined frames are already in flight: call fyx_frame_wait first");
     c->cur = slot;
     c->cp.nf = (int)nf;
-    c->cp.counts = V.d_counts;
+    c->cp.counts = V.d_counts.as<uint32_t>();
     c->cp.one = 1.0f;
     c->cp.negzero = -0.0f;
     for (uint32_t f = 0; f < nf; ++f) {
@@ -438,7 +522,7 @@ int32_t prepare_cull(fyx_ctx *c, uint32_t nf, const fyx_frustum *fr, const uint3
     V.have_slots = c->instances_enabled;
     for (auto &o : c->inst) o.valid = false;
     c->lights_valid = false;
-    CU(cudaMemsetAsync(V.d_counts, 0, sizeof(uint32_t) * kCountStride * FYX_MAX_FRUSTA, c->stream));
+    CU(cudaMemsetAsync(V.d_counts.p, 0, sizeof(uint32_t) * kCountStride * FYX_MAX_FRUSTA, c->stream));
     V.nf = nf;
     V.counts_on_host = V.lists_on_host = false;
     V.gathered = V.gathered_on_host = false;
@@ -484,45 +568,22 @@ int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cu
 
 int32_t commit_surfaces(fyx_ctx *c);
 
-int32_t host_list_ensure(fyx_ctx *c, VisSlot &V, uint32_t f, size_t n)
-{
-    if (n <= V.h_vis_cap[f]) return FYX_OK;
-    if (V.h_vis[f]) cudaFreeHost(V.h_vis[f]);
-    V.h_vis[f] = nullptr;
-    const size_t cap = std::max<size_t>(1024, n + n / 2);
-    CU(cudaHostAlloc(reinterpret_cast<void **>(&V.h_vis[f]), cap * sizeof(uint32_t), cudaHostAllocDefault));
-    V.h_vis_cap[f] = cap;
-    return FYX_OK;
-}
-
-int32_t host_gath_ensure(fyx_ctx *c, VisSlot &V, uint32_t f, size_t n)
-{
-    if (n <= V.h_gath_cap[f]) return FYX_OK;
-    if (V.h_gath[f]) cudaFreeHost(V.h_gath[f]);
-    V.h_gath[f] = nullptr;
-    const size_t cap = std::max<size_t>(1024, n + n / 2);
-    CU(cudaHostAlloc(reinterpret_cast<void **>(&V.h_gath[f]), cap * sizeof(uint32_t), cudaHostAllocDefault));
-    V.h_gath_cap[f] = cap;
-    return FYX_OK;
-}
-
 // counts, then the lists sized by them, to pinned host memory (stream `s`, two synchronisations)
 int32_t readback_visible(fyx_ctx *c, VisSlot &V, cudaStream_t s)
 {
     const uint32_t nf = V.nf;
     if (!nf) return FYX_OK;
     if (!V.counts_on_host) {
-        CU(cudaMemcpy2DAsync(V.h_counts, sizeof(uint32_t), V.d_counts, sizeof(uint32_t) * kCountStride, sizeof(uint32_t), nf,
+        CU(cudaMemcpy2DAsync(V.h_counts.p, sizeof(uint32_t), V.d_counts.p, sizeof(uint32_t) * kCountStride, sizeof(uint32_t), nf,
                              cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         V.counts_on_host = true;
     }
     if (!V.lists_on_host) {
         for (uint32_t f = 0; f < nf; ++f) {
-            const size_t n = V.h_counts[f];
-            int32_t rc = host_list_ensure(c, V, f, n);
-            if (rc) return rc;
-            if (n) CU(cudaMemcpyAsync(V.h_vis[f], V.b_vis[f].p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+            const size_t n = V.h_counts.as<uint32_t>()[f];
+            CU(V.h_vis[f].ensure(n * sizeof(uint32_t)));
+            if (n) CU(cudaMemcpyAsync(V.h_vis[f].p, V.b_vis[f].p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
         }
         CU(cudaStreamSynchronize(s));
         V.lists_on_host = true;
@@ -564,72 +625,52 @@ extern "C" int32_t fyx_create(const fyx_config *cfg, fyx_ctx **out_ctx)
     if (prop.major != 9 || prop.minor != 0)
         return fail(nullptr, FYX_ERR_CUDA, "device %d is sm_%d%d; this library ships sm_90a code only", dev, prop.major, prop.minor);
 
-    fyx_ctx *ctx = new (std::nothrow) fyx_ctx();
+    // a failure below frees whatever was already made; CU() reports to fyx_last_error(NULL) because `c` stays NULL
+    std::unique_ptr<fyx_ctx> ctx(new (std::nothrow) fyx_ctx());
     if (!ctx) return fail(nullptr, FYX_ERR_OUT_OF_MEMORY, "host allocation failed");
-    c = ctx;
-    c->device = dev;
-    auto bail = [&](int32_t rc) {
-        g_create_error = c->err;
-        fyx_destroy(c);
-        return rc;
-    };
-#define CUB(call)                                                                                   \
-    do {                                                                                            \
-        cudaError_t e__ = (call);                                                                   \
-        if (e__ != cudaSuccess) {                                                                   \
-            fail(c, FYX_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e__));                 \
-            return bail(FYX_ERR_CUDA);                                                              \
-        }                                                                                           \
-    } while (0)
+    ctx->device = dev;
     if (stream) {
-        c->stream = static_cast<cudaStream_t>(stream);
+        ctx->stream = static_cast<cudaStream_t>(stream);
     } else {
-        CUB(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-        c->own_stream = true;
+        CU(ctx->own_stream.create());
+        ctx->stream = ctx->own_stream;
     }
-    CUB(cudaMalloc(reinterpret_cast<void **>(&c->d_err), sizeof(uint32_t)));
-    CUB(cudaMemset(c->d_err, 0, sizeof(uint32_t)));
-    CUB(cudaHostAlloc(reinterpret_cast<void **>(&c->h_err), sizeof(uint32_t), cudaHostAllocDefault));
-    *c->h_err = 0;
-    for (VisSlot &V : c->vs) {
-        CUB(cudaMalloc(reinterpret_cast<void **>(&V.d_counts), sizeof(uint32_t) * kCountStride * FYX_MAX_FRUSTA));
-        CUB(cudaMemset(V.d_counts, 0, sizeof(uint32_t) * kCountStride * FYX_MAX_FRUSTA));
-        CUB(cudaHostAlloc(reinterpret_cast<void **>(&V.h_counts), sizeof(uint32_t) * FYX_MAX_FRUSTA, cudaHostAllocDefault));
-        memset(V.h_counts, 0, sizeof(uint32_t) * FYX_MAX_FRUSTA);
-        CUB(cudaEventCreateWithFlags(&V.ev_cull, cudaEventDisableTiming));
-        CUB(cudaEventCreateWithFlags(&V.ev_counts, cudaEventDisableTiming));
-        CUB(cudaEventCreateWithFlags(&V.ev_done, cudaEventDisableTiming));
-        CUB(cudaEventCreateWithFlags(&V.ev_gather, cudaEventDisableTiming));
-        CUB(cudaEventCreateWithFlags(&V.ev_counts_all, cudaEventDisableTiming));
+    CU(ctx->d_err.alloc(sizeof(uint32_t)));
+    CU(cudaMemset(ctx->d_err.p, 0, sizeof(uint32_t)));
+    CU(ctx->h_err.ensure(sizeof(uint32_t)));
+    *ctx->h_err.as<uint32_t>() = 0;
+    for (VisSlot &V : ctx->vs) {
+        CU(V.d_counts.alloc(sizeof(uint32_t) * kCountStride * FYX_MAX_FRUSTA));
+        CU(cudaMemset(V.d_counts.p, 0, sizeof(uint32_t) * kCountStride * FYX_MAX_FRUSTA));
+        CU(V.h_counts.ensure(sizeof(uint32_t) * FYX_MAX_FRUSTA));
+        memset(V.h_counts.p, 0, sizeof(uint32_t) * FYX_MAX_FRUSTA);
+        for (Event *ev : {&V.ev_cull, &V.ev_counts, &V.ev_done, &V.ev_gather, &V.ev_counts_all}) CU(ev->create(cudaEventDisableTiming));
     }
     for (int i = 0; i < 2; ++i) {
-        CUB(cudaEventCreateWithFlags(&c->ev_gath_read[i], cudaEventDisableTiming));
-        CUB(cudaEventCreate(&c->ev_x0[i]));
-        CUB(cudaEventCreate(&c->ev_x1[i]));
+        CU(ctx->ev_gath_read[i].create(cudaEventDisableTiming));
+        CU(ctx->ev_x0[i].create(cudaEventDefault));
+        CU(ctx->ev_x1[i].create(cudaEventDefault));
     }
-    CUB(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
-    CUB(cudaStreamCreateWithFlags(&c->d2h_stream, cudaStreamNonBlocking));
-    CUB(cudaStreamCreateWithFlags(&c->fold_stream, cudaStreamNonBlocking));
-    CUB(cudaEventCreateWithFlags(&c->ev_levels_done, cudaEventDisableTiming));
-    CUB(cudaEventCreateWithFlags(&c->ev_fold_done, cudaEventDisableTiming));
+    CU(ctx->copy_stream.create());
+    CU(ctx->d2h_stream.create());
+    CU(ctx->fold_stream.create());
+    CU(ctx->ev_levels_done.create(cudaEventDisableTiming));
+    CU(ctx->ev_fold_done.create(cudaEventDisableTiming));
     for (int i = 0; i < 2; ++i) {
-        CUB(cudaEventCreateWithFlags(&c->ev_upload[i], cudaEventDisableTiming));
-        CUB(cudaEventCreateWithFlags(&c->ev_slot_free[i], cudaEventDisableTiming));
+        CU(ctx->ev_upload[i].create(cudaEventDisableTiming));
+        CU(ctx->ev_slot_free[i].create(cudaEventDisableTiming));
     }
-    for (int i = 0; i < EV_COUNT; ++i) CUB(cudaEventCreate(&c->ev[i]));
-#undef CUB
-    *out_ctx = c;
+    for (int i = 0; i < EV_COUNT; ++i) CU(ctx->ev[i].create(cudaEventDefault));
+    *out_ctx = ctx.release();
     return FYX_OK;
 }
 
 static void fyx_comm_destroy_internal(fyx_ctx *c); // fyx_comm.inl
-namespace { void inst_free(fyx_ctx *c); }              // fyx_drawprep.inl
 static bool lod_active(const fyx_ctx *c, uint32_t nf);  // fyx_drawprep.inl
 static int32_t lod_pass(fyx_ctx *c);                    // fyx_drawprep.inl
 // DFS-pruning features (LOD filter, static batches): the cull cannot be fused into the level kernels
 static bool unfused_cull(const fyx_ctx *c, uint32_t nf);
 static int32_t cull_unfused(fyx_ctx *c, uint32_t nf);
-namespace { void anim_free(fyx_ctx *c); }              // fyx_anim.inl
 static int32_t animate_enqueue(fyx_ctx *c, float dt);  // fyx_anim.inl
 static int32_t allgather_enqueue(fyx_ctx *c, VisSlot &V, cudaStream_t s);
 static int32_t allgather_finish(fyx_ctx *c, VisSlot &V, cudaStream_t s);
@@ -640,62 +681,10 @@ extern "C" void fyx_destroy(fyx_ctx *c)
 {
     if (!c) return;
     cudaSetDevice(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
+    // no stream may still use what the members free when they die
+    for (cudaStream_t s : {c->stream, c->copy_stream.h, c->d2h_stream.h, c->fold_stream.h, c->comm_stream.h})
+        if (s) cudaStreamSynchronize(s);
     fyx_comm_destroy_internal(c);
-    inst_free(c);
-    anim_free(c);
-    DevBuf *bufs[] = {&c->b_parent, &c->b_flags, &c->b_mask, &c->b_gidx, &c->b_slot_of_node, &c->d_stage, &c->b_statics, &c->b_trs, &c->b_vblk,
-                      &c->b_ms_range, &c->b_ms_bundle, &c->b_ms_skin, &c->b_prune, &c->b_sf_rng, &c->b_opos, &c->b_onrm, &c->b_bs, &c->b_bs_w, &c->b_surf_of_slot, &c->b_surf_bones, &c->b_palette, &c->b_bone_slot, &c->b_tiles, &c->b_fold_node,
-                      &c->b_fold_begin, &c->b_fold_bone, &c->b_fold_stale_idx, &c->b_late_slot, &c->b_stale_pos, &c->b_counts_packed, &c->b_counts_all};
-    for (DevBuf *b : bufs) dev_free(*b);
-    for (int i = 0; i < 3; ++i) {
-        dev_free(c->b_L[i]);
-        dev_free(c->b_G[i]);
-        dev_free(c->b_la[i]);
-        dev_free(c->b_wa[i]);
-        dev_free(c->b_ib[i]);
-    }
-    if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
-    if (c->d2h_stream) cudaStreamSynchronize(c->d2h_stream);
-    if (c->fold_stream) cudaStreamSynchronize(c->fold_stream);
-    for (VisSlot &V : c->vs) {
-        for (uint32_t f = 0; f < FYX_MAX_FRUSTA; ++f) {
-            dev_free(V.b_vis[f]);
-            if (V.h_vis[f]) cudaFreeHost(V.h_vis[f]);
-            dev_free(V.b_gath_pad[f]);
-            dev_free(V.b_gath[f]);
-            if (V.h_gath[f]) cudaFreeHost(V.h_gath[f]);
-        }
-        if (V.ev_gather) cudaEventDestroy(V.ev_gather);
-        if (V.ev_counts_all) cudaEventDestroy(V.ev_counts_all);
-        if (V.d_counts) cudaFree(V.d_counts);
-        if (V.h_counts) cudaFreeHost(V.h_counts);
-        if (V.ev_cull) cudaEventDestroy(V.ev_cull);
-        if (V.ev_counts) cudaEventDestroy(V.ev_counts);
-        if (V.ev_done) cudaEventDestroy(V.ev_done);
-    }
-    for (int i = 0; i < 2; ++i) {
-        dev_free(c->d_stage_frame[i]);
-        if (c->ev_upload[i]) cudaEventDestroy(c->ev_upload[i]);
-        if (c->ev_slot_free[i]) cudaEventDestroy(c->ev_slot_free[i]);
-    }
-    if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-    if (c->d2h_stream) cudaStreamDestroy(c->d2h_stream);
-    if (c->fold_stream) cudaStreamDestroy(c->fold_stream);
-    if (c->ev_levels_done) cudaEventDestroy(c->ev_levels_done);
-    if (c->ev_fold_done) cudaEventDestroy(c->ev_fold_done);
-    for (int i = 0; i < 2; ++i) {
-        if (c->ev_gath_read[i]) cudaEventDestroy(c->ev_gath_read[i]);
-        if (c->ev_x0[i]) cudaEventDestroy(c->ev_x0[i]);
-        if (c->ev_x1[i]) cudaEventDestroy(c->ev_x1[i]);
-    }
-    if (c->d_err) cudaFree(c->d_err);
-    if (c->h_err) cudaFreeHost(c->h_err);
-    if (c->h_counts_all) cudaFreeHost(c->h_counts_all);
-    if (c->h_stage) cudaFreeHost(c->h_stage);
-    for (int i = 0; i < EV_COUNT; ++i)
-        if (c->ev[i]) cudaEventDestroy(c->ev[i]);
-    if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
 
@@ -933,13 +922,8 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
         if (r2) return r2;
         launch_permute_words(c->stream, fresh.p, col.p, b_map.as<uint32_t>(), n_slots, words, def);
         c->launches++;
-        cudaError_t e = cudaStreamSynchronize(c->stream);
-        if (e != cudaSuccess) {
-            dev_free(fresh);
-            return fail(c, FYX_ERR_CUDA, "carrying a column over the topology change failed: %s", cudaGetErrorString(e));
-        }
-        dev_free(col);
-        col = fresh;
+        CU(cudaStreamSynchronize(c->stream));
+        col = std::move(fresh);
         return FYX_OK;
     };
     auto f2u = [](float v) { uint32_t u; memcpy(&u, &v, 4); return u; };
@@ -972,7 +956,6 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
             d.w[0] = 0x7FC00000u; // begin = NaN: not a LOD object
             if ((rc = carry_column(c->b_lod_range, 2, d))) return rc;
         }
-        dev_free(b_map);
     }
     c->light_table_dirty = true; // the light-source records stay with their node indices; their slots are looked up again
     if ((rc = dev_ensure(c, c->b_parent, n * 4))) return rc;
@@ -1066,7 +1049,7 @@ extern "C" int32_t fyx_set_local_matrices(fyx_ctx *c, uint32_t count, const uint
     int32_t rc = stage_to_device(c, m16, (size_t)count * 64, idx, idx ? (size_t)count * 4 : 0, false, &d_m, &d_i);
     if (rc) return rc;
     launch_scatter_locals(c->stream, c->a, count, static_cast<const uint32_t *>(d_i), static_cast<const float *>(d_m),
-                          c->b_slot_of_node.as<uint32_t>(), c->n_nodes, c->d_err);
+                          c->b_slot_of_node.as<uint32_t>(), c->n_nodes, c->d_err.as<uint32_t>());
     c->launches++;
     CU(cudaGetLastError());
     return FYX_OK;
@@ -1097,7 +1080,7 @@ extern "C" int32_t fyx_set_local_rotations(fyx_ctx *c, uint32_t count, const uin
     if (rc) return rc;
     launch_scatter_trs(c->stream, c->a, count, static_cast<const uint32_t *>(d_i), d_q, true, c->b_trs.as<fyx_trs>(),
                        c->have_statics ? c->b_statics.as<fyx_transform_statics>() : nullptr, c->b_slot_of_node.as<uint32_t>(), c->n_nodes,
-                       c->d_err);
+                       c->d_err.as<uint32_t>());
     c->launches++;
     CU(cudaGetLastError());
     return FYX_OK;
@@ -1117,7 +1100,7 @@ extern "C" int32_t fyx_set_local_trs(fyx_ctx *c, uint32_t count, const uint32_t 
     if (rc) return rc;
     launch_scatter_trs(c->stream, c->a, count, static_cast<const uint32_t *>(d_i), d_t, false, c->b_trs.as<fyx_trs>(),
                        c->have_statics ? c->b_statics.as<fyx_transform_statics>() : nullptr, c->b_slot_of_node.as<uint32_t>(), c->n_nodes,
-                       c->d_err);
+                       c->d_err.as<uint32_t>());
     c->launches++;
     CU(cudaGetLastError());
     return FYX_OK;
@@ -1400,14 +1383,14 @@ extern "C" int32_t fyx_add_skinned_surface(fyx_ctx *c, uint32_t mesh_node, uint3
         void *d_m = nullptr;
         if ((rc = stage_to_device(c, inv_bind, (size_t)n_bones * 64, nullptr, 0, false, &d_m, nullptr))) return rc;
         launch_ib_rows(c->stream, n_bones, static_cast<const float *>(d_m), c->b_ib[0].as<float4>() + sf.bone_off,
-                       c->b_ib[1].as<float4>() + sf.bone_off, c->b_ib[2].as<float4>() + sf.bone_off, c->d_err);
+                       c->b_ib[1].as<float4>() + sf.bone_off, c->b_ib[2].as<float4>() + sf.bone_off, c->d_err.as<uint32_t>());
         c->launches++;
     }
     if (n_verts) {
         void *d_v = nullptr;
         if ((rc = stage_to_device(c, verts, (size_t)n_verts * layout->stride, nullptr, 0, false, &d_v, nullptr))) return rc;
         launch_deinterleave(c->stream, n_verts, static_cast<const unsigned char *>(d_v), *layout, n_bones,
-                            c->b_vblk.as<float4>(), sf.vert_off, c->d_err);
+                            c->b_vblk.as<float4>(), sf.vert_off, c->d_err.as<uint32_t>());
         c->launches++;
     }
     CU(cudaGetLastError());
@@ -1587,8 +1570,8 @@ extern "C" int32_t fyx_get_visible(fyx_ctx *c, uint32_t f, const uint32_t **out_
     CU(cudaSetDevice(c->device));
     int32_t rc = readback_visible(c, V, c->stream);
     if (rc) return rc;
-    *out_idx = V.own_in_seg ? V.seg_own[f] : V.h_vis[f]; // a gathered frame's own lists sit inside the node-wide host segment
-    *out_count = V.h_counts[f];
+    *out_idx = V.own_in_seg ? V.seg_own[f] : V.h_vis[f].as<uint32_t>(); // a gathered frame's own lists sit inside the node-wide host segment
+    *out_count = V.h_counts.as<uint32_t>()[f];
     return FYX_OK;
 }
 
@@ -1598,7 +1581,7 @@ extern "C" int32_t fyx_get_visible_device(fyx_ctx *c, uint32_t f, const uint32_t
     VisSlot &V = c->vs[c->cur];
     if (f >= V.nf) return fail(c, FYX_ERR_INVALID_ARGUMENT, "frustum %u was not part of the last cull (%u frusta)", f, V.nf);
     *d_idx = V.b_vis[f].as<uint32_t>();
-    *d_count = V.d_counts + f * kCountStride;
+    *d_count = V.d_counts.as<uint32_t>() + f * kCountStride;
     return FYX_OK;
 }
 
@@ -1694,10 +1677,10 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
         auto scatter = [&](cudaStream_t ss, const void *d_p, const uint32_t *d_i) {
             if (as_rot || as_trs)
                 launch_scatter_trs(ss, c->a, fr->n_changed, d_i, d_p, as_rot, c->b_trs.as<fyx_trs>(), st, c->b_slot_of_node.as<uint32_t>(),
-                                   c->n_nodes, c->d_err);
+                                   c->n_nodes, c->d_err.as<uint32_t>());
             else
                 launch_scatter_locals(ss, c->a, fr->n_changed, d_i, static_cast<const float *>(d_p), c->b_slot_of_node.as<uint32_t>(),
-                                      c->n_nodes, c->d_err);
+                                      c->n_nodes, c->d_err.as<uint32_t>());
         };
         if (async && is_pinned(payload) && (!fr->changed_idx || is_pinned(fr->changed_idx))) {
             const int u = (c->upload_parity ^= 1);
@@ -1752,7 +1735,7 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
             return !(e && *e == '0');
         }();
         side_fold = side_fold_allowed && async && !unf && c->fold.n && fr->do_skin && c->n_tiles;
-        rc = run_update(c, fr->update_flags, (fr->n_frusta && !unf) ? &c->cp : nullptr, side_fold ? c->fold_stream : nullptr);
+        rc = run_update(c, fr->update_flags, (fr->n_frusta && !unf) ? &c->cp : nullptr, side_fold ? c->fold_stream.h : nullptr);
         if (rc) return rc;
         if (unf && (rc = cull_unfused(c, fr->n_frusta))) return rc;
     }
@@ -1801,7 +1784,7 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
         // deferred: counts travel on the read-back stream as soon as the cull is done; fyx_frame_wait fetches the lists
         CU(cudaEventRecord(V.ev_done, s));
         CU(cudaStreamWaitEvent(c->d2h_stream, V.ev_cull, 0));
-        CU(cudaMemcpy2DAsync(V.h_counts, sizeof(uint32_t), V.d_counts, sizeof(uint32_t) * kCountStride, sizeof(uint32_t), V.nf,
+        CU(cudaMemcpy2DAsync(V.h_counts.p, sizeof(uint32_t), V.d_counts.p, sizeof(uint32_t) * kCountStride, sizeof(uint32_t), V.nf,
                              cudaMemcpyDeviceToHost, c->d2h_stream));
         CU(cudaEventRecord(V.ev_counts, c->d2h_stream));
         V.pending = true;
@@ -1839,10 +1822,9 @@ extern "C" int32_t fyx_frame_wait(fyx_ctx *c)
     const bool seg = V.gathered && c->hostseg_ready && !V.host_copy_private;
     const bool own = !seg && (!V.gathered || V.own_only);
     for (uint32_t f = 0; f < V.nf && own; ++f) {
-        const size_t n = V.h_counts[f];
-        int32_t rc = host_list_ensure(c, V, f, n);
-        if (rc) return rc;
-        if (n) CU(cudaMemcpyAsync(V.h_vis[f], V.b_vis[f].p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->d2h_stream));
+        const size_t n = V.h_counts.as<uint32_t>()[f];
+        CU(V.h_vis[f].ensure(n * sizeof(uint32_t)));
+        if (n) CU(cudaMemcpyAsync(V.h_vis[f].p, V.b_vis[f].p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->d2h_stream));
     }
     if (seg) {
         // multi-GPU frame: this rank's own lists go into the node-wide host segment at their offsets (every rank does the
@@ -1855,16 +1837,15 @@ extern "C" int32_t fyx_frame_wait(fyx_ctx *c)
         CU(cudaStreamWaitEvent(c->d2h_stream, V.ev_gather, 0));
         for (uint32_t f = 0; f < V.nf; ++f) {
             const size_t n = V.gath_count[f];
-            rc = host_gath_ensure(c, V, f, n);
-            if (rc) return rc;
-            if (n) CU(cudaMemcpyAsync(V.h_gath[f], V.gath_ptr[f], n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->d2h_stream));
+            CU(V.h_gath[f].ensure(n * sizeof(uint32_t)));
+            if (n) CU(cudaMemcpyAsync(V.h_gath[f].p, V.gath_ptr[f], n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->d2h_stream));
         }
         CU(cudaEventRecord(c->ev_gath_read[V.epoch & 1], c->d2h_stream));
         c->gath_read_valid[V.epoch & 1] = true;
         V.gathered_on_host = true;
     }
     CU(cudaStreamWaitEvent(c->d2h_stream, V.ev_done, 0)); // the error word is final once the frame's last kernel ran
-    CU(cudaMemcpyAsync(c->h_err, c->d_err, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->d2h_stream));
+    CU(cudaMemcpyAsync(c->h_err.p, c->d_err.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->d2h_stream));
     CU(cudaStreamSynchronize(c->d2h_stream));
     V.lists_on_host = own || V.own_in_seg;
     V.pending = false;
