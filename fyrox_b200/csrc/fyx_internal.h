@@ -10,6 +10,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "../../include/fyrox_b200.h"
 #include "fyx_math.cuh"
@@ -224,13 +225,12 @@ void launch_scatter_trs(cudaStream_t s, const NodeArrays &a, uint32_t count, con
                         bool rot_only, fyx_trs *trs_by_slot /* device copy of the last records; may be nullptr unless rot_only */,
                         const fyx_transform_statics *statics_by_slot /* nullptr = defaults */, const uint32_t *slot_of_node,
                         uint32_t n_nodes, uint32_t *d_err);
-void launch_fill_identity_trs(cudaStream_t s, fyx_trs *trs_by_slot, uint32_t n);
-void launch_scatter_statics(cudaStream_t s, const NodeArrays &a, uint32_t count, const uint32_t *d_idx,
-                            const fyx_transform_statics *d_in, fyx_transform_statics *statics_by_slot,
-                            const uint32_t *slot_of_node, uint32_t n_nodes);
-void launch_fill_default_statics(cudaStream_t s, fyx_transform_statics *statics_by_slot, uint32_t n);
-void launch_scatter_u32(cudaStream_t s, uint32_t *dst_col, uint32_t count, const uint32_t *d_idx,
-                        const uint32_t *d_val, const uint32_t *slot_of_node, uint32_t n_nodes, int mode);
+// record e of d_val (`words` 32-bit words) into the slot of node d_idx[e] (d_idx nullptr = node e) of dst
+void launch_scatter_words(cudaStream_t s, uint32_t *dst, uint32_t words, uint32_t count, const uint32_t *d_idx,
+                          const uint32_t *d_val, const uint32_t *slot_of_node, uint32_t n_nodes);
+// node flags: the public input bits except ALIVE are replaced, the computed bits kept
+void launch_scatter_flags(cudaStream_t s, uint32_t *flags, uint32_t count, const uint32_t *d_idx,
+                          const uint32_t *d_val, const uint32_t *slot_of_node, uint32_t n_nodes);
 void launch_scatter_aabbs(cudaStream_t s, const NodeArrays &a, uint32_t count, const uint32_t *d_idx,
                           const float *d_aabb6, const uint32_t *slot_of_node, uint32_t n_nodes);
 void launch_gather_globals(cudaStream_t s, const NodeArrays &a, uint32_t count, const uint32_t *d_idx,
@@ -245,10 +245,19 @@ constexpr int kVblkRows = 11;                    // float4 rows per block
 constexpr int kVblkStride = kVblkRows * 32;      // float4 per block of 128 vertices
 void launch_ib_rows(cudaStream_t s, uint32_t n, const float *d_m16, float4 *r0, float4 *r1, float4 *r2, uint32_t *d_err);
 void launch_or_u32(cudaStream_t s, uint32_t *p, uint32_t bits);
-// dst[s] = map[s] != FYX_NONE ? src[map[s]] : default, records of `words` 32-bit words (<= 32): carries per-slot data over a
-// topology change (slots move; fyx_set_topology)
-struct PermuteDefault { uint32_t w[32]; };
-void launch_permute_words(cudaStream_t s, void *dst, const void *src, const uint32_t *map, uint32_t n, uint32_t words, const PermuteDefault &def);
+// One record of at most 32 words, copied from a value of a plain type (fyx_trs, float2, ...)
+struct WordRecord {
+    uint32_t words;
+    uint32_t w[32];
+    template <class T> explicit WordRecord(const T &v) : words(sizeof(T) / 4), w{}
+    {
+        static_assert(sizeof(T) % 4 == 0 && sizeof(T) <= sizeof(w), "a record is a whole number of at most 32 words");
+        memcpy(w, &v, sizeof(T));
+    }
+};
+// dst[s] = (map && map[s] != FYX_NONE) ? src[map[s]] : def, records of def.words words: carries per-slot data over a topology
+// change (slots move; fyx_set_topology), and with map == nullptr fills n records with def
+void launch_permute_words(cudaStream_t s, void *dst, const void *src, const uint32_t *map, uint32_t n, const WordRecord &def);
 void launch_compact_gathered(cudaStream_t s, const uint32_t *pad, uint32_t maxc, const uint32_t *counts_all, int nranks, int f,
                              uint32_t *dst);
 

@@ -996,45 +996,29 @@ __global__ void __launch_bounds__(kBlock) k_scatter_trs(const NodeArrays a, cons
     atomicOr(a.flags + slot, F_DIRTY_SELF); // NodeMessageKind::TransformChanged
 }
 
-__global__ void __launch_bounds__(kBlock) k_scatter_statics(const NodeArrays a, const uint32_t count, const uint32_t *d_idx,
-                                                            const fyx_transform_statics *d_in, fyx_transform_statics *st_by_slot,
-                                                            const uint32_t *slot_of_node, const uint32_t n_nodes)
+// one thread per word of the records
+__global__ void __launch_bounds__(kBlock) k_scatter_words(uint32_t *dst, const uint32_t words, const uint32_t count,
+                                                          const uint32_t *d_idx, const uint32_t *d_val,
+                                                          const uint32_t *slot_of_node, const uint32_t n_nodes)
+{
+    const uint64_t t = (uint64_t)blockIdx.x * kBlock + threadIdx.x;
+    if (t >= (uint64_t)count * words) return;
+    const uint32_t e = (uint32_t)(t / words), w = (uint32_t)(t % words);
+    const uint32_t slot = resolve_slot(d_idx, e, slot_of_node, n_nodes);
+    if (slot == FYX_NONE) return;
+    dst[(size_t)slot * words + w] = d_val[t];
+}
+
+__global__ void __launch_bounds__(kBlock) k_scatter_flags(uint32_t *flags, const uint32_t count, const uint32_t *d_idx,
+                                                          const uint32_t *d_val, const uint32_t *slot_of_node,
+                                                          const uint32_t n_nodes)
 {
     const uint32_t e = blockIdx.x * kBlock + threadIdx.x;
     if (e >= count) return;
     const uint32_t slot = resolve_slot(d_idx, e, slot_of_node, n_nodes);
     if (slot == FYX_NONE) return;
-    st_by_slot[slot] = d_in[e];
-}
-
-__global__ void __launch_bounds__(kBlock) k_fill_default_statics(fyx_transform_statics *st, const uint32_t n)
-{
-    const uint32_t e = blockIdx.x * kBlock + threadIdx.x;
-    if (e >= n) return;
-    fyx_transform_statics s;
-    s.pre_rotation[0] = s.pre_rotation[1] = s.pre_rotation[2] = 0.f;
-    s.pre_rotation[3] = 1.f;
-    for (int i = 0; i < 9; ++i) s.post_rotation_matrix[i] = (i % 4 == 0) ? 1.f : 0.f;
-    for (int i = 0; i < 3; ++i) s.rotation_offset[i] = s.rotation_pivot[i] = s.scaling_offset[i] = s.scaling_pivot[i] = 0.f;
-    st[e] = s;
-}
-
-// mode 0: node flags (public input bits except ALIVE are replaced); mode 1: plain column store
-__global__ void __launch_bounds__(kBlock) k_scatter_u32(uint32_t *dst_col, const uint32_t count, const uint32_t *d_idx,
-                                                        const uint32_t *d_val, const uint32_t *slot_of_node,
-                                                        const uint32_t n_nodes, const int mode)
-{
-    const uint32_t e = blockIdx.x * kBlock + threadIdx.x;
-    if (e >= count) return;
-    const uint32_t slot = resolve_slot(d_idx, e, slot_of_node, n_nodes);
-    if (slot == FYX_NONE) return;
-    if (mode == 0) {
-        constexpr uint32_t settable = FYX_NODE_INPUT_MASK & ~FYX_NODE_ALIVE;
-        const uint32_t old = dst_col[slot];
-        dst_col[slot] = (old & ~settable) | (d_val[e] & settable);
-    } else {
-        dst_col[slot] = d_val[e];
-    }
+    constexpr uint32_t settable = FYX_NODE_INPUT_MASK & ~FYX_NODE_ALIVE;
+    flags[slot] = (flags[slot] & ~settable) | (d_val[e] & settable);
 }
 
 __global__ void __launch_bounds__(kBlock) k_scatter_aabbs(const NodeArrays a, const uint32_t count, const uint32_t *d_idx,
@@ -1163,12 +1147,13 @@ __global__ void __launch_bounds__(kBlock) k_ib_rows(const uint32_t n, const floa
 __global__ void k_or_u32(uint32_t *p, const uint32_t bits) { atomicOr(p, bits); }
 
 __global__ void __launch_bounds__(kBlock) k_permute_words(uint32_t *dst, const uint32_t *src, const uint32_t *map, const uint32_t n,
-                                                          const uint32_t words, const PermuteDefault def)
+                                                          const WordRecord def)
 {
+    const uint32_t words = def.words;
     const uint64_t t = (uint64_t)blockIdx.x * kBlock + threadIdx.x;
     if (t >= (uint64_t)n * words) return;
     const uint32_t s = (uint32_t)(t / words), w = (uint32_t)(t % words);
-    const uint32_t o = map[s];
+    const uint32_t o = map ? map[s] : FYX_NONE;
     dst[t] = (o != FYX_NONE) ? src[(size_t)o * words + w] : def.w[w];
 }
 
@@ -1369,42 +1354,18 @@ void launch_scatter_trs(cudaStream_t s, const NodeArrays &a, uint32_t count, con
     }
 }
 
-__global__ void __launch_bounds__(kBlock) k_fill_identity_trs(fyx_trs *t, const uint32_t n)
+void launch_scatter_words(cudaStream_t s, uint32_t *dst, uint32_t words, uint32_t count, const uint32_t *d_idx,
+                          const uint32_t *d_val, const uint32_t *slot_of_node, uint32_t n_nodes)
 {
-    const uint32_t e = blockIdx.x * kBlock + threadIdx.x;
-    if (e >= n) return;
-    fyx_trs r;
-    r.position[0] = r.position[1] = r.position[2] = 0.f;
-    r.rotation[0] = r.rotation[1] = r.rotation[2] = 0.f;
-    r.rotation[3] = 1.f;
-    r.scale[0] = r.scale[1] = r.scale[2] = 1.f;
-    t[e] = r;
+    if (!count || !words) return;
+    k_scatter_words<<<grid_for((uint64_t)count * words), kBlock, 0, s>>>(dst, words, count, d_idx, d_val, slot_of_node, n_nodes);
 }
 
-void launch_fill_identity_trs(cudaStream_t s, fyx_trs *t, uint32_t n)
-{
-    if (!n) return;
-    k_fill_identity_trs<<<grid_for(n), kBlock, 0, s>>>(t, n);
-}
-
-void launch_scatter_statics(cudaStream_t s, const NodeArrays &a, uint32_t count, const uint32_t *d_idx, const fyx_transform_statics *d_in,
-                            fyx_transform_statics *st, const uint32_t *slot_of_node, uint32_t n_nodes)
+void launch_scatter_flags(cudaStream_t s, uint32_t *flags, uint32_t count, const uint32_t *d_idx,
+                          const uint32_t *d_val, const uint32_t *slot_of_node, uint32_t n_nodes)
 {
     if (!count) return;
-    k_scatter_statics<<<grid_for(count), kBlock, 0, s>>>(a, count, d_idx, d_in, st, slot_of_node, n_nodes);
-}
-
-void launch_fill_default_statics(cudaStream_t s, fyx_transform_statics *st, uint32_t n)
-{
-    if (!n) return;
-    k_fill_default_statics<<<grid_for(n), kBlock, 0, s>>>(st, n);
-}
-
-void launch_scatter_u32(cudaStream_t s, uint32_t *dst_col, uint32_t count, const uint32_t *d_idx,
-                        const uint32_t *d_val, const uint32_t *slot_of_node, uint32_t n_nodes, int mode)
-{
-    if (!count) return;
-    k_scatter_u32<<<grid_for(count), kBlock, 0, s>>>(dst_col, count, d_idx, d_val, slot_of_node, n_nodes, mode);
+    k_scatter_flags<<<grid_for(count), kBlock, 0, s>>>(flags, count, d_idx, d_val, slot_of_node, n_nodes);
 }
 
 void launch_scatter_aabbs(cudaStream_t s, const NodeArrays &a, uint32_t count, const uint32_t *d_idx, const float *d_aabb6,
@@ -1451,10 +1412,10 @@ void launch_ib_rows(cudaStream_t s, uint32_t n, const float *d_m16, float4 *r0, 
 
 void launch_or_u32(cudaStream_t s, uint32_t *p, uint32_t bits) { k_or_u32<<<1, 1, 0, s>>>(p, bits); }
 
-void launch_permute_words(cudaStream_t s, void *dst, const void *src, const uint32_t *map, uint32_t n, uint32_t words, const PermuteDefault &def)
+void launch_permute_words(cudaStream_t s, void *dst, const void *src, const uint32_t *map, uint32_t n, const WordRecord &def)
 {
-    if (!n || !words) return;
-    k_permute_words<<<grid_for((uint64_t)n * words), kBlock, 0, s>>>(static_cast<uint32_t *>(dst), static_cast<const uint32_t *>(src), map, n, words, def);
+    if (!n || !def.words) return;
+    k_permute_words<<<grid_for((uint64_t)n * def.words), kBlock, 0, s>>>(static_cast<uint32_t *>(dst), static_cast<const uint32_t *>(src), map, n, def);
 }
 
 void launch_compact_gathered(cudaStream_t s, const uint32_t *pad, uint32_t maxc, const uint32_t *counts_all, int nranks, int f,

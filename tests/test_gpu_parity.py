@@ -730,7 +730,10 @@ def test_add_link_remove_then_incremental_update_with_only_the_new_matrices(ctx)
     """The sequence INTEGRATION.md gives the Rust shim (ADVICE r1): fyx_set_topology with the pool's new columns after
     add / link / remove, then upload ONLY the matrices of the new nodes, then an incremental update.  Locals, TRS records,
     transform statics, bundle ids and LOD ranges of the surviving nodes must have followed them to their new slots: the
-    result equals an oracle built from scratch with every node's data."""
+    result equals an oracle built from scratch with every node's data.  Revived pool records start from the defaults: one
+    that is given only a rotation has position 0, scale 1 and the default statics, bundle 0 and no LOD range."""
+    from test_gpu_drawprep import check_instances
+
     rng = np.random.default_rng(17)
     n = 6000
     parent, flags, mask, local, aabb = random_graph(rng, n, p_dead=0.15)
@@ -745,7 +748,8 @@ def test_add_link_remove_then_incremental_update_with_only_the_new_matrices(ctx)
     trs[:, 3:7] = q / np.linalg.norm(q, axis=1, keepdims=True)
     trs[:, 7:10] = rng.uniform(0.5, 2.0, (len(trs_nodes), 3))
     ctx.set_local_trs(trs, trs_nodes)
-    fo, ff = camera_frustum(zfar=800.0, fovy=np.deg2rad(110.0))
+    eye = (0.0, 0.0, 150.0)  # the whole forest in view
+    fo, ff = camera_frustum(eye=eye, target=(0, 0, 0), zfar=800.0, fovy=np.deg2rad(110.0))
     ctx.update_and_cull([ff], fb.UPDATE_ALL)
 
     # topology B: revive dead pool records as new nodes, re-parent some old nodes, remove some leaves (a removed node takes
@@ -765,12 +769,43 @@ def test_add_link_remove_then_incremental_update_with_only_the_new_matrices(ctx)
     local2[new_nodes] = new_m
     movers = leaves[150:300]
     parent2[movers] = rng.choice(new_nodes, len(movers)).astype(np.uint32)  # old nodes under the new ones
+    # revived records that get nothing but a rotation, under the root
+    rng2 = np.random.default_rng(18)
+    revived = dead[len(dead) // 2: len(dead) // 2 + 8].astype(np.uint32)
+    flags2[revived] = fb.NODE_DEFAULT | fb.NODE_RENDERABLE
+    parent2[revived] = 0
+
+    # the side columns, each away from its default, set before topology B
+    st_nodes = trs_nodes[:150]
+    statics = np.zeros((len(st_nodes), 25), np.float32)
+    sq = rng2.normal(size=(len(st_nodes), 4)).astype(np.float32)
+    statics[:, 0:4] = sq / np.linalg.norm(sq, axis=1, keepdims=True)
+    statics[:, 4:13] = rng2.normal(size=(len(st_nodes), 9)).astype(np.float32)
+    statics[:, 13:25] = rng2.uniform(-2, 2, (len(st_nodes), 12)).astype(np.float32)
+    ctx.set_transform_statics(statics, st_nodes)
+    bundle = rng2.integers(1, 13, n).astype(np.uint32)  # every node; 0 is the default
+    ctx.set_bundle_ids(bundle)
+    zn, zf = 0.1, 800.0  # the camera's near / far planes, observer at its eye
+    # LOD objects: the visible survivors and some others; half of them in range for the observer before topology B
+    lod_nodes = np.union1d(np.intersect1d(ctx.get_visible(0), survivors), rng2.choice(survivors[survivors != 0], 200, replace=False))
+    lod_nodes = lod_nodes.astype(np.uint32)
+    dist = np.linalg.norm(ctx.get_global_matrices(lod_nodes)[:, 12:15] - np.float32(eye), axis=1)
+    cut = float(np.median((dist - zn) / (zf - zn)))
+    near = rng2.random(len(lod_nodes)) < 0.5
+    lod = np.where(near[:, None], [0.0, cut], [cut, 1.0]).astype(np.float32)
+    ctx.set_lod_ranges(lod, lod_nodes)
+    ctx.set_observers([(eye, zn, zf)])
+
     ctx.set_topology(parent2, flags2, mask, aabb)
     ctx.set_local_matrices(new_m, new_nodes)  # ONLY the new nodes
-    # a rotation-only update of the TRS-driven nodes must still find their positions / scales on the device
+    # a rotation-only update of the TRS-driven nodes must still find their positions / scales / statics on the device
     q2 = rng.normal(size=(len(trs_nodes), 4)).astype(np.float32)
     q2 /= np.linalg.norm(q2, axis=1, keepdims=True).astype(np.float32)
     ctx.set_local_rotations(q2, trs_nodes)
+    qr = rng2.normal(size=(len(revived), 4)).astype(np.float32)
+    qr /= np.linalg.norm(qr, axis=1, keepdims=True).astype(np.float32)
+    ctx.set_local_rotations(qr, revived)
+    ctx.enable_instances()
     ctx.update_and_cull([ff], fb.UPDATE_INCREMENTAL)
 
     # the oracle from scratch, with everybody's data
@@ -781,14 +816,33 @@ def test_add_link_remove_then_incremental_update_with_only_the_new_matrices(ctx)
     loc = sp.trs_bone_local(trs2)
     for k, i in enumerate(trs_nodes):
         local2[i] = loc(k)
+    for k, i in enumerate(st_nodes):
+        local2[i] = _oracle_transform(trs2[k, 0:3], trs2[k, 3:7], trs2[k, 7:10], statics[k])
+    for k, i in enumerate(revived):
+        local2[i] = _oracle_transform(np.zeros(3, np.float32), qr[k], np.ones(3, np.float32))
     og = ob.Graph.build(parent2, flags2, mask, local2, aabb)
     og.L.orc_graph_drop_messages(og.h)
+    og.set_lod_group(0, [(float(b), float(e), [int(x)]) for x, (b, e) in zip(lod_nodes, lod)])
     og.update_hierarchical_data()
     # the reference updates what its DFS reaches from the root; orphan sub-trees are not part of the comparison
     live = np.nonzero(reachable_from_root(parent2, flags2))[0].astype(np.uint32)
-    assert live.size > 4000
+    assert live.size > 4000 and np.isin(revived, live).all()
+    # local rows, TRS records and statics: every reachable node's global transform and box
     assert_same_hierarchy(og, ctx, live)
+    # LOD ranges: the culled list is LOD-filtered, and the filter hides something
+    want = og.from_graph_lod(fo, eye, zn, zf)
+    assert og.from_graph(fo).size - want.size >= 30
+    assert np.array_equal(np.sort(ctx.get_visible(0)), np.sort(want))
+    # bundle ids: the packed instances of the unfiltered list are grouped by the carried ids, the revived nodes' are 0
+    ctx.set_observers([])
+    ctx.cull([ff])
     assert_same_visible(og, ctx, [fo])
+    bundle2 = bundle.copy()
+    bundle2[new_nodes] = 0
+    bundle2[revived] = 0
+    view = ob.look_at_rh(eye, (0, 0, 0), (0, 1, 0))
+    vp = ob.mat4_mul(ob.perspective(16 / 9, float(np.deg2rad(110.0)), zn, zf), view)
+    assert check_instances(og, ctx, 0, fo, view, vp, bundle2) > 100
     # removed nodes read back as "not there" (identity / default box), like Pool::try_borrow failing
     assert np.array_equal(ctx.get_global_matrices(removed[:5]), np.tile(np.eye(4, dtype=np.float32).reshape(16), (5, 1)))
 
