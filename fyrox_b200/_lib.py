@@ -255,6 +255,13 @@ SYMBOLS = {
     "fyx_pack_bone_matrices": (C.c_int32, [ctx_p, C.c_uint32]),
     "fyx_get_bone_matrix_block": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     "fyx_get_bone_matrix_blocks_device": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
+    "fyx_pack_shadow_instances": (C.c_int32, [ctx_p]),
+    "fyx_get_shadow_instances": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),
+    "fyx_get_shadow_instances_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),
+    "fyx_get_shadow_instance_surfaces": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(u32p)]),
+    "fyx_pack_shadow_bone_matrices": (C.c_int32, [ctx_p]),
+    "fyx_get_shadow_bone_matrix_blocks_device": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
+    "fyx_get_shadow_bone_matrix_block": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     "fyx_set_blend_shapes": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]),
     "fyx_set_blend_shape_weights": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "fyx_allgather_visible": (C.c_int32, [ctx_p]),

@@ -466,6 +466,10 @@ class Context:
         self._chk(self._lib.fyx_pack_instances(self._h, frustum, _ptr(v), _ptr(vp)))
         out = L.fyx_instances()
         self._chk(self._lib.fyx_get_instances(self._h, frustum, C.byref(out)))
+        return self._instances_dict(out, self.get_instance_surfaces(frustum, out.count))
+
+    @staticmethod
+    def _instances_dict(out: L.fyx_instances, surface: np.ndarray) -> dict:
         n, nb = out.count, out.n_bundles
         bdt = np.dtype([("id", "<u4"), ("first", "<u4"), ("count", "<u4"), ("reserved", "<u4"), ("sort_index", "<u8")])
 
@@ -477,7 +481,7 @@ class Context:
 
         mats = arr(out.matrices, np.float32, n * 32).reshape(n, 2, 16)
         return {
-            "surface": self.get_instance_surfaces(frustum, n),
+            "surface": surface,
             "node": arr(out.node, np.uint32, n),
             "sort_index": arr(out.sort_index, np.uint64, n),
             "world": mats[:, 0, :].copy(),
@@ -494,6 +498,32 @@ class Context:
         out = np.empty((255, 16), dtype=np.float32)
         has = C.c_uint32()
         self._chk(self._lib.fyx_get_bone_matrix_block(self._h, frustum, instance, out.ctypes.data_as(C.c_void_p), C.byref(has)))
+        return out if has.value else None
+
+    def pack_shadow_instances(self):
+        """Pack the instances of every shadow map of the last cull_shadow_casters (made with enable_instances) in one call;
+        read them with get_shadow_instances(map)."""
+        self._chk(self._lib.fyx_pack_shadow_instances(self._h))
+
+    def get_shadow_instances(self, map: int) -> dict:
+        """Instances of shadow map `map`: the same dict as pack_instances, for the map's observer (its look_at_rh and
+        view_projection).  bundles["first"] counts from the map's first instance."""
+        out = L.fyx_instances()
+        self._chk(self._lib.fyx_get_shadow_instances(self._h, map, C.byref(out)))
+        p = L.u32p()
+        self._chk(self._lib.fyx_get_shadow_instance_surfaces(self._h, map, C.byref(p)))
+        surface = np.ctypeslib.as_array(p, shape=(out.count,)).copy() if out.count else np.empty(0, np.uint32)
+        return self._instances_dict(out, surface)
+
+    def pack_shadow_bone_matrices(self):
+        """One bone-matrix block (255 mat4, zero padded) per skinned surface, for the last pack_shadow_instances."""
+        self._chk(self._lib.fyx_pack_shadow_bone_matrices(self._h))
+
+    def get_shadow_bone_matrix_block(self, map: int, instance: int):
+        """(255,16) f32 block of instance `instance` of shadow map `map`, or None for an unskinned instance."""
+        out = np.empty((255, 16), dtype=np.float32)
+        has = C.c_uint32()
+        self._chk(self._lib.fyx_get_shadow_bone_matrix_block(self._h, map, instance, out.ctypes.data_as(C.c_void_p), C.byref(has)))
         return out if has.value else None
 
     def build_palettes(self):

@@ -300,6 +300,7 @@ struct fyx_ctx {
     std::vector<uint2> ms_of_node;       // (first, count) into ms_bundle_h / ms_skin_h; count 0 = default single surface
     std::vector<uint32_t> ms_bundle_h, ms_skin_h;
     bool ms_dirty = false, have_ms = false;
+    uint32_t ms_max = 0;                 // the most surfaces any node was given (bounds the shadow maps' bundle tables)
     DevBuf b_ms_range, b_ms_bundle, b_ms_skin;
     DevBuf b_surf_of_slot, b_surf_bones; // per slot: the node's first skinned surface (FYX_NONE = none); per surface: (first palette entry, n_bones)
     DevBuf b_bs, b_bs_w;          // blend-shape offsets (blocked f16) and weights
@@ -358,6 +359,12 @@ struct fyx_ctx {
     PinnedBuf h_sh_maps, h_sh_entries;
     uint32_t sh_n_maps = 0, sh_total = 0;
     bool sh_valid = false, sh_on_host = false;
+    // the shadow maps' instances (fyx_pack_shadow_instances): the shadow cull also records slots (with instances enabled)
+    // and view matrices; one packed InstOut for all maps, per map its instance and bundle ranges; bone blocks per surface
+    DevBuf b_sh_slots, b_sh_views, b_shi_seg, b_shi_tiles, b_shi_small;
+    bool sh_have_slots = false, sh_slots_stale = false;
+    InstOut shi;
+    std::vector<uint32_t> shi_inst_first, shi_bundle_first; // [maps + 1]
 
     // N3 draw-prep (fyx_drawprep.inl)
     bool instances_enabled = false, rank_on_device = false;
@@ -1037,6 +1044,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     c->updated_once = false;
     if (!same_capacity) c->dfs_rank.clear(); // indexed by node: stays valid while the pool capacity does
     c->rank_on_device = false; // re-derived from dfs_rank in the new slot order
+    c->sh_slots_stale = true;  // the last shadow cull's entry slots
     c->ms_dirty = c->have_ms;  // the per-slot surface table too (the CSR itself is by node)
     if (c->ms_of_node.size() < capacity) c->ms_of_node.resize(capacity, make_uint2(0u, 0u));
     c->anim_csr_dirty = true; // animated nodes are addressed by slot

@@ -39,32 +39,58 @@ __device__ __forceinline__ uint2 surfaces_of(const InstParams &ip, const uint32_
 }
 __device__ __forceinline__ uint32_t warp_max_u32(const uint32_t v) { return __reduce_max_sync(0xFFFFFFFFu, v); }
 
+// the segment (shadow map of the group) that owns list position i: the last map whose first entry is <= the entry (maps with
+// an empty list share their first with the next map and lose to it)
+__device__ __forceinline__ uint32_t segment_of(const InstParams &ip, const uint32_t i)
+{
+    const uint32_t e = ip.maps[ip.map0].first + i;
+    uint32_t lo = 0u, hi = ip.n_seg - 1u;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (ip.maps[ip.map0 + mid].first <= e) lo = mid;
+        else hi = mid - 1u;
+    }
+    return lo;
+}
+
 // pass 1: sort index per visible entry, bundle histogram over its surfaces (Mesh::collect_render_data pushes one instance per
-// surface, all with the node's sort index, scene/mesh/mod.rs:726-805), first-pushed instance per bundle
-__global__ void __launch_bounds__(kBlock) k_inst_keys(const NodeArrays a, const InstParams ip)
+// surface, all with the node's sort index, scene/mesh/mod.rs:726-805), first-pushed instance per bundle.  kSeg: the list is
+// several shadow maps; each entry takes its map's view matrix and counts into its map's bins.
+template <bool kSeg> __device__ __forceinline__ void inst_keys(const NodeArrays &a, const InstParams &ip)
 {
     const uint32_t i = blockIdx.x * kBlock + threadIdx.x;
     const bool valid = i < ip.n;
-    uint32_t slot = 0u, nsurf = 0u;
+    uint32_t slot = 0u, nsurf = 0u, seg = FYX_NONE, bin0 = 0u;
     uint2 sr = make_uint2(0u, 0u);
     unsigned long long key = ~0ull;
     if (valid) {
         slot = ip.vis_slot[i];
         // Base::global_position() = translation column of the global transform
         const float px = a.G[0][slot].w, py = a.G[1][slot].w, pz = a.G[2][slot].w;
-        ip.tmp_sort[i] = sorting_index(ip.view, px, py, pz);
+        if constexpr (kSeg) {
+            seg = segment_of(ip, i);
+            bin0 = seg * ip.n_bundle_ids;
+            ip.tmp_sort[i] = sorting_index(ip.views + (size_t)(ip.map0 + seg) * 16u, px, py, pz);
+        } else {
+            ip.tmp_sort[i] = sorting_index(ip.view, px, py, pz);
+        }
         const uint32_t rank = ip.rank_of_slot ? ip.rank_of_slot[slot] : ip.vis_node[i];
         key = ((unsigned long long)rank << 32) | i;
         sr = surfaces_of(ip, slot);
         nsurf = sr.y ? sr.y : 1u;
     }
-    const uint32_t rounds = warp_max_u32(nsurf);
     const int lane = threadIdx.x & 31;
+    if constexpr (kSeg) { // instances per map (a map's entries are contiguous: one or two atomics per warp)
+        const uint32_t peers = __match_any_sync(0xFFFFFFFFu, seg);
+        const uint32_t sum = __reduce_add_sync(peers, nsurf);
+        if (valid && lane == __ffs(peers) - 1) atomicAdd(ip.seg_inst + seg, sum);
+    }
+    const uint32_t rounds = warp_max_u32(nsurf);
     for (uint32_t k = 0; k < rounds; ++k) {
         const bool act = k < nsurf;
         uint32_t b = 0xFFFFFFFFu;
-        if (act) b = sr.y ? ip.ms_bundle[sr.x + k] : (ip.bundle_of_slot ? ip.bundle_of_slot[slot] : 0u);
-        // warp-aggregated histogram: one atomic per distinct bundle in the warp
+        if (act) b = bin0 + (sr.y ? ip.ms_bundle[sr.x + k] : (ip.bundle_of_slot ? ip.bundle_of_slot[slot] : 0u));
+        // warp-aggregated histogram: one atomic per distinct bin in the warp
         const uint32_t peers = __match_any_sync(0xFFFFFFFFu, b);
         if (act) {
             if ((peers & ((1u << lane) - 1u)) == 0u) atomicAdd(ip.hist + b, (uint32_t)__popc(peers));
@@ -73,6 +99,9 @@ __global__ void __launch_bounds__(kBlock) k_inst_keys(const NodeArrays a, const 
         }
     }
 }
+
+__global__ void __launch_bounds__(kBlock) k_inst_keys(const NodeArrays a, const InstParams ip) { inst_keys<false>(a, ip); }
+__global__ void __launch_bounds__(kBlock) k_shadow_inst_keys(const NodeArrays a, const InstParams ip) { inst_keys<true>(a, ip); }
 
 // pass 2 (one CTA): exclusive scan of the histogram -> first instance of every bundle, table of the non-empty
 // bundles; the histogram is zeroed again (pass 3 uses it as the scatter cursor)
@@ -135,27 +164,164 @@ __global__ void __launch_bounds__(kScanBlock) k_inst_scan(const InstParams ip)
     }
 }
 
+// Device-wide exclusive scan of the (segment, bundle) bins of a shadow group, in three launches: per-tile sums, one CTA
+// that scans the tile sums and the segments' instance counts, and a downsweep that writes every bin's first instance,
+// the compacted bundle table in (segment, id) order and each segment's first bundle.  kScanTile bins per CTA of 1024
+// threads, four consecutive bins per thread.
+constexpr int kBinThreads = 1024;
+static_assert(kScanTile == 4u * kBinThreads, "four bins per thread");
+
+// (instances, bundles) of a thread's four bins, summed over the CTA; every thread gets the CTA-wide exclusive prefix of its
+// own pair and the CTA total
+__device__ __forceinline__ uint2 cta_exclusive_scan(const uint2 v, uint2 &total)
+{
+    __shared__ uint2 s_w[kBinThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint2 x = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t tx = __shfl_up_sync(0xFFFFFFFFu, x.x, d), ty = __shfl_up_sync(0xFFFFFFFFu, x.y, d);
+        if (lane >= d) { x.x += tx; x.y += ty; }
+    }
+    if (lane == 31) s_w[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        uint2 w = s_w[lane];
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t tx = __shfl_up_sync(0xFFFFFFFFu, w.x, d), ty = __shfl_up_sync(0xFFFFFFFFu, w.y, d);
+            if (lane >= d) { w.x += tx; w.y += ty; }
+        }
+        s_w[lane] = w; // inclusive over warps
+    }
+    __syncthreads();
+    total = s_w[kBinThreads / 32 - 1];
+    const uint2 before = warp ? s_w[warp - 1] : make_uint2(0u, 0u);
+    const uint2 r = make_uint2(before.x + x.x - v.x, before.y + x.y - v.y);
+    __syncthreads(); // s_w is reused by the next call
+    return r;
+}
+
+__device__ __forceinline__ uint4 load_bins(const InstParams &ip, const uint32_t bin0, const uint32_t n_bins)
+{
+    uint4 c = make_uint4(0u, 0u, 0u, 0u);
+    if (bin0 + 3u < n_bins) return *reinterpret_cast<const uint4 *>(ip.hist + bin0); // 16-B aligned: bin0 % 4 == 0
+    if (bin0 < n_bins) c.x = ip.hist[bin0];
+    if (bin0 + 1u < n_bins) c.y = ip.hist[bin0 + 1u];
+    if (bin0 + 2u < n_bins) c.z = ip.hist[bin0 + 2u];
+    return c;
+}
+
+__global__ void __launch_bounds__(kBinThreads) k_bin_reduce(const InstParams ip)
+{
+    pdl_trigger();
+    pdl_wait(); // the histogram of the keys pass
+    const uint32_t n_bins = ip.n_seg * ip.n_bundle_ids;
+    const uint4 c = load_bins(ip, blockIdx.x * kScanTile + threadIdx.x * 4u, n_bins);
+    const uint2 v = make_uint2(c.x + c.y + c.z + c.w, (c.x != 0u) + (c.y != 0u) + (c.z != 0u) + (c.w != 0u));
+    uint2 total;
+    cta_exclusive_scan(v, total);
+    if (threadIdx.x == 0) ip.tile_sum[blockIdx.x] = total;
+}
+
+// one CTA: tile sums -> their exclusive prefix (in place), segment instance counts -> every segment's first instance, totals
+__global__ void __launch_bounds__(kBinThreads) k_bin_scan(const InstParams ip, const uint32_t n_tiles)
+{
+    __shared__ uint2 s_carry;
+    pdl_trigger();
+    pdl_wait(); // the tile sums
+    if (threadIdx.x == 0) s_carry = make_uint2(0u, 0u);
+    __syncthreads();
+    for (uint32_t base = 0; base < n_tiles; base += kBinThreads) {
+        const uint32_t t = base + threadIdx.x;
+        const uint2 v = t < n_tiles ? ip.tile_sum[t] : make_uint2(0u, 0u);
+        uint2 total;
+        const uint2 ex = cta_exclusive_scan(v, total);
+        if (t < n_tiles) ip.tile_sum[t] = make_uint2(s_carry.x + ex.x, s_carry.y + ex.y);
+        __syncthreads();
+        if (threadIdx.x == 0) s_carry = make_uint2(s_carry.x + total.x, s_carry.y + total.y);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        ip.o_totals[0] = s_carry.y;
+        ip.o_totals[1] = s_carry.x;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) s_carry = make_uint2(0u, 0u);
+    __syncthreads();
+    for (uint32_t base = 0; base < ip.n_seg; base += kBinThreads) {
+        const uint32_t sg = base + threadIdx.x;
+        const uint2 v = make_uint2(sg < ip.n_seg ? ip.seg_inst[sg] : 0u, 0u);
+        uint2 total;
+        const uint2 ex = cta_exclusive_scan(v, total);
+        if (sg < ip.n_seg) ip.seg_first[sg] = ip.base_inst + s_carry.x + ex.x;
+        __syncthreads();
+        if (threadIdx.x == 0) s_carry.x += total.x;
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(kBinThreads) k_bin_downsweep(const InstParams ip)
+{
+    pdl_trigger();
+    pdl_wait(); // the tile prefixes and the segments' first instances
+    const uint32_t n_bins = ip.n_seg * ip.n_bundle_ids;
+    const uint32_t bin0 = blockIdx.x * kScanTile + threadIdx.x * 4u;
+    const uint4 c4 = load_bins(ip, bin0, n_bins);
+    const uint32_t c[4] = {c4.x, c4.y, c4.z, c4.w};
+    const uint2 v = make_uint2(c[0] + c[1] + c[2] + c[3], (c[0] != 0u) + (c[1] != 0u) + (c[2] != 0u) + (c[3] != 0u));
+    uint2 total;
+    const uint2 ex = cta_exclusive_scan(v, total);
+    const uint2 tb = ip.tile_sum[blockIdx.x];
+    uint32_t off = ip.base_inst + tb.x + ex.x, k = ip.base_bundle + tb.y + ex.y;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const uint32_t bin = bin0 + j;
+        if (bin >= n_bins) break;
+        const uint32_t seg = bin / ip.n_bundle_ids, id = bin - seg * ip.n_bundle_ids;
+        if (id == 0u) ip.seg_bfirst[seg] = k;
+        ip.offset[bin] = off;
+        ip.hist[bin] = 0u; // the scatter cursor
+        if (c[j]) {
+            fyx_bundle r;
+            r.id = id;
+            r.first = off - ip.seg_first[seg]; // relative to the map's instances
+            r.count = c[j];
+            r.reserved = 0u;
+            r.sort_index = ip.tmp_sort[(uint32_t)(ip.first_key[bin] & 0xFFFFFFFFull)];
+            ip.o_bundles[k] = r;
+            ++k;
+        }
+        off += c[j];
+    }
+}
+
 // pass 3: scatter into bundle order; matrices are written by 8 lanes per instance (one float4 column each), so a
-// warp store covers four whole 128-byte instance records
-__global__ void __launch_bounds__(kBlock) k_inst_scatter(const NodeArrays a, const InstParams ip)
+// warp store covers four whole 128-byte instance records.  kSeg: the bins and view_projection of each entry's map.
+template <bool kSeg> __device__ __forceinline__ void inst_scatter(const NodeArrays &a, const InstParams &ip)
 {
     const uint32_t i = blockIdx.x * kBlock + threadIdx.x;
     const int lane = threadIdx.x & 31;
     const bool valid = i < ip.n;
-    uint32_t slot = 0u, nsurf = 0u, node_flags = 0u;
+    uint32_t slot = 0u, nsurf = 0u, node_flags = 0u, bin0 = 0u, map = 0u;
     uint2 sr = make_uint2(0u, 0u);
     if (valid) {
         slot = ip.vis_slot[i];
         sr = surfaces_of(ip, slot);
         nsurf = sr.y ? sr.y : 1u;
         node_flags = a.flags[slot];
+        if constexpr (kSeg) {
+            const uint32_t seg = segment_of(ip, i);
+            bin0 = seg * ip.n_bundle_ids;
+            map = ip.map0 + seg;
+        }
     }
     const uint32_t rounds = warp_max_u32(nsurf);
     for (uint32_t k = 0; k < rounds; ++k) {
         const bool act = k < nsurf;
         uint32_t b = 0xFFFFFFFFu, pos = 0u, skin = FYX_NONE;
         if (act) {
-            b = sr.y ? ip.ms_bundle[sr.x + k] : (ip.bundle_of_slot ? ip.bundle_of_slot[slot] : 0u);
+            b = bin0 + (sr.y ? ip.ms_bundle[sr.x + k] : (ip.bundle_of_slot ? ip.bundle_of_slot[slot] : 0u));
             skin = sr.y ? ip.ms_skin[sr.x + k] : ip.surf_of_slot[slot];
         }
         const uint32_t peers = __match_any_sync(0xFFFFFFFFu, b);
@@ -181,6 +347,8 @@ __global__ void __launch_bounds__(kBlock) k_inst_scatter(const NodeArrays a, con
             const uint32_t se = __shfl_sync(0xFFFFFFFFu, slot, e);
             const bool ve = __shfl_sync(0xFFFFFFFFu, (int)act, e) != 0;
             const bool ie = __shfl_sync(0xFFFFFFFFu, (int)ident, e) != 0;
+            uint32_t me = 0u;
+            if constexpr (kSeg) me = __shfl_sync(0xFFFFFFFFu, map, e);
             if (!ve) continue;
             float w0, w1, w2, w3 = (c == 3) ? 1.0f : 0.0f;
             if (ie) {
@@ -198,7 +366,9 @@ __global__ void __launch_bounds__(kBlock) k_inst_scatter(const NodeArrays a, con
                 o = make_float4(w0, w1, w2, w3);
             } else {
                 // (view_projection * world)[r, c], nalgebra order (Appendix A1), full 4x4: VP is projective
-                const float *m = ip.vp;
+                const float *m;
+                if constexpr (kSeg) m = ip.maps[me].view_projection;
+                else m = ip.vp;
                 o.x = FYX_ADD(FYX_ADD(FYX_ADD(FYX_MUL(m[0], w0), FYX_MUL(m[4], w1)), FYX_MUL(m[8], w2)), FYX_MUL(m[12], w3));
                 o.y = FYX_ADD(FYX_ADD(FYX_ADD(FYX_MUL(m[1], w0), FYX_MUL(m[5], w1)), FYX_MUL(m[9], w2)), FYX_MUL(m[13], w3));
                 o.z = FYX_ADD(FYX_ADD(FYX_ADD(FYX_MUL(m[2], w0), FYX_MUL(m[6], w1)), FYX_MUL(m[10], w2)), FYX_MUL(m[14], w3));
@@ -208,6 +378,9 @@ __global__ void __launch_bounds__(kBlock) k_inst_scatter(const NodeArrays a, con
         }
     }
 }
+
+__global__ void __launch_bounds__(kBlock) k_inst_scatter(const NodeArrays a, const InstParams ip) { inst_scatter<false>(a, ip); }
+__global__ void __launch_bounds__(kBlock) k_shadow_inst_scatter(const NodeArrays a, const InstParams ip) { inst_scatter<true>(a, ip); }
 
 } // namespace
 
@@ -250,14 +423,15 @@ __global__ void __launch_bounds__(kBlock) k_bone_block_index(const uint32_t n, c
     if (i >= n) return;
     block_of_inst[i] = (inst_skin[i] != FYX_NONE) ? atomicAdd(counter, 1u) : FYX_NONE;
 }
-// pass 2: one CTA per instance copies the surface's palette and pads with zeros (1020 float4 per block)
+// pass 2: one CTA per instance (or, without inst_skin / block_of_inst, per surface: the shadow maps' blocks) copies the
+// surface's palette and pads with zeros (1020 float4 per block)
 __global__ void __launch_bounds__(kBlock) k_bone_blocks(const uint32_t *inst_skin, const uint2 *surf_bones /* (first palette entry, n_bones) */,
                                                         const float4 *palette, const uint32_t *block_of_inst, float4 *blocks)
 {
     const uint32_t i = blockIdx.x;
-    const uint32_t blk = block_of_inst[i];
+    const uint32_t blk = block_of_inst ? block_of_inst[i] : i;
     if (blk == FYX_NONE) return;
-    const uint2 sb = surf_bones[inst_skin[i]];
+    const uint2 sb = surf_bones[inst_skin ? inst_skin[i] : i];
     float4 *dst = blocks + (size_t)blk * (FYX_MAX_BONES * 4);
     const float4 *src = palette + (size_t)sb.x * 4;
     for (uint32_t e = threadIdx.x; e < FYX_MAX_BONES * 4; e += kBlock) dst[e] = (e < sb.y * 4u) ? src[e] : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -282,6 +456,21 @@ void launch_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip
 void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip)
 {
     if (ip.n) k_inst_scatter<<<(ip.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, ip);
+}
+
+// the scratch is cleared by the caller: hist 0, first_key ~0, seg_inst 0
+void launch_shadow_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip)
+{
+    const uint32_t n_tiles = (ip.n_seg * ip.n_bundle_ids + kScanTile - 1) / kScanTile;
+    if (ip.n) k_shadow_inst_keys<<<(ip.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, ip);
+    launch_pdl(k_bin_reduce, n_tiles, kBinThreads, 0, s, ip);
+    launch_pdl(k_bin_scan, 1, kBinThreads, 0, s, ip, n_tiles);
+    launch_pdl(k_bin_downsweep, n_tiles, kBinThreads, 0, s, ip);
+}
+
+void launch_shadow_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip)
+{
+    if (ip.n) k_shadow_inst_scatter<<<(ip.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, ip);
 }
 
 } // namespace fyx

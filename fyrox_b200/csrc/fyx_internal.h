@@ -26,6 +26,32 @@ constexpr uint32_t F_ROOT = 1u << 14;       // Graph::root
 constexpr int kCountStride = 32; // u32s between per-frustum counters (128 B: one L2 line each)
 constexpr int kBlock = 256;
 
+// ------------------------------------------------------------------------------------------------
+// Programmatic dependent launch: the kernels of a frame form a chain of true data dependencies (level l
+// needs level l-1, the fold needs every level, the palettes the bones, the skinning the palettes), several
+// of them tiny.  Each is launched with programmatic stream serialization: it lets the next kernel's CTAs be
+// scheduled right away (pdl_trigger) and waits for the previous kernel's results only where it first needs
+// them (pdl_wait) — launch latency and the loads that do not depend on the predecessor overlap its tail.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+
+template <class... Params, class... Args>
+static void launch_pdl(void (*kernel)(Params...), unsigned grid, unsigned block, size_t smem, cudaStream_t s, Args... args)
+{
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(block);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, kernel, static_cast<Params>(args)...);
+}
+
 struct NodeArrays {
     uint32_t cap; // number of slots (alive nodes)
     uint32_t *parent;
@@ -153,10 +179,27 @@ struct InstParams {
     float4 *o_mats;                 // 8 float4 per instance: world (4 columns), view_projection * world (4 columns)
     fyx_bundle *o_bundles;
     uint32_t *o_n_bundles;
+    // ---- segments (fyx_pack_shadow_instances): the list is the entries of shadow maps [map0, map0 + n_seg), each map one
+    // segment with its own observer; bin = segment * n_bundle_ids + bundle.  vis_node / vis_slot / tmp_sort start at the
+    // group's first entry, `n` counts the group's entries.
+    const fyx_shadow_map *maps;     // all maps of the shadow cull (first / count, view_projection)
+    const float *views;             // [maps * 16] the maps' view matrices
+    uint32_t map0, n_seg;
+    uint32_t base_inst, base_bundle; // instances and bundles of the groups packed before this one
+    uint32_t *seg_inst;             // [n_seg] instances per segment (keys pass, cleared by the caller)
+    uint32_t *seg_first;            // [n_seg] first instance of the segment (all groups)
+    uint32_t *seg_bfirst;           // [n_seg] first bundle of the segment (all groups)
+    uint2 *tile_sum;                // [tiles] (instances, bundles) per tile of kScanTile bins, then their exclusive prefix
+    uint32_t *o_totals;             // [2] the group's bundles and instances
 };
 void launch_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip);   // keys + scan: o_n_bundles[0] = bundles, [2] = instances
 void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip);
+// the same three steps over the shadow maps of one group: keys, the device-wide scan of the bins, scatter
+constexpr uint32_t kScanTile = 4096; // bins per CTA of the device-wide scan
+void launch_shadow_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip);
+void launch_shadow_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip);
 void launch_bone_block_index(cudaStream_t s, uint32_t n, const uint32_t *inst_skin, uint32_t *block_of_inst, uint32_t *counter);
+// one CTA per block; inst_skin / block_of_inst nullptr = block i is surface i's
 void launch_bone_blocks(cudaStream_t s, uint32_t n, const uint32_t *inst_skin, const uint2 *surf_bones, const float *palette, const uint32_t *block_of_inst,
                         float *blocks);
 
@@ -205,12 +248,14 @@ struct ShadowParams {
     fyx_frustum *scratch; // [max maps] the map frusta as planes + corners
     FrustumDev *frusta;   // [max maps]
     fyx_shadow_map *maps; // [max maps]
+    float *views;         // [max maps * 16] the maps' view matrices (look_at_rh), for fyx_pack_shadow_instances
     uint32_t *n_maps;     // one u32
     // node pass: per-map counts (each on its own 128 B line), then the lists
     uint32_t *counts;     // [max maps * kCountStride]
     uint32_t *warp_any;   // [warps]: the warp's nodes are in at least one map (written by the count pass, read by the emit pass)
     uint32_t *total;      // one u32: entries of all maps
     uint32_t *entries;    // [total], sized by the host from the count pass
+    uint32_t *entry_slot; // [total] the same entries as HBM slots; nullptr unless fyx_enable_instances
 };
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp); // map table + frusta, count pass, scan
 void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);

@@ -48,32 +48,6 @@ __device__ __forceinline__ void st_stream(float2 *p, const float2 v)
 }
 
 // ------------------------------------------------------------------------------------------------
-// Programmatic dependent launch: the kernels of a frame form a chain of true data dependencies (level l
-// needs level l-1, the fold needs every level, the palettes the bones, the skinning the palettes), several
-// of them tiny.  Each is launched with programmatic stream serialization: it lets the next kernel's CTAs be
-// scheduled right away (pdl_trigger) and waits for the previous kernel's results only where it first needs
-// them (pdl_wait) — launch latency and the loads that do not depend on the predecessor overlap its tail.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-template <class... Params, class... Args>
-static void launch_pdl(void (*kernel)(Params...), unsigned grid, unsigned block, size_t smem, cudaStream_t s, Args... args)
-{
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(block);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = s;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    cudaLaunchKernelEx(&cfg, kernel, static_cast<Params>(args)...);
-}
-
-// ------------------------------------------------------------------------------------------------
 // NodeTrait::should_be_rendered (scene/node/mod.rs:231-256) + the shadow-pass cast_shadows test of
 // Mesh::collect_render_data (scene/mesh/mod.rs:696-698) + reachability from Graph::root
 // (iterate_recursive, renderer/bundle.rs:988-1004), for every frustum of the call.  Bit f of the
@@ -1462,6 +1436,7 @@ __device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uin
     o.first = 0u;
     o.count = 0u;
     for (int k = 0; k < 16; ++k) o.view_projection[k] = VP[k];
+    for (int k = 0; k < 16; ++k) sp.views[(size_t)m * 16 + k] = V[k]; // the observer's view_matrix of the map's instances
     if (frustum_from_view_projection(VP, sp.scratch[m])) to_dev_frustum(sp.scratch[m], sp.cam.cam_mask, FYX_PASS_SHADOW, sp.frusta[m]);
     else sp.frusta[m] = sp.fallback;
 }
@@ -1648,7 +1623,7 @@ __global__ void __launch_bounds__(1024) k_shadow_scan(const ShadowParams sp)
     if (tid == 0) *sp.total = s_base;
 }
 
-// pass 3: the warps that had an entry test again and write their node indices
+// pass 3: the warps that had an entry test again and write their node indices (and, with instances enabled, their slots)
 __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const ShadowParams sp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
@@ -1681,7 +1656,10 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
         uint32_t at = 0u;
         if (lane == 0u) at = atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
         at = __shfl_sync(0xFFFFFFFFu, at, 0);
-        if (ok) sp.entries[at + __popc(b & lt)] = gi;
+        if (ok) {
+            sp.entries[at + __popc(b & lt)] = gi;
+            if (sp.entry_slot) sp.entry_slot[at + __popc(b & lt)] = slot;
+        }
     }
 }
 

@@ -263,7 +263,8 @@ int32_t fyx_get_visible_lights(fyx_ctx *ctx, uint32_t frustum, const uint32_t **
  * One pass over the nodes tests every map; list memory grows with the visible entries.  Synchronous.
  * Not modelled: directional lights and cascaded shadow maps (shadow/csm.rs: they need the camera's projection and the
  * frame size — cull those frusta with fyx_cull and FYX_PASS_SHADOW), light occlusion queries
- * (use_light_occlusion_culling = false), shadow alpha and other shading-only values, instance packing of the lists.
+ * (use_light_occlusion_culling = false), shadow alpha and other shading-only values.  The lists' instances: made with
+ * fyx_enable_instances, the cull also records each entry's slot for fyx_pack_shadow_instances.
  * Returns FYX_ERR_STATE when no cull has been made, a frame is still in flight, LOD ranges with observers are active or a
  * node carries FYX_NODE_STATIC_BATCH (the per-map LOD filter and static-batch pruning are not modelled: the call refuses
  * rather than give a different set), or the context is sharded (fyx_comm_init); FYX_ERR_INVALID_ARGUMENT when
@@ -536,6 +537,34 @@ int32_t fyx_pack_bone_matrices(fyx_ctx *ctx, uint32_t frustum);
 int32_t fyx_get_bone_matrix_blocks_device(fyx_ctx *ctx, uint32_t frustum, fyx_bone_blocks *out);
 /* Host copy of one instance's block (out_255x16 may be NULL to ask only whether it has one). */
 int32_t fyx_get_bone_matrix_block(fyx_ctx *ctx, uint32_t frustum, uint32_t instance, float *out_255x16, uint32_t *out_has_block);
+
+/* The same packing for every shadow map of the last fyx_cull_shadow_casters, in one call (the reference builds a whole
+ * RenderDataBundleStorage::from_graph per map, renderer/shadow/spot.rs:142-159, shadow/point.rs:173-197).  Map m is packed
+ * exactly as fyx_pack_instances packs a frustum for an observer whose view_matrix is the map's look_at_rh (spot or cube
+ * face) and whose view_projection is maps[m].view_projection: one instance per (listed node, surface), grouped by bundle id,
+ * bundle sort index by the fyx_set_dfs_order rule.  The shadow cull must have been made with fyx_enable_instances (it then
+ * records each entry's slot, 4 bytes per entry).  The instances of all maps live in one packed array: the fyx_instances of
+ * map m points at its part, and bundles[k].first counts from the map's first instance.  Synchronous; a fixed number of
+ * launches per group of consecutive maps whose (map, bundle id) bins stay under 2^25 (one group unless the id space is huge).
+ * FYX_ERR_STATE when there is no shadow cull, it was made without fyx_enable_instances, fyx_set_topology has run since it
+ * (its slots are stale) or a frame is still in flight. */
+int32_t fyx_pack_shadow_instances(fyx_ctx *ctx);
+/* Result of the last fyx_pack_shadow_instances for map `map` (FYX_ERR_INVALID_ARGUMENT when map >= the map count): pinned host
+ * copies of the map's part, valid until the next call of this function ... */
+int32_t fyx_get_shadow_instances(fyx_ctx *ctx, uint32_t map, fyx_instances *out);
+/* ... or pointers into the device arrays. */
+int32_t fyx_get_shadow_instances_device(fyx_ctx *ctx, uint32_t map, fyx_instances *out);
+/* [count] ordinal of each of the map's instances' surface within its node (host copy, valid until the next call). */
+int32_t fyx_get_shadow_instance_surfaces(fyx_ctx *ctx, uint32_t map, const uint32_t **out_ordinal);
+/* Bone matrices of the shadow instances.  Unlike write_uniforms, which copies a surface's palette into every instance that
+ * uses it (16 320 bytes per instance), there is ONE block per fyx surface (fyx_add_skinned_surface): block s is surface s's
+ * palette of the last fyx_build_palettes / fyx_render_prep followed by zero matrices, bit for bit the block write_uniforms
+ * builds (renderer/bundle.rs:484-496).  In the fyx_bone_blocks of a map, block_of_instance[i] is the id of the surface that
+ * skins instance i (FYX_NONE = unskinned) and n_blocks is the number of surfaces.  FYX_ERR_STATE before
+ * fyx_pack_shadow_instances (and, for the getters, before this call). */
+int32_t fyx_pack_shadow_bone_matrices(fyx_ctx *ctx);
+int32_t fyx_get_shadow_bone_matrix_blocks_device(fyx_ctx *ctx, uint32_t map, fyx_bone_blocks *out);
+int32_t fyx_get_shadow_bone_matrix_block(fyx_ctx *ctx, uint32_t map, uint32_t instance, float *out_255x16, uint32_t *out_has_block);
 
 /* ---- multi-GPU: one context per GPU, one process per GPU ------------------------------------- */
 /* The node array is sharded (sub-trees + replicated ancestors, SURVEY §8e); each context culls its
