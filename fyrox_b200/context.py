@@ -450,10 +450,13 @@ class Context:
         self._chk(self._lib.fyx_set_node_surfaces(self._h, len(idx), _ptr(idx), _ptr(first), ba.ctypes.data_as(C.c_void_p) if ba.size else None,
                                                   sa.ctypes.data_as(C.c_void_p) if sa.size else None))
 
-    def get_instance_surfaces(self, frustum: int, count: int) -> np.ndarray:
+    def _instance_surfaces(self, fn, index: int, count: int) -> np.ndarray:
         p = L.u32p()
-        self._chk(self._lib.fyx_get_instance_surfaces(self._h, frustum, C.byref(p)))
+        self._chk(fn(self._h, index, C.byref(p)))
         return np.ctypeslib.as_array(p, shape=(count,)).copy() if count else np.empty(0, np.uint32)
+
+    def get_instance_surfaces(self, frustum: int, count: int) -> np.ndarray:
+        return self._instance_surfaces(self._lib.fyx_get_instance_surfaces, frustum, count)
 
     def enable_instances(self, enable: bool = True):
         self._chk(self._lib.fyx_enable_instances(self._h, 1 if enable else 0))
@@ -493,12 +496,15 @@ class Context:
         """Bone-matrix blocks (255 mat4, zero padded) of the skinned instances of the last pack_instances (bundle.rs:484-496)."""
         self._chk(self._lib.fyx_pack_bone_matrices(self._h, frustum))
 
-    def get_bone_matrix_block(self, frustum: int, instance: int):
-        """(255,16) f32 block of packed instance `instance`, or None for an unskinned instance."""
+    def _bone_matrix_block(self, fn, index: int, instance: int):
         out = np.empty((255, 16), dtype=np.float32)
         has = C.c_uint32()
-        self._chk(self._lib.fyx_get_bone_matrix_block(self._h, frustum, instance, out.ctypes.data_as(C.c_void_p), C.byref(has)))
+        self._chk(fn(self._h, index, instance, out.ctypes.data_as(C.c_void_p), C.byref(has)))
         return out if has.value else None
+
+    def get_bone_matrix_block(self, frustum: int, instance: int):
+        """(255,16) f32 block of packed instance `instance`, or None for an unskinned instance."""
+        return self._bone_matrix_block(self._lib.fyx_get_bone_matrix_block, frustum, instance)
 
     def pack_shadow_instances(self):
         """Pack the instances of every shadow map of the last cull_shadow_casters (made with enable_instances) in one call;
@@ -510,10 +516,7 @@ class Context:
         view_projection).  bundles["first"] counts from the map's first instance."""
         out = L.fyx_instances()
         self._chk(self._lib.fyx_get_shadow_instances(self._h, map, C.byref(out)))
-        p = L.u32p()
-        self._chk(self._lib.fyx_get_shadow_instance_surfaces(self._h, map, C.byref(p)))
-        surface = np.ctypeslib.as_array(p, shape=(out.count,)).copy() if out.count else np.empty(0, np.uint32)
-        return self._instances_dict(out, surface)
+        return self._instances_dict(out, self._instance_surfaces(self._lib.fyx_get_shadow_instance_surfaces, map, out.count))
 
     def pack_shadow_bone_matrices(self):
         """One bone-matrix block (255 mat4, zero padded) per skinned surface, for the last pack_shadow_instances."""
@@ -521,10 +524,7 @@ class Context:
 
     def get_shadow_bone_matrix_block(self, map: int, instance: int):
         """(255,16) f32 block of instance `instance` of shadow map `map`, or None for an unskinned instance."""
-        out = np.empty((255, 16), dtype=np.float32)
-        has = C.c_uint32()
-        self._chk(self._lib.fyx_get_shadow_bone_matrix_block(self._h, map, instance, out.ctypes.data_as(C.c_void_p), C.byref(has)))
-        return out if has.value else None
+        return self._bone_matrix_block(self._lib.fyx_get_shadow_bone_matrix_block, map, instance)
 
     def build_palettes(self):
         self._chk(self._lib.fyx_build_palettes(self._h))

@@ -216,17 +216,27 @@ struct AnimHost {
     AnimStateDev st{};
 };
 
-// N3: packed instances of one frustum (fyx_drawprep.inl)
-struct InstOut {
+// N3: packed instances in segments, segment after segment (fyx_drawprep.inl): one segment for a camera frustum, one per
+// map for the shadow maps
+struct InstPack {
     DevBuf b_node, b_sort, b_mats, b_bundles, b_surf, b_skin;
-    PinnedBuf h_surf;
-    uint32_t n_visible = 0;
-    DevBuf b_block_of, b_blocks; // bone-matrix blocks of the skinned instances (fyx_pack_bone_matrices)
+    DevBuf b_block_of, b_blocks; // bone-matrix blocks of the instances
+    std::vector<uint32_t> inst_first, bundle_first; // [segments + 1]
+    const uint32_t *block_of = nullptr;             // [instances] block of each instance: b_block_of, or b_skin (one block per surface)
     uint32_t n_blocks = 0;
-    bool blocks_valid = false;
-    PinnedBuf h[4];
-    uint32_t count = 0, n_bundles = 0;
-    bool valid = false, on_host = false;
+    // pinned host copies of one segment (node, sort, mats, bundles; surface ordinals) and the segment each holds
+    PinnedBuf h[4], h_surf;
+    uint32_t h_seg = FYX_NONE, h_surf_seg = FYX_NONE;
+    bool valid = false, blocks_valid = false;
+    uint32_t segments() const { return (uint32_t)inst_first.size() - 1; }
+};
+
+// Scratch of the instance packs, shared by all of them: per bin (histogram, first key, offset), per entry (sort index), per
+// segment (instances, first instance, first bundle), the device-wide scan's tile sums, and the totals with a pinned copy
+struct PackScratch {
+    DevBuf hist, first_key, offset, tmp_sort, seg, tiles, totals;
+    PinnedBuf h_totals;
+    int32_t ensure(fyx_ctx *c, size_t bins, size_t entries, size_t segments);
 };
 
 } // namespace
@@ -360,19 +370,18 @@ struct fyx_ctx {
     uint32_t sh_n_maps = 0, sh_total = 0;
     bool sh_valid = false, sh_on_host = false;
     // the shadow maps' instances (fyx_pack_shadow_instances): the shadow cull also records slots (with instances enabled)
-    // and view matrices; one packed InstOut for all maps, per map its instance and bundle ranges; bone blocks per surface
-    DevBuf b_sh_slots, b_sh_views, b_shi_seg, b_shi_tiles, b_shi_small;
+    // and view matrices; one pack for all maps, a segment per map; bone blocks per surface
+    DevBuf b_sh_slots, b_sh_views;
     bool sh_have_slots = false, sh_slots_stale = false;
-    InstOut shi;
-    std::vector<uint32_t> shi_inst_first, shi_bundle_first; // [maps + 1]
+    InstPack shi;
 
     // N3 draw-prep (fyx_drawprep.inl)
     bool instances_enabled = false, rank_on_device = false;
     uint32_t n_bundle_ids = 1;
     SlotColumn bundle{uint32_t(0)}; // bundle id per slot
-    DevBuf b_rank_slot, b_inst_hist, b_inst_first, b_inst_offset, b_inst_tmp, b_inst_nb;
-    PinnedBuf h_inst_nb;
-    InstOut inst[FYX_MAX_FRUSTA];
+    DevBuf b_rank_slot;
+    PackScratch pack;
+    InstPack inst[FYX_MAX_FRUSTA];
 
     // multi-GPU (fyx_comm.cu)
     void *comm = nullptr;

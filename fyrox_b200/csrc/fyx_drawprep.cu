@@ -159,8 +159,8 @@ __global__ void __launch_bounds__(kScanBlock) k_inst_scan(const InstParams ip)
         __syncthreads();
     }
     if (threadIdx.x == 0) {
-        ip.o_n_bundles[0] = s_carry[1];
-        ip.o_n_bundles[2] = s_carry[0]; // instances = sum of the histogram
+        ip.o_totals[0] = s_carry[1];
+        ip.o_totals[1] = s_carry[0]; // instances = sum of the histogram
     }
 }
 
@@ -447,30 +447,28 @@ void launch_bone_blocks(cudaStream_t s, uint32_t n, const uint32_t *inst_skin, c
     if (n) k_bone_blocks<<<n, kBlock, 0, s>>>(inst_skin, surf_bones, reinterpret_cast<const float4 *>(palette), block_of_inst, reinterpret_cast<float4 *>(blocks));
 }
 
-void launch_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip)
+// the scratch is cleared by the caller: hist 0, first_key ~0 (segmented: seg_inst 0)
+void launch_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip, bool segmented)
 {
-    if (ip.n) k_inst_keys<<<(ip.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, ip);
-    k_inst_scan<<<1, kScanBlock, 0, s>>>(ip);
-}
-
-void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip)
-{
-    if (ip.n) k_inst_scatter<<<(ip.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, ip);
-}
-
-// the scratch is cleared by the caller: hist 0, first_key ~0, seg_inst 0
-void launch_shadow_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip)
-{
+    const unsigned grid = (ip.n + kBlock - 1) / kBlock;
+    if (!segmented) {
+        if (ip.n) k_inst_keys<<<grid, kBlock, 0, s>>>(a, ip);
+        k_inst_scan<<<1, kScanBlock, 0, s>>>(ip);
+        return;
+    }
     const uint32_t n_tiles = (ip.n_seg * ip.n_bundle_ids + kScanTile - 1) / kScanTile;
-    if (ip.n) k_shadow_inst_keys<<<(ip.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, ip);
+    if (ip.n) k_shadow_inst_keys<<<grid, kBlock, 0, s>>>(a, ip);
     launch_pdl(k_bin_reduce, n_tiles, kBinThreads, 0, s, ip);
     launch_pdl(k_bin_scan, 1, kBinThreads, 0, s, ip, n_tiles);
     launch_pdl(k_bin_downsweep, n_tiles, kBinThreads, 0, s, ip);
 }
 
-void launch_shadow_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip)
+void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip, bool segmented)
 {
-    if (ip.n) k_shadow_inst_scatter<<<(ip.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, ip);
+    if (!ip.n) return;
+    const unsigned grid = (ip.n + kBlock - 1) / kBlock;
+    if (segmented) k_shadow_inst_scatter<<<grid, kBlock, 0, s>>>(a, ip);
+    else k_inst_scatter<<<grid, kBlock, 0, s>>>(a, ip);
 }
 
 } // namespace fyx

@@ -178,7 +178,7 @@ struct InstParams {
     uint32_t *o_skin;               // fyx surface id whose palette skins the instance, FYX_NONE = unskinned
     float4 *o_mats;                 // 8 float4 per instance: world (4 columns), view_projection * world (4 columns)
     fyx_bundle *o_bundles;
-    uint32_t *o_n_bundles;
+    uint32_t *o_totals;             // [2] bundles and instances (of the group)
     // ---- segments (fyx_pack_shadow_instances): the list is the entries of shadow maps [map0, map0 + n_seg), each map one
     // segment with its own observer; bin = segment * n_bundle_ids + bundle.  vis_node / vis_slot / tmp_sort start at the
     // group's first entry, `n` counts the group's entries.
@@ -190,14 +190,12 @@ struct InstParams {
     uint32_t *seg_first;            // [n_seg] first instance of the segment (all groups)
     uint32_t *seg_bfirst;           // [n_seg] first bundle of the segment (all groups)
     uint2 *tile_sum;                // [tiles] (instances, bundles) per tile of kScanTile bins, then their exclusive prefix
-    uint32_t *o_totals;             // [2] the group's bundles and instances
 };
-void launch_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip);   // keys + scan: o_n_bundles[0] = bundles, [2] = instances
-void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip);
-// the same three steps over the shadow maps of one group: keys, the device-wide scan of the bins, scatter
+// keys + scan (o_totals), then the scatter.  One segment: the one-CTA scan; segmented (the shadow maps of one group): the
+// device-wide scan of the bins
 constexpr uint32_t kScanTile = 4096; // bins per CTA of the device-wide scan
-void launch_shadow_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip);
-void launch_shadow_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip);
+void launch_inst_count(cudaStream_t s, const NodeArrays &a, const InstParams &ip, bool segmented);
+void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &ip, bool segmented);
 void launch_bone_block_index(cudaStream_t s, uint32_t n, const uint32_t *inst_skin, uint32_t *block_of_inst, uint32_t *counter);
 // one CTA per block; inst_skin / block_of_inst nullptr = block i is surface i's
 void launch_bone_blocks(cudaStream_t s, uint32_t n, const uint32_t *inst_skin, const uint2 *surf_bones, const float *palette, const uint32_t *block_of_inst,

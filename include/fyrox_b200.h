@@ -550,11 +550,12 @@ int32_t fyx_get_bone_matrix_block(fyx_ctx *ctx, uint32_t frustum, uint32_t insta
  * (its slots are stale) or a frame is still in flight. */
 int32_t fyx_pack_shadow_instances(fyx_ctx *ctx);
 /* Result of the last fyx_pack_shadow_instances for map `map` (FYX_ERR_INVALID_ARGUMENT when map >= the map count): pinned host
- * copies of the map's part, valid until the next call of this function ... */
+ * copies of the map's part, valid until the next host getter call on the same pack, or the next pack ... */
 int32_t fyx_get_shadow_instances(fyx_ctx *ctx, uint32_t map, fyx_instances *out);
 /* ... or pointers into the device arrays. */
 int32_t fyx_get_shadow_instances_device(fyx_ctx *ctx, uint32_t map, fyx_instances *out);
-/* [count] ordinal of each of the map's instances' surface within its node (host copy, valid until the next call). */
+/* [count] ordinal of each of the map's instances' surface within its node (host copy, valid until the next host getter call on
+ * the same pack, or the next pack). */
 int32_t fyx_get_shadow_instance_surfaces(fyx_ctx *ctx, uint32_t map, const uint32_t **out_ordinal);
 /* Bone matrices of the shadow instances.  Unlike write_uniforms, which copies a surface's palette into every instance that
  * uses it (16 320 bytes per instance), there is ONE block per fyx surface (fyx_add_skinned_surface): block s is surface s's
