@@ -179,6 +179,18 @@ class fyx_shadow_map(C.Structure):
                 ("view_projection", C.c_float * 16)]
 
 
+PROJECTION_PERSPECTIVE, PROJECTION_ORTHOGRAPHIC = 0, 1
+
+
+class fyx_csm_options(C.Structure):
+    _fields_ = [("relative", C.c_uint32), ("splits", C.c_float * 3)]
+
+
+class fyx_csm_camera(C.Structure):
+    _fields_ = [("projection", C.c_uint32), ("fov_or_vertical_size", C.c_float), ("z_near", C.c_float), ("z_far", C.c_float),
+                ("frame_size", C.c_float * 2), ("view_matrix", C.c_float * 16), ("csm_enabled", C.c_uint32)]
+
+
 # every symbol include/fyrox_b200.h declares: name -> (restype, argtypes)
 ctx_p = C.c_void_p
 SYMBOLS = {
@@ -219,6 +231,8 @@ SYMBOLS = {
     "fyx_get_visible_lights": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(u32p), u32p]),
     "fyx_set_light_sources": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     "fyx_cull_shadow_casters": (C.c_int32, [ctx_p, C.c_uint32, f32p, C.POINTER(fyx_shadow_settings)]),
+    "fyx_set_csm_options": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "fyx_cull_shadow_casters_csm": (C.c_int32, [ctx_p, C.c_uint32, f32p, C.POINTER(fyx_shadow_settings), C.POINTER(fyx_csm_camera)]),
     "fyx_get_shadow_maps": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p)]),
     "fyx_get_shadow_maps_device": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p)]),
     "fyx_build_palettes": (C.c_int32, [ctx_p]),

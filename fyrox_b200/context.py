@@ -340,14 +340,44 @@ class Context:
         ix = _u32(idx)
         self._chk(self._lib.fyx_set_light_sources(self._h, src.size, _ptr(ix), src.ctypes.data_as(C.c_void_p)))
 
+    CSM_OPTIONS_DTYPE = np.dtype([("relative", "<u4"), ("splits", "<f4", 3)])
+
+    def set_csm_options(self, options, idx=None):
+        """FrustumSplitOptions per directional light node (CSM_OPTIONS_DTYPE: relative 0 = Absolute far planes, 1 = Relative
+        fractions; splits).  Nodes without a record use Absolute {5, 25, 64}."""
+        opt = np.ascontiguousarray(options, dtype=self.CSM_OPTIONS_DTYPE)
+        ix = _u32(idx)
+        self._chk(self._lib.fyx_set_csm_options(self._h, opt.size, _ptr(ix), opt.ctypes.data_as(C.c_void_p)))
+
+    @staticmethod
+    def csm_camera(view_matrix, frame_size, z_near: float, z_far: float, fov: float | None = None, vertical_size: float | None = None,
+                   csm_enabled: bool = True):
+        """The camera of the cascaded shadow maps: a perspective projection (fov in radians) or an orthographic one
+        (vertical_size), its own z_near / z_far, Camera::view_matrix and the frame size the cascades are rendered for."""
+        if (fov is None) == (vertical_size is None):
+            raise ValueError("give exactly one of fov (perspective) and vertical_size (orthographic)")
+        cam = L.fyx_csm_camera()
+        cam.projection = L.PROJECTION_PERSPECTIVE if fov is not None else L.PROJECTION_ORTHOGRAPHIC
+        cam.fov_or_vertical_size = float(fov if fov is not None else vertical_size)
+        cam.z_near, cam.z_far = float(z_near), float(z_far)
+        cam.frame_size[:] = [float(v) for v in frame_size]
+        cam.view_matrix[:] = [float(v) for v in np.asarray(view_matrix, np.float32).reshape(16)]
+        cam.csm_enabled = int(bool(csm_enabled))
+        return cam
+
     def cull_shadow_casters(self, camera_frustum: int, camera_translation, spot_shadows_distance: float = 10.0, point_shadows_distance: float = 10.0,
-                            spot_shadows_enabled: bool = True, point_shadows_enabled: bool = True):
-        """The spot and point shadow maps the deferred light renderer draws for frustum `camera_frustum` of the last cull, and
-        their visible sets (renderer/light.rs:509-606, 695-763).  Defaults are QualitySettings::default() (renderer/settings.rs)."""
+                            spot_shadows_enabled: bool = True, point_shadows_enabled: bool = True, csm_camera=None):
+        """The shadow maps the deferred light renderer draws for frustum `camera_frustum` of the last cull, and their visible
+        sets (renderer/light.rs:509-606, 695-782).  Defaults are QualitySettings::default() (renderer/settings.rs).  Spot and
+        point maps always; the cascades of directional lights (renderer/shadow/csm.rs) when `csm_camera` (Context.csm_camera
+        or an fyx_csm_camera) is given, through fyx_cull_shadow_casters_csm."""
         t = _f32(camera_translation)
         st = L.fyx_shadow_settings(float(spot_shadows_distance), float(point_shadows_distance), int(bool(spot_shadows_enabled)),
                                    int(bool(point_shadows_enabled)))
-        self._chk(self._lib.fyx_cull_shadow_casters(self._h, camera_frustum, t.ctypes.data_as(L.f32p), C.byref(st)))
+        if csm_camera is None:
+            self._chk(self._lib.fyx_cull_shadow_casters(self._h, camera_frustum, t.ctypes.data_as(L.f32p), C.byref(st)))
+        else:
+            self._chk(self._lib.fyx_cull_shadow_casters_csm(self._h, camera_frustum, t.ctypes.data_as(L.f32p), C.byref(st), C.byref(csm_camera)))
 
     def get_shadow_maps(self, copy: bool = True):
         """(maps, entries): maps is a SHADOW_MAP_DTYPE array; map k's visible set is entries[first:first + count].

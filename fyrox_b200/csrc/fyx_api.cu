@@ -362,6 +362,7 @@ struct fyx_ctx {
     // N4 shadow casters (fyx_drawprep.inl): light-source records by node index, their device table by pool order, the maps
     std::vector<fyx_light_source> light_src; // kind FYX_LIGHT_UNKNOWN = no record
     std::vector<float> light_m22;
+    std::vector<fyx_csm_options> csm_opts; // by node index; missing = FrustumSplitOptions::default()
     bool light_table_dirty = false;
     uint32_t n_light_table = 0;
     DevBuf b_light_table, b_sh_scratch, b_sh_frusta, b_sh_maps, b_sh_counts, b_sh_warp_any, b_sh_small, b_sh_entries;

@@ -183,15 +183,113 @@ __host__ __device__ __forceinline__ void look_at_rh(const float *eye, const floa
     out[3] = 0.0f; out[7] = 0.0f; out[11] = 0.0f; out[15] = 1.0f;
 }
 
-// Matrix4::new_perspective(1.0, fovy, znear, zfar) with m22 = 1 / tan(fovy / 2) given (nalgebra Perspective3::new)
-__host__ __device__ __forceinline__ void perspective_square(const float m22, const float znear, const float zfar, float *out)
+// Matrix4::new_perspective(aspect, fovy, znear, zfar) with m22 = 1 / tan(fovy / 2) given (nalgebra Perspective3::new)
+__host__ __device__ __forceinline__ void perspective(const float m22, const float aspect, const float znear, const float zfar, float *out)
 {
     for (int k = 0; k < 16; ++k) out[k] = 0.0f;
     out[5] = m22;
-    out[0] = m22 / 1.0f;
+    out[0] = m22 / aspect;
     out[10] = FYX_ADD(zfar, znear) / FYX_SUB(znear, zfar);
     out[14] = FYX_MUL(FYX_MUL(zfar, znear), 2.0f) / FYX_SUB(znear, zfar);
     out[11] = -1.0f;
+}
+
+// The cascaded shadow maps' math (renderer/shadow/csm.rs:165-249).  nalgebra and approx have no source in the reference
+// tree: look_at_lh, new_orthographic and relative_eq are restated from their documented definitions (unpinned), in the
+// order of the oracle's orc_look_at_rh / orc_orthographic.
+
+// Matrix4::new_orthographic(l, r, b, t, znear, zfar) (nalgebra Orthographic3::new; the oracle's orc_orthographic)
+__host__ __device__ __forceinline__ void orthographic(const float l, const float r, const float b, const float t, const float zn, const float zf,
+                                                      float *out)
+{
+    for (int k = 0; k < 16; ++k) out[k] = 0.0f;
+    out[0] = 2.0f / FYX_SUB(r, l);
+    out[5] = 2.0f / FYX_SUB(t, b);
+    out[10] = -2.0f / FYX_SUB(zf, zn);
+    out[12] = -FYX_ADD(r, l) / FYX_SUB(r, l);
+    out[13] = -FYX_ADD(t, b) / FYX_SUB(t, b);
+    out[14] = -FYX_ADD(zf, zn) / FYX_SUB(zf, zn);
+    out[15] = 1.0f;
+}
+
+// Matrix4::look_at_lh (nalgebra: IsometryMatrix3::look_at_lh = Rotation3::face_towards(target − eye, up) inverted, then the
+// rotation applied to −eye): rows s, u, f with f = normalize(target − eye), s = normalize(up × f), u = f × s
+__host__ __device__ __forceinline__ void look_at_lh(const float *eye, const float *target, const float *up, float *out)
+{
+    float f[3] = {FYX_SUB(target[0], eye[0]), FYX_SUB(target[1], eye[1]), FYX_SUB(target[2], eye[2])};
+    const float fl = sqrtf(dot3(f, f));
+    f[0] = f[0] / fl;
+    f[1] = f[1] / fl;
+    f[2] = f[2] / fl;
+    float s[3];
+    cross3(up, f, s);
+    const float sl = sqrtf(dot3(s, s));
+    s[0] = s[0] / sl;
+    s[1] = s[1] / sl;
+    s[2] = s[2] / sl;
+    float u[3];
+    cross3(f, s, u);
+    const float ne[3] = {-eye[0], -eye[1], -eye[2]};
+    out[0] = s[0]; out[4] = s[1]; out[8] = s[2]; out[12] = dot3(s, ne);
+    out[1] = u[0]; out[5] = u[1]; out[9] = u[2]; out[13] = dot3(u, ne);
+    out[2] = f[0]; out[6] = f[1]; out[10] = f[2]; out[14] = dot3(f, ne);
+    out[3] = 0.0f; out[7] = 0.0f; out[11] = 0.0f; out[15] = 1.0f;
+}
+
+// approx's relative_eq!(a, b) for f32 (epsilon = max_relative = f32::EPSILON)
+__host__ __device__ __forceinline__ bool relative_eq(const float a, const float b)
+{
+    constexpr float eps = 1.1920929e-07f;
+    if (a == b) return true;
+    if (isinf(a) || isinf(b)) return false;
+    const float d = fabsf(FYX_SUB(a, b));
+    if (d <= eps) return true;
+    const float aa = fabsf(a), ab = fabsf(b);
+    const float largest = ab > aa ? ab : aa;
+    return d <= FYX_MUL(largest, eps);
+}
+
+// Projection::with_z_near(zn).with_z_far(zf).matrix(frame_size) (scene/camera.rs:89-174).  Perspective: m22_or_vsize is
+// 1 / tan(fov / 2) (evaluated on the host); orthographic: vertical_size.
+__host__ __device__ __forceinline__ void camera_projection(const uint32_t kind, const float m22_or_vsize, const float z_near, const float z_far,
+                                                           const float w, const float h, float *out)
+{
+    constexpr float limit = 1.1920929e-06f; // 10 * f32::EPSILON
+    const float zn = fminf(z_far, z_near);
+    float zf = fmaxf(z_far, z_near);
+    if (FYX_SUB(zf, zn) < limit) zf = FYX_ADD(zf, limit);
+    const float aspect = fmaxf(w / h, limit);
+    if (kind == FYX_PROJECTION_PERSPECTIVE) {
+        perspective(m22_or_vsize, aspect, zn, zf, out);
+        return;
+    }
+    auto clamp_to_limit_signed = [](const float v) { return (v < 0.0f && -v < limit) ? -limit : (v >= 0.0f && v < limit) ? limit : v; };
+    const float vs = clamp_to_limit_signed(m22_or_vsize);
+    const float hs = clamp_to_limit_signed(FYX_MUL(aspect, vs));
+    orthographic(-hs, hs, -vs, vs, zn, zf, out);
+}
+
+// Frustum::center (fyrox-math/src/frustum.rs:197-202): the corners folded from Vector3::default(), scaled by 1/8
+__host__ __device__ __forceinline__ void frustum_center(const fyx_frustum &f, float *c)
+{
+    float a[3] = {0.0f, 0.0f, 0.0f};
+    for (int i = 0; i < 8; ++i)
+        for (int k = 0; k < 3; ++k) a[k] = FYX_ADD(a[k], f.corners[i][k]);
+    for (int k = 0; k < 3; ++k) c[k] = FYX_MUL(a[k], 0.125f);
+}
+
+// Matrix4::transform_point (the oracle's orc_mat4_transform_point): (M3x3 p + t) / n, n = row3 · p + m33, unless n == 0
+__host__ __device__ __forceinline__ void transform_point(const float *m, const float *p, float *out)
+{
+    const float n = FYX_ADD(FYX_ADD(FYX_ADD(FYX_MUL(m[3], p[0]), FYX_MUL(m[7], p[1])), FYX_MUL(m[11], p[2])), m[15]);
+    float t[3];
+    for (int i = 0; i < 3; ++i) t[i] = FYX_ADD(FYX_ADD(FYX_ADD(FYX_MUL(m[i], p[0]), FYX_MUL(m[4 + i], p[1])), FYX_MUL(m[8 + i], p[2])), m[12 + i]);
+    if (n != 0.0f) {
+        t[0] = t[0] / n;
+        t[1] = t[1] / n;
+        t[2] = t[2] / n;
+    }
+    out[0] = t[0]; out[1] = t[1]; out[2] = t[2];
 }
 
 } // namespace fyx

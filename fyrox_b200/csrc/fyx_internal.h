@@ -232,6 +232,17 @@ struct ShadowLightDev {
     uint32_t kind; // FYX_LIGHT_*
     float m22;     // 1 / tan(fovy / 2), evaluated on the host
     float distance_or_radius;
+    fyx_csm_options csm; // directional lights: the cascades' FrustumSplitOptions
+};
+// the camera of the cascaded shadow maps (fyx_cull_shadow_casters_csm); enabled = 0: directional lights get no maps
+struct CsmCameraDev {
+    uint32_t enabled;
+    uint32_t projection;        // FYX_PROJECTION_*
+    float m22_or_vertical_size; // perspective: 1 / tan(fov / 2), evaluated on the host; orthographic: vertical_size
+    float z_near, z_far;
+    float frame_size[2];
+    float view[16];
+    fyx_frustum fallback; // Frustum::default() as planes + corners: a cascade slice's unwrap_or_default (shadow/csm.rs:215-219)
 };
 struct ShadowParams {
     const ShadowLightDev *lights;
@@ -254,6 +265,7 @@ struct ShadowParams {
     uint32_t *total;      // one u32: entries of all maps
     uint32_t *entries;    // [total], sized by the host from the count pass
     uint32_t *entry_slot; // [total] the same entries as HBM slots; nullptr unless fyx_enable_instances
+    CsmCameraDev csm;     // last, so that the node passes' parameter offsets do not move
 };
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp); // map table + frusta, count pass, scan
 void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);

@@ -1400,9 +1400,10 @@ void launch_compact_gathered(cudaStream_t s, const uint32_t *pad, uint32_t maxc,
 }
 
 // ------------------------------------------------------------------------------------------------
-// N4 shadow casters (fyx_cull_shadow_casters): the shadow-map loop of the deferred light renderer (renderer/light.rs:509-606,
-// 695-763) and, for every map, the cull of RenderDataBundleStorage::from_graph in its shadow pass (renderer/shadow/spot.rs:142,
-// shadow/point.rs:162-180).  Pass 1 (one CTA) builds the map table; pass 2 reads every node once and counts its entries in
+// N4 shadow casters (fyx_cull_shadow_casters[_csm]): the shadow-map loop of the deferred light renderer (renderer/light.rs:509-606,
+// 695-782) and, for every map, the cull of RenderDataBundleStorage::from_graph in its shadow pass (renderer/shadow/spot.rs:142,
+// shadow/point.rs:162-180, shadow/csm.rs:251-265).  Pass 1 (one CTA) builds the map table: 1 map per spot light, 6 per
+// point light, 3 cascades per directional light; pass 2 reads every node once and counts its entries in
 // every map; a one-CTA scan places the lists; pass 3 re-tests the warps that had an entry and writes the lists.
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kShadowNeed = kNeedBits | FYX_NODE_CAST_SHADOWS;
@@ -1424,10 +1425,9 @@ __constant__ float c_face_up[6][3] = {{0.f, -1.f, 0.f}, {0.f, -1.f, 0.f}, {0.f, 
 
 // one map: view_projection = P · V, its frustum (Frustum::default if the matrix has none, renderer/bundle.rs:893-896)
 __device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uint32_t m, const uint32_t light, const uint32_t face, const uint32_t cascade,
-                               const float *P, const float *eye, const float *target, const float *up)
+                               const float *P, const float *V)
 {
-    float V[16], VP[16];
-    look_at_rh(eye, target, up, V);
+    float VP[16];
     mat4_mul(P, V, VP);
     fyx_shadow_map &o = sp.maps[m];
     o.light = light;
@@ -1439,6 +1439,43 @@ __device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uin
     for (int k = 0; k < 16; ++k) sp.views[(size_t)m * 16 + k] = V[k]; // the observer's view_matrix of the map's instances
     if (frustum_from_view_projection(VP, sp.scratch[m])) to_dev_frustum(sp.scratch[m], sp.cam.cam_mask, FYX_PASS_SHADOW, sp.frusta[m]);
     else sp.frusta[m] = sp.fallback;
+}
+
+// cascade i of a directional light (renderer/shadow/csm.rs:195-249): the light-space box around slice i of the camera
+// frustum.  V = the map's look_at_lh, P = its orthographic projection.
+__device__ __forceinline__ void csm_cascade(const CsmCameraDev &cam, const fyx_csm_options &opt, const uint32_t i, const float *light_dir,
+                                         const float *light_up, float *V, float *P)
+{
+    // csm.rs:181-194: z_values = [z_near, far planes] (Absolute) or [z_near, z_far * fractions] (Relative)
+    const float a = i == 0u ? cam.z_near : opt.relative ? FYX_MUL(cam.z_far, opt.splits[i - 1]) : opt.splits[i - 1];
+    const float b = opt.relative ? FYX_MUL(cam.z_far, opt.splits[i]) : opt.splits[i];
+    const float z_near = a;
+    float z_far = b;
+    // csm.rs:200-205: MIN_DEPTH_DELTA = 2 * f32::EPSILON
+    if (relative_eq(z_far, z_near)) z_far = FYX_ADD(z_far, FYX_MUL(2.3841858e-07f, z_near));
+    float M[16];
+    camera_projection(cam.projection, cam.m22_or_vertical_size, z_near, z_far, cam.frame_size[0], cam.frame_size[1], P);
+    mat4_mul(P, cam.view, M);
+    fyx_frustum fr;
+    if (!frustum_from_view_projection(M, fr)) fr = cam.fallback;
+    float c[3];
+    frustum_center(fr, c);
+    const float eye[3] = {FYX_ADD(c[0], light_dir[0]), FYX_ADD(c[1], light_dir[1]), FYX_ADD(c[2], light_dir[2])};
+    look_at_lh(eye, c, light_up, V);
+    // AxisAlignedBoundingBox::default + add_point of every light-space corner
+    float mn[3] = {3.40282347e+38f, 3.40282347e+38f, 3.40282347e+38f}, mx[3] = {-3.40282347e+38f, -3.40282347e+38f, -3.40282347e+38f};
+    for (int k = 0; k < 8; ++k) {
+        float t[3];
+        transform_point(V, fr.corners[k], t);
+        for (int q = 0; q < 3; ++q) {
+            if (t[q] < mn[q]) mn[q] = t[q];
+            if (t[q] > mx[q]) mx[q] = t[q];
+        }
+    }
+    // csm.rs:235-246: z_mult = 10
+    mn[2] = mn[2] < 0.0f ? FYX_MUL(mn[2], 10.0f) : mn[2] / 10.0f;
+    mx[2] = mx[2] < 0.0f ? mx[2] / 10.0f : FYX_MUL(mx[2], 10.0f);
+    orthographic(mn[0], mx[0], mn[1], mx[1], mn[2], mx[2], P);
 }
 
 __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, const ShadowParams sp)
@@ -1455,15 +1492,18 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
         const uint32_t i = base + tid;
         uint32_t n_maps = 0u, cascade = 0u, slot = 0u, kind = FYX_LIGHT_UNKNOWN;
         float pos[3] = {0.f, 0.f, 0.f}, upv[3] = {0.f, 0.f, 0.f}, lookv[3] = {0.f, 0.f, 0.f}, radius = 0.f, m22 = 0.f;
+        fyx_csm_options csm_opt{0u, {0.f, 0.f, 0.f}};
         if (i < sp.n_lights) {
             const ShadowLightDev L = sp.lights[i];
             slot = L.slot;
             kind = L.kind;
             m22 = L.m22;
+            csm_opt = L.csm;
             const uint32_t nf = a.flags[slot];
             // in the camera's light list (renderer/bundle.rs:926-974, as k_cull_lights)
             constexpr uint32_t need = FYX_NODE_ALIVE | FYX_NODE_LIGHT | FYX_NODE_GLOBAL_VISIBILITY | FYX_NODE_GLOBAL_ENABLED;
-            bool ok = (nf & need) == need && (kind == FYX_LIGHT_SPOT || kind == FYX_LIGHT_POINT);
+            const bool dir = kind == FYX_LIGHT_DIRECTIONAL;
+            bool ok = (nf & need) == need && (kind == FYX_LIGHT_SPOT || kind == FYX_LIGHT_POINT || (dir && sp.csm.enabled));
             if (ok) {
                 const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
                 ok = frustum_intersects_aabb(sp.cam, wx, wy, wz, kc, aabb_is_tame(wx, wy, wz));
@@ -1478,8 +1518,9 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
                 const float dist = sqrtf(dot3(d, d));
                 const bool spot = kind == FYX_LIGHT_SPOT;
                 const float sd = spot ? sp.spot_distance : sp.point_distance;
-                // light.rs:529-532, 547-549: cast_shadows && distance_to_camera <= shadows_distance && enabled
-                ok = (nf & FYX_NODE_CAST_SHADOWS) && dist <= sd && (spot ? sp.spot_enabled : sp.point_enabled);
+                // light.rs:529-532, 547-549: cast_shadows && distance_to_camera <= shadows_distance && enabled;
+                // light.rs:555-565 (directional): cast_shadows && csm_settings.enabled (checked above), raw radius f32::MAX
+                ok = (nf & FYX_NODE_CAST_SHADOWS) && (dir || (dist <= sd && (spot ? sp.spot_enabled : sp.point_enabled)));
                 // light.rs:570-572: max(local scale) * raw radius
                 float sx = 1.f, sy = 1.f, sz = 1.f;
                 if (sp.trs) {
@@ -1487,7 +1528,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
                     sy = sp.trs[slot].scale[1];
                     sz = sp.trs[slot].scale[2];
                 }
-                radius = FYX_MUL(fmaxf(fmaxf(sx, sy), sz), L.distance_or_radius);
+                radius = FYX_MUL(fmaxf(fmaxf(sx, sy), sz), dir ? 3.40282347e+38f : L.distance_or_radius);
                 // light.rs:585-587, Frustum::is_intersects_sphere (fyrox-math/src/frustum.rs:336-347)
                 bool sphere = true;
                 for (int p = 0; p < 6; ++p) {
@@ -1503,7 +1544,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
                 const float e[3] = {FYX_SUB(sp.cam_t[0], pos[0]), FYX_SUB(sp.cam_t[1], pos[1]), FYX_SUB(sp.cam_t[2], pos[2])};
                 const float metric = sqrtf(dot3(e, e));
                 cascade = (dist < b1 || metric <= radius) ? 0u : (dist > b1 && dist < b2) ? 1u : 2u;
-                n_maps = ok ? (spot ? 1u : 6u) : 0u;
+                n_maps = ok ? (dir ? 3u : spot ? 1u : 6u) : 0u;
             }
         }
         // ordered compaction: maps in light (pool) order
@@ -1519,23 +1560,38 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
         for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
         if (n_maps) {
             const uint32_t light = a.gidx[slot];
-            float P[16];
-            perspective_square(m22, 0.01f, radius, P); // z_near 0.01, z_far light_radius (light.rs:702-704, point.rs:167-170)
-            if (kind == FYX_LIGHT_SPOT) {
-                // light.rs:706-722: look_at_rh(pos, pos - emit_direction, look_vector normalised)
-                const float zdir[3] = {0.f, 0.f, 1.f}, ydir[3] = {0.f, 1.f, 0.f};
-                float emit[3], up[3];
-                try_normalize(upv, zdir, emit);
-                try_normalize(lookv, ydir, up);
-                const float target[3] = {FYX_SUB(pos[0], emit[0]), FYX_SUB(pos[1], emit[1]), FYX_SUB(pos[2], emit[2])};
-                shadow_map_out(sp, first, light, 0u, cascade, P, pos, target, up);
-            } else {
-                // shadow/point.rs:172-180: one map per cube face
+            const float zdir[3] = {0.f, 0.f, 1.f}, ydir[3] = {0.f, 1.f, 0.f};
+            float P[16], V[16];
+            if (kind == FYX_LIGHT_DIRECTIONAL) {
+                // shadow/csm.rs:170-179: light_direction = -up (normalised, else y), light_up = look (normalised, else z)
+                float dir[3], up[3];
+                try_normalize(upv, ydir, dir);
+                dir[0] = -dir[0]; dir[1] = -dir[1]; dir[2] = -dir[2];
+                try_normalize(lookv, zdir, up);
 #pragma unroll 1
-                for (uint32_t k = 0; k < 6u; ++k) {
-                    const float target[3] = {FYX_ADD(pos[0], c_face_look[k][0]), FYX_ADD(pos[1], c_face_look[k][1]), FYX_ADD(pos[2], c_face_look[k][2])};
-                    const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
-                    shadow_map_out(sp, first + k, light, k, cascade, P, pos, target, up);
+                for (uint32_t k = 0; k < 3u; ++k) {
+                    csm_cascade(sp.csm, csm_opt, k, dir, up, V, P);
+                    shadow_map_out(sp, first + k, light, 0u, k, P, V);
+                }
+            } else {
+                perspective(m22, 1.0f, 0.01f, radius, P); // z_near 0.01, z_far light_radius (light.rs:702-704, point.rs:167-170)
+                if (kind == FYX_LIGHT_SPOT) {
+                    // light.rs:706-722: look_at_rh(pos, pos - emit_direction, look_vector normalised)
+                    float emit[3], up[3];
+                    try_normalize(upv, zdir, emit);
+                    try_normalize(lookv, ydir, up);
+                    const float target[3] = {FYX_SUB(pos[0], emit[0]), FYX_SUB(pos[1], emit[1]), FYX_SUB(pos[2], emit[2])};
+                    look_at_rh(pos, target, up, V);
+                    shadow_map_out(sp, first, light, 0u, cascade, P, V);
+                } else {
+                    // shadow/point.rs:172-180: one map per cube face
+#pragma unroll 1
+                    for (uint32_t k = 0; k < 6u; ++k) {
+                        const float target[3] = {FYX_ADD(pos[0], c_face_look[k][0]), FYX_ADD(pos[1], c_face_look[k][1]), FYX_ADD(pos[2], c_face_look[k][2])};
+                        const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
+                        look_at_rh(pos, target, up, V);
+                        shadow_map_out(sp, first + k, light, k, cascade, P, V);
+                    }
                 }
             }
         }

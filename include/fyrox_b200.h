@@ -261,14 +261,31 @@ int32_t fyx_get_visible_lights(fyx_ctx *ctx, uint32_t frustum, const uint32_t **
  * look_at_rh(pos, pos + face.look, face.up); z_near 0.01, z_far light_radius) and the visible set of
  * from_graph(map frustum, cam_mask, shadow pass): alive, renderable, reachable, should_be_rendered and cast_shadows.
  * One pass over the nodes tests every map; list memory grows with the visible entries.  Synchronous.
- * Not modelled: directional lights and cascaded shadow maps (shadow/csm.rs: they need the camera's projection and the
- * frame size — cull those frusta with fyx_cull and FYX_PASS_SHADOW), light occlusion queries
- * (use_light_occlusion_culling = false), shadow alpha and other shading-only values.  The lists' instances: made with
+ * Directional lights get maps only through fyx_cull_shadow_casters_csm (below); fyx_cull_shadow_casters(..) is exactly
+ * fyx_cull_shadow_casters_csm(.., NULL).  Not modelled: light occlusion queries (use_light_occlusion_culling = false),
+ * shadow alpha, cascade distances, shadow bias and other shading-only values.  The lists' instances: made with
  * fyx_enable_instances, the cull also records each entry's slot for fyx_pack_shadow_instances.
  * Returns FYX_ERR_STATE when no cull has been made, a frame is still in flight, LOD ranges with observers are active or a
  * node carries FYX_NODE_STATIC_BATCH (the per-map LOD filter and static-batch pruning are not modelled: the call refuses
  * rather than give a different set), or the context is sharded (fyx_comm_init); FYX_ERR_INVALID_ARGUMENT when
- * camera_frustum is not a frustum of the last cull. */
+ * camera_frustum is not a frustum of the last cull.
+ *
+ * fyx_set_csm_options: the FrustumSplitOptions (scene/light/directional.rs:60-91) of `count` directional light nodes (idx
+ * NULL = nodes 0..count-1).  A node without a record uses the reference's default, Absolute {5, 25, 64}.  Carried over by
+ * fyx_set_topology with the node indices.  FYX_ERR_INVALID_ARGUMENT for a node out of range or `relative` other than 0 / 1.
+ *
+ * fyx_cull_shadow_casters_csm: fyx_cull_shadow_casters plus the cascaded shadow maps of the directional lights
+ * (renderer/shadow/csm.rs:165-277).  A directional light in the camera's light list gets maps when its node has
+ * FYX_NODE_CAST_SHADOWS, cam->csm_enabled is set and the camera frustum intersects the sphere (position, max(local scale)
+ * * f32::MAX) (light.rs:555-565); it then gets three maps in the light loop's pool order, face 0, cascade 0, 1, 2.  Cascade
+ * i splits the camera's depth range at z_values = [z_near, splits[0..3]] (Absolute) or [z_near, z_far * splits[k]]
+ * (Relative), builds the camera projection of that slice (scene/camera.rs:89-174) and its frustum (Frustum::default if
+ * it has none), and takes view_projection = new_orthographic(box) · look_at_lh(center − up/|up|, center, look/|look|), the box being
+ * the slice's corners in light space with its depth stretched ×10.  Its list is from_graph(map frustum, cam_mask, shadow
+ * pass), as for the spot and point maps; fyx_pack_shadow_instances sorts its instances by the map's look_at_lh.  The
+ * perspective's 1 / tan(fov / 2) is evaluated here with the platform's tanf.  cam NULL or csm_enabled = 0: directional
+ * lights get no maps.  Same refusals as fyx_cull_shadow_casters, plus FYX_ERR_INVALID_ARGUMENT for an unknown projection
+ * kind.  Inputs for which the reference panics (superimposed planes, a collapsed light-space box) give a defined result. */
 #define FYX_LIGHT_UNKNOWN 0u
 #define FYX_LIGHT_SPOT 1u
 #define FYX_LIGHT_POINT 2u
@@ -293,6 +310,23 @@ typedef struct fyx_shadow_map {
 } fyx_shadow_map;
 int32_t fyx_set_light_sources(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const fyx_light_source *src);
 int32_t fyx_cull_shadow_casters(fyx_ctx *ctx, uint32_t camera_frustum, const float camera_translation[3], const fyx_shadow_settings *settings);
+#define FYX_PROJECTION_PERSPECTIVE 0u
+#define FYX_PROJECTION_ORTHOGRAPHIC 1u
+typedef struct fyx_csm_options { /* FrustumSplitOptions */
+    uint32_t relative;           /* 0: Absolute { far_planes }, 1: Relative { fractions } */
+    float splits[3];
+} fyx_csm_options;
+typedef struct fyx_csm_camera {
+    uint32_t projection;         /* FYX_PROJECTION_* */
+    float fov_or_vertical_size;  /* PerspectiveProjection::fov (radians) or OrthographicProjection::vertical_size */
+    float z_near, z_far;         /* the projection's own values (ObserverPosition::from_camera, renderer/observer.rs:64-72) */
+    float frame_size[2];         /* the frame the cascades are rendered for: the G-buffer's width and height (light.rs:767) */
+    float view_matrix[16];       /* Camera::view_matrix, column-major */
+    uint32_t csm_enabled;        /* QualitySettings::csm_settings.enabled */
+} fyx_csm_camera;
+int32_t fyx_set_csm_options(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const fyx_csm_options *opts);
+int32_t fyx_cull_shadow_casters_csm(fyx_ctx *ctx, uint32_t camera_frustum, const float camera_translation[3], const fyx_shadow_settings *settings,
+                                    const fyx_csm_camera *cam);
 /* Result of the last fyx_cull_shadow_casters: pinned host copies ... */
 int32_t fyx_get_shadow_maps(fyx_ctx *ctx, const fyx_shadow_map **out_maps, uint32_t *out_n_maps, const uint32_t **out_entries);
 /* ... or the device arrays (*out_n_maps is a host value). */
