@@ -306,6 +306,8 @@ struct fyx_ctx {
     uint64_t vert_cap = 0;
     uint32_t n_entries = 0, entry_cap = 0;
     DevBuf b_vblk, b_opos, b_onrm, b_ib[3], b_palette, b_bone_slot, b_tiles;
+    DevBuf b_vflag;        // one byte per vertex block: raw or coded (fyx_vcode.cuh)
+    bool vblk_raw = false; // a palette of more than kSkinRingMaxBones bones was loaded: every block raw from then on
     // surfaces per node (fyx_set_node_surfaces): host CSR by node, device table by slot (rebuilt when dirty)
     std::vector<uint2> ms_of_node;       // (first, count) into ms_bundle_h / ms_skin_h; count 0 = default single surface
     std::vector<uint32_t> ms_bundle_h, ms_skin_h;
@@ -1199,9 +1201,11 @@ int32_t grow_vertex_streams(fyx_ctx *c, uint64_t need)
     int32_t rc;
     const uint64_t blocks = (need + 127) / 128 + 1; // 128-vertex blocks of 11 x 512 B
     if ((rc = dev_ensure(c, c->b_vblk, blocks * kVblkStride * sizeof(float4), true))) return rc;
+    if ((rc = dev_ensure(c, c->b_vflag, blocks, true))) return rc;
     if ((rc = dev_ensure(c, c->b_opos, need * 12, true))) return rc;
     if ((rc = dev_ensure(c, c->b_onrm, need * 12, true))) return rc;
-    c->vert_cap = std::min<uint64_t>({(c->b_vblk.bytes / (kVblkStride * sizeof(float4)) - 1) * 128, c->b_opos.bytes / 12, c->b_onrm.bytes / 12});
+    c->vert_cap = std::min<uint64_t>({(c->b_vblk.bytes / (kVblkStride * sizeof(float4)) - 1) * 128, (c->b_vflag.bytes - 1) * 128,
+                                      c->b_opos.bytes / 12, c->b_onrm.bytes / 12});
     return FYX_OK;
 }
 
@@ -1312,6 +1316,7 @@ int32_t commit_surfaces(fyx_ctx *c)
     CU(cudaStreamSynchronize(c->stream));
     if (!bone_slot.empty()) CU(cudaMemcpy(c->b_bone_slot.p, bone_slot.data(), bone_slot.size() * 4, cudaMemcpyHostToDevice));
     if (!tiles.empty()) CU(cudaMemcpy(c->b_tiles.p, tiles.data(), tiles.size() * sizeof(SkinTile), cudaMemcpyHostToDevice));
+    launch_tile_vcode(c->stream, c->b_tiles.as<SkinTile>(), (uint32_t)tiles.size(), c->b_vflag.as<uint8_t>());
     if (!fold_node.empty()) CU(cudaMemcpy(c->b_fold_node.p, fold_node.data(), fold_node.size() * 4, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(c->b_fold_begin.p, fold_begin.data(), fold_begin.size() * 4, cudaMemcpyHostToDevice));
     if (!fold_bone.empty()) CU(cudaMemcpy(c->b_fold_bone.p, fold_bone.data(), fold_bone.size() * 4, cudaMemcpyHostToDevice));
@@ -1400,8 +1405,12 @@ extern "C" int32_t fyx_add_skinned_surface(fyx_ctx *c, uint32_t mesh_node, uint3
     if (n_verts) {
         void *d_v = nullptr;
         if ((rc = stage_to_device(c, verts, (size_t)n_verts * layout->stride, nullptr, 0, false, &d_v, nullptr))) return rc;
-        launch_deinterleave(c->stream, n_verts, static_cast<const unsigned char *>(d_v), *layout, n_bones,
-                            c->b_vblk.as<float4>(), sf.vert_off, c->d_err.as<uint32_t>());
+        if (n_bones > kSkinRingMaxBones && !c->vblk_raw) { // k_skin's register-load form reads raw blocks
+            launch_vdecode_all(c->stream, c->b_vblk.as<float4>(), c->b_vflag.as<uint8_t>(), (c->n_verts_total + 127) / 128);
+            c->vblk_raw = true;
+        }
+        launch_deinterleave(c->stream, n_verts, static_cast<const unsigned char *>(d_v), *layout, n_bones, c->b_vblk.as<float4>(),
+                            c->b_vflag.as<uint8_t>(), !c->vblk_raw, sf.vert_off, c->d_err.as<uint32_t>());
         c->launches++;
     }
     CU(cudaGetLastError());

@@ -83,6 +83,7 @@ struct SkinArrays {
     //   rows 0-2 position x,y,z   rows 3-5 normal x,y,z   rows 6-9 weight 0..3   row 10 the 4x u8 bone indices;
     // element l of a row belongs to group l of the block and holds the value of its 4 vertices.  A warp reads
     // a row with one perfectly coalesced 512 B access and every 32 B sector exactly once (44 B/vertex).
+    // A block may instead hold the exact code of fyx_vcode.cuh (5 136 B at the same stride; SkinTile::vcoded).
     const float4 *vblk;
     float *opos, *onrm;        // skinned streams, packed xyz (each surface padded to a multiple of 4 vertices)
     // N4 blend shapes (optional): f16 position / normal offsets per (shape, vertex) in blocks of 128 vertices x 6 rows
@@ -102,7 +103,7 @@ struct SkinTile {
     uint32_t bs_blocks;   // 128-vertex blocks per shape
     uint32_t w_off;       // first weight in bs_w
     uint32_t local_quad0; // the tile's first group relative to the surface's first group
-    uint32_t pad[3];
+    uint32_t vcoded[3];   // bit s: block quad_start / 32 + s is coded (fyx_vcode.cuh); a tile spans at most 65 blocks
 };
 constexpr uint32_t kBsBlockU2 = 6 * 32; // uint2 per (shape, block)
 void launch_bs_layout(cudaStream_t s, uint32_t n_verts, uint32_t n_shapes, uint32_t layer_stride, const uint16_t *d_records, uint2 *d_dst, uint32_t bs_blocks);
@@ -294,8 +295,14 @@ void launch_gather_aabbs(cudaStream_t s, const NodeArrays &a, uint32_t count, co
                          const uint32_t *slot_of_node, uint32_t n_nodes, float *d_out6);
 void launch_gather_flags(cudaStream_t s, const NodeArrays &a, uint32_t count, const uint32_t *d_idx,
                          const uint32_t *slot_of_node, uint32_t n_nodes, uint32_t *d_out);
+// a surface's vertices into the raw blocks at first_vertex (a multiple of 4); with `code`, the blocks the load completes are
+// then coded where they fit (fyx_vcode.cuh; vflag: one byte per block)
 void launch_deinterleave(cudaStream_t s, uint32_t n_verts, const unsigned char *d_bytes, fyx_vertex_layout layout,
-                         uint32_t n_bones, float4 *vblk, uint64_t first_vertex, uint32_t *d_err);
+                         uint32_t n_bones, float4 *vblk, uint8_t *vflag, bool code, uint64_t first_vertex, uint32_t *d_err);
+// every coded block back to raw (a context whose palettes need the register-load form of k_skin, which reads raw blocks)
+void launch_vdecode_all(cudaStream_t s, float4 *vblk, uint8_t *vflag, uint64_t n_blocks);
+void launch_tile_vcode(cudaStream_t s, SkinTile *tiles, uint32_t n_tiles, const uint8_t *vflag); // SkinTile::vcoded
+constexpr uint32_t kSkinRingMaxBones = 64; // palettes up to this size: the prefetching form of k_skin, which reads coded blocks
 constexpr int kVblkRows = 11;                    // float4 rows per block
 constexpr int kVblkStride = kVblkRows * 32;      // float4 per block of 128 vertices
 void launch_ib_rows(cudaStream_t s, uint32_t n, const float *d_m16, float4 *r0, float4 *r1, float4 *r2, uint32_t *d_err);

@@ -8,6 +8,7 @@
 #include "fyx_frustum.cuh"
 #include "fyx_internal.h"
 #include "fyx_trs.cuh"
+#include "fyx_vcode.cuh"
 
 namespace fyx {
 
@@ -808,6 +809,28 @@ __device__ __forceinline__ void cp_async16(float4 *dst, const float4 *src)
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
+// a coded group as read from the ring (its 10 float4 and the block's header in iq) -> the raw rows
+__device__ __forceinline__ void decode_group(float4 &x4, float4 &y4, float4 &z4, float4 &nx4, float4 &ny4, float4 &nz4, float4 &w0, float4 &w1,
+                                             float4 &w2, float4 &w3, uint4 &iq)
+{
+    float4 *const rows[vcode::kRows] = {&x4, &y4, &z4, &nx4, &ny4, &nz4, &w0, &w1, &w2, &w3};
+    uint32_t w[vcode::kWords];
+#pragma unroll
+    for (int r = 0; r < vcode::kRows; ++r) {
+        w[4 * r + 0] = __float_as_uint(rows[r]->x);
+        w[4 * r + 1] = __float_as_uint(rows[r]->y);
+        w[4 * r + 2] = __float_as_uint(rows[r]->z);
+        w[4 * r + 3] = __float_as_uint(rows[r]->w);
+    }
+    const uint32_t h[3] = {iq.x, iq.y, iq.z};
+    float v[vcode::kRows][4];
+    uint32_t idx[4];
+    vcode::unpack_group(w, h, v, idx);
+#pragma unroll
+    for (int r = 0; r < vcode::kRows; ++r) *rows[r] = make_float4(v[r][0], v[r][1], v[r][2], v[r][3]);
+    iq = make_uint4(idx[0], idx[1], idx[2], idx[3]);
+}
+
 constexpr int kSkinStageF4 = 2 * 96;        // per warp: 128 skinned positions + 128 normals
 constexpr int kSkinRingF4 = kVblkRows * 32; // per warp: the next group of every lane, 11 rows x 32 lanes (5 632 B)
 // shared memory of k_skin: palette planes, output stages, and with PREFETCH the input ring
@@ -818,7 +841,8 @@ template <int S, int LOG2C, bool PREFETCH> constexpr size_t skin_smem_bytes()
 
 // One CTA per tile; a warp skins 32 consecutive groups (128 vertices) per step and writes them as full lines (store_lines).
 // PREFETCH: while group i is computed, group i + 1 of the same lane is already on its way into the warp's shared ring by
-// 11 cp.async.cg 16-byte copies; lane l only ever reads the 16-byte pieces it copied itself, so cp.async.wait_group is the
+// 11 cp.async.cg 16-byte copies (a coded block, fyx_vcode.cuh: the group's 10 float4 and the block's header, decoded in
+// registers after the reads); lane l only ever reads the 16-byte pieces it copied itself, so cp.async.wait_group is the
 // whole synchronisation (no mbarrier, no __syncwarp, no bank conflicts: a row of the ring is 32 consecutive float4).  The
 // first copies are issued before griddepcontrol.wait (the vertex blocks are static).  Without PREFETCH the inputs are loaded
 // straight into registers (LDG.128, L1-bypassing): the form for palettes too large to leave room for the ring at 2 CTAs/SM.
@@ -837,12 +861,19 @@ __global__ void __launch_bounds__(kBlock, MINB) k_skin(const SkinArrays sk, cons
     float4 *const stage = smem + PAL + warp * kSkinStageF4;
     float4 *const ring = smem + PAL + (kBlock / 32) * kSkinStageF4 + warp * kSkinRingF4 + lane; // this lane's column
     const uint32_t zero = __float_as_uint(negzero) << 1; // 0, but not a constant the compiler can fold
+    // the lane's block is coded (fyx_vcode.cuh): bit (block - the tile's first block) of the tile
+    auto coded_of = [&](const uint32_t q) {
+        const uint32_t s = ((T.quad_start + q) >> 5) - (T.quad_start >> 5);
+        return (((s < 32 ? T.vcoded[0] : s < 64 ? T.vcoded[1] : T.vcoded[2]) >> (s & 31u)) & 1u) != 0u;
+    };
     auto prefetch = [&](const uint32_t q, const uint32_t dep) {
         if (q < T.n_quads) {
             const size_t quad = (size_t)T.quad_start + q;
-            const float4 *row = sk.vblk + (quad >> 5) * kVblkStride + (quad & 31);
+            const float4 *blk = sk.vblk + (quad >> 5) * kVblkStride, *row = blk + (quad & 31);
 #pragma unroll
-            for (int r = 0; r < kVblkRows; ++r) cp_async16(ring + r * 32 + dep, row + r * 32);
+            for (int r = 0; r < vcode::kRows; ++r) cp_async16(ring + r * 32 + dep, row + r * 32);
+            // the 11th copy: the index row of a raw block, the header of a coded one
+            cp_async16(ring + 10 * 32 + dep, coded_of(q) ? blk + vcode::kHeaderF4 : row + 10 * 32);
         }
         cp_async_commit();
     };
@@ -870,6 +901,7 @@ __global__ void __launch_bounds__(kBlock, MINB) k_skin(const SkinArrays sk, cons
                                            __float_as_uint(ny4.x) ^ __float_as_uint(nz4.x) ^ __float_as_uint(w0.x) ^ __float_as_uint(w1.x) ^
                                            __float_as_uint(w2.x) ^ __float_as_uint(w3.x) ^ iq.x) & zero)
                                        : 0u;
+            if (valid && coded_of(q)) decode_group(x4, y4, z4, nx4, ny4, nz4, w0, w1, w2, w3, iq);
             prefetch(q + kBlock, dep);
         } else if (valid) {
             const float4 *row = sk.vblk + (quad >> 5) * kVblkStride + (quad & 31); // block, then this group's column
@@ -1103,6 +1135,58 @@ __global__ void __launch_bounds__(kBlock) k_deinterleave(const uint32_t n_verts,
     reinterpret_cast<uint32_t *>(blk)[10 * rs + j] = bi;
 }
 
+// The encode pass of a surface's load (fyx_vcode.cuh): one warp per block the load completes, coded in place where it fits.
+__global__ void __launch_bounds__(kBlock) k_vcode(float4 *vblk, uint8_t *vflag, const vcode::LoadBlocks lb)
+{
+    const uint64_t b = lb.first + (uint64_t)blockIdx.x * (kBlock / 32) + (threadIdx.x >> 5);
+    const uint32_t lane = threadIdx.x & 31u;
+    if (b >= lb.complete_end || vflag[b] != vcode::kVflagRaw) return;
+    if (vcode::encode_block_warp(reinterpret_cast<uint32_t *>(vblk + b * kVblkStride), lane) && lane == 0) vflag[b] = vcode::kVflagCoded;
+}
+
+// every coded block of [0, n_blocks) back to the raw layout, in place: one warp per block
+__global__ void __launch_bounds__(kBlock) k_vdecode_all(float4 *vblk, uint8_t *vflag, const uint64_t n_blocks)
+{
+    const uint64_t b = (uint64_t)blockIdx.x * (kBlock / 32) + (threadIdx.x >> 5);
+    const uint32_t lane = threadIdx.x & 31u;
+    if (b >= n_blocks || vflag[b] != vcode::kVflagCoded) return;
+    uint32_t *blk = reinterpret_cast<uint32_t *>(vblk + b * kVblkStride);
+    uint32_t raw[vcode::kRawF4 * 4 / vcode::kGroups]; // this group's 11 raw float4, gathered before any lane writes
+    const uint32_t h[3] = {blk[vcode::kHeaderF4 * 4], blk[vcode::kHeaderF4 * 4 + 1], blk[vcode::kHeaderF4 * 4 + 2]};
+    uint32_t w[vcode::kWords], idx[4];
+    float v[vcode::kRows][4];
+#pragma unroll
+    for (int r = 0; r < vcode::kRows; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) w[4 * r + c] = blk[(r * 32 + lane) * 4 + c];
+    vcode::unpack_group(w, h, v, idx);
+#pragma unroll
+    for (int r = 0; r < vcode::kRows; ++r)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) raw[4 * r + j] = __float_as_uint(v[r][j]);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) raw[40 + j] = idx[j];
+    __syncwarp(); // the header and every group are read before the raw rows overwrite them
+#pragma unroll
+    for (int r = 0; r < 11; ++r)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) blk[(r * 32 + lane) * 4 + j] = raw[4 * r + j];
+    if (lane == 0) vflag[b] = vcode::kVflagRaw;
+}
+
+// tile t's bit s: block (quad_start / 32) + s of the tile is coded
+__global__ void __launch_bounds__(kBlock) k_tile_vcode(SkinTile *tiles, const uint32_t n_tiles, const uint8_t *vflag)
+{
+    const uint32_t t = blockIdx.x * kBlock + threadIdx.x;
+    if (t >= n_tiles) return;
+    SkinTile &T = tiles[t];
+    const uint32_t b0 = T.quad_start >> 5, nb = ((T.quad_start + T.n_quads - 1) >> 5) - b0 + 1;
+    uint32_t m[3] = {0u, 0u, 0u};
+    for (uint32_t s = 0; s < nb; ++s)
+        if (vflag[b0 + s] == vcode::kVflagCoded) m[s >> 5] |= 1u << (s & 31);
+    for (int k = 0; k < 3; ++k) T.vcoded[k] = m[k];
+}
+
 __global__ void __launch_bounds__(kBlock) k_ib_rows(const uint32_t n, const float *d_m16, float4 *r0, float4 *r1, float4 *r2,
                                                     uint32_t *d_err)
 {
@@ -1297,6 +1381,7 @@ void launch_skin(cudaStream_t s, const SkinArrays &sk, const SkinTile *tiles, ui
     if (!n_tiles) return;
     // <= 64 bones: the prefetching form, 2 CTAs/SM (<= 128 registers; 25 KB palette + 24 KB output stages + 44 KB ring per CTA).
     // Larger palettes leave no room for the ring at 2 CTAs/SM: loads into registers, 3 CTAs/SM (<= 85 registers).
+    static_assert(kSkinRingMaxBones == 64, "the prefetching form (the one that reads coded blocks) holds 65 palette entries");
     if (max_bones <= 64) {       // 8 copies: 25 KB of palette planes
         launch_skin_t<65, 3, 2, true>(s, sk, tiles, n_tiles, blend_shapes);
     } else if (max_bones <= 128) { // 8 copies: 50 KB
@@ -1371,11 +1456,23 @@ void launch_gather_flags(cudaStream_t s, const NodeArrays &a, uint32_t count, co
 }
 
 void launch_deinterleave(cudaStream_t s, uint32_t n_verts, const unsigned char *d_bytes, fyx_vertex_layout layout,
-                         uint32_t n_bones, float4 *vblk, uint64_t first_vertex, uint32_t *d_err)
+                         uint32_t n_bones, float4 *vblk, uint8_t *vflag, bool code, uint64_t first_vertex, uint32_t *d_err)
 {
     const uint32_t n_padded = (n_verts + 3u) & ~3u;
     if (!n_padded) return;
     k_deinterleave<<<grid_for(n_padded), kBlock, 0, s>>>(n_verts, n_padded, d_bytes, layout, n_bones, vblk, first_vertex, d_err);
+    const vcode::LoadBlocks lb = vcode::load_blocks(first_vertex, n_padded);
+    if (code && lb.complete_end > lb.first) k_vcode<<<grid_for((lb.complete_end - lb.first) * 32), kBlock, 0, s>>>(vblk, vflag, lb);
+}
+
+void launch_vdecode_all(cudaStream_t s, float4 *vblk, uint8_t *vflag, uint64_t n_blocks)
+{
+    if (n_blocks) k_vdecode_all<<<grid_for(n_blocks * 32), kBlock, 0, s>>>(vblk, vflag, n_blocks);
+}
+
+void launch_tile_vcode(cudaStream_t s, SkinTile *tiles, uint32_t n_tiles, const uint8_t *vflag)
+{
+    if (n_tiles) k_tile_vcode<<<grid_for(n_tiles), kBlock, 0, s>>>(tiles, n_tiles, vflag);
 }
 
 void launch_ib_rows(cudaStream_t s, uint32_t n, const float *d_m16, float4 *r0, float4 *r1, float4 *r2, uint32_t *d_err)
