@@ -557,6 +557,22 @@ int32_t sync_and_check(fyx_ctx *c)
     return check_device_errors(c);
 }
 
+// The opening of every call that needs the scene: a context, and a topology (fyx_set_topology).  enter() also makes the
+// context's device current; calls that check their arguments before they touch CUDA call topology_check() instead.
+int32_t topology_check(fyx_ctx *c)
+{
+    if (!c) return FYX_ERR_INVALID_ARGUMENT;
+    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    return FYX_OK;
+}
+
+int32_t enter(fyx_ctx *c)
+{
+    if (int32_t rc = topology_check(c)) return rc;
+    CU(cudaSetDevice(c->device));
+    return FYX_OK;
+}
+
 void rebuild_node_arrays(fyx_ctx *c)
 {
     NodeArrays &a = c->a;
@@ -614,7 +630,7 @@ int32_t prepare_cull(fyx_ctx *c, uint32_t nf, const fyx_frustum *fr, const uint3
 // fold_on: stream for the skinned-mesh fold (+ cull of the skinned meshes); nullptr = the main stream, in order.  Another stream
 // is given by asynchronous frames that go on to the palette / skinning kernels: those need the bones' matrices, not the meshes'
 // boxes, so the (latency-bound) fold runs beside them; the caller joins the streams.
-int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cudaStream_t fold_on = nullptr)
+int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cudaStream_t fold_on)
 {
     const bool all = (update_flags & FYX_UPDATE_ALL) || !c->updated_once;
     const size_t nl = c->level_off.size() ? c->level_off.size() - 1 : 0;
@@ -644,8 +660,6 @@ int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cu
     CU(cudaGetLastError());
     return FYX_OK;
 }
-
-int32_t commit_surfaces(fyx_ctx *c);
 
 // counts, then the lists sized by them, to pinned host memory (stream `s`, two synchronisations)
 int32_t readback_visible(fyx_ctx *c, VisSlot &V, cudaStream_t s)
@@ -745,9 +759,7 @@ extern "C" int32_t fyx_create(const fyx_config *cfg, fyx_ctx **out_ctx)
 }
 
 static void fyx_comm_destroy_internal(fyx_ctx *c); // fyx_comm.inl
-static bool lod_active(const fyx_ctx *c, uint32_t nf);  // fyx_drawprep.inl
-static int32_t lod_pass(fyx_ctx *c);                    // fyx_drawprep.inl
-// DFS-pruning features (LOD filter, static batches): the cull cannot be fused into the level kernels
+// DFS-pruning features (LOD filter, static batches): the cull cannot be fused into the level kernels (fyx_drawprep.inl)
 static bool unfused_cull(const fyx_ctx *c, uint32_t nf);
 static int32_t cull_unfused(fyx_ctx *c, uint32_t nf);
 static int32_t animate_enqueue(fyx_ctx *c, float dt);  // fyx_anim.inl
@@ -1067,8 +1079,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
 
 extern "C" int32_t fyx_set_dfs_order(fyx_ctx *c, uint32_t capacity, const uint32_t *preorder_rank)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (preorder_rank && capacity != c->n_nodes) return fail(c, FYX_ERR_INVALID_ARGUMENT, "capacity %u != topology capacity %u", capacity, c->n_nodes);
     if (preorder_rank) c->dfs_rank.assign(preorder_rank, preorder_rank + capacity);
     else c->dfs_rank.clear();
@@ -1077,67 +1088,64 @@ extern "C" int32_t fyx_set_dfs_order(fyx_ctx *c, uint32_t capacity, const uint32
     return FYX_OK;
 }
 
+// The forms of changed local transforms: 4x4 matrices, TRS records, or rotations alone (the last position and scale stay)
+enum LocalsForm { LOCALS_M16, LOCALS_TRS, LOCALS_ROT };
+
+// `count` changed local transforms, already on the device (d_idx NULL = nodes 0..count-1), into their nodes' slots on stream `s`.
+// The TRS forms go through the TRS column, which keeps the parts a rotation alone does not change.
+static int32_t scatter_locals(fyx_ctx *c, cudaStream_t s, LocalsForm form, uint32_t count, const uint32_t *d_idx, const void *d_payload)
+{
+    if (form == LOCALS_M16) {
+        launch_scatter_locals(s, c->a, count, d_idx, static_cast<const float *>(d_payload), c->b_slot_of_node.as<uint32_t>(), c->n_nodes,
+                              c->d_err.as<uint32_t>());
+    } else {
+        int32_t rc = c->trs.ensure(c);
+        if (rc) return rc;
+        launch_scatter_trs(s, c->a, count, d_idx, d_payload, form == LOCALS_ROT, c->trs.buf.as<fyx_trs>(),
+                           c->statics.live ? c->statics.buf.as<fyx_transform_statics>() : nullptr, c->b_slot_of_node.as<uint32_t>(), c->n_nodes,
+                           c->d_err.as<uint32_t>());
+    }
+    c->launches++;
+    CU(cudaGetLastError());
+    return FYX_OK;
+}
+
 extern "C" int32_t fyx_set_local_matrices(fyx_ctx *c, uint32_t count, const uint32_t *idx, const float *m16)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!m16) return fail(c, FYX_ERR_INVALID_ARGUMENT, "m16 is NULL");
     CU(cudaSetDevice(c->device));
     void *d_m = nullptr, *d_i = nullptr;
     int32_t rc = stage_to_device(c, m16, (size_t)count * 64, idx, idx ? (size_t)count * 4 : 0, false, &d_m, &d_i);
-    if (rc) return rc;
-    launch_scatter_locals(c->stream, c->a, count, static_cast<const uint32_t *>(d_i), static_cast<const float *>(d_m),
-                          c->b_slot_of_node.as<uint32_t>(), c->n_nodes, c->d_err.as<uint32_t>());
-    c->launches++;
-    CU(cudaGetLastError());
-    return FYX_OK;
+    return rc ? rc : scatter_locals(c, c->stream, LOCALS_M16, count, static_cast<const uint32_t *>(d_i), d_m);
 }
 
 extern "C" int32_t fyx_set_local_rotations(fyx_ctx *c, uint32_t count, const uint32_t *idx, const float *quat_ijkw)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!quat_ijkw) return fail(c, FYX_ERR_INVALID_ARGUMENT, "rotations are NULL");
     CU(cudaSetDevice(c->device));
-    int32_t rc = c->trs.ensure(c);
-    if (rc) return rc;
     void *d_q = nullptr, *d_i = nullptr;
-    rc = stage_to_device(c, quat_ijkw, (size_t)count * 16, idx, idx ? (size_t)count * 4 : 0, false, &d_q, &d_i);
-    if (rc) return rc;
-    launch_scatter_trs(c->stream, c->a, count, static_cast<const uint32_t *>(d_i), d_q, true, c->trs.buf.as<fyx_trs>(),
-                       c->statics.live ? c->statics.buf.as<fyx_transform_statics>() : nullptr, c->b_slot_of_node.as<uint32_t>(), c->n_nodes,
-                       c->d_err.as<uint32_t>());
-    c->launches++;
-    CU(cudaGetLastError());
-    return FYX_OK;
+    int32_t rc = stage_to_device(c, quat_ijkw, (size_t)count * 16, idx, idx ? (size_t)count * 4 : 0, false, &d_q, &d_i);
+    return rc ? rc : scatter_locals(c, c->stream, LOCALS_ROT, count, static_cast<const uint32_t *>(d_i), d_q);
 }
 
 extern "C" int32_t fyx_set_local_trs(fyx_ctx *c, uint32_t count, const uint32_t *idx, const fyx_trs *trs)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!trs) return fail(c, FYX_ERR_INVALID_ARGUMENT, "trs is NULL");
     CU(cudaSetDevice(c->device));
-    int32_t rc = c->trs.ensure(c);
-    if (rc) return rc;
     void *d_t = nullptr, *d_i = nullptr;
-    rc = stage_to_device(c, trs, (size_t)count * sizeof(fyx_trs), idx, idx ? (size_t)count * 4 : 0, false, &d_t, &d_i);
-    if (rc) return rc;
-    launch_scatter_trs(c->stream, c->a, count, static_cast<const uint32_t *>(d_i), d_t, false, c->trs.buf.as<fyx_trs>(),
-                       c->statics.live ? c->statics.buf.as<fyx_transform_statics>() : nullptr, c->b_slot_of_node.as<uint32_t>(), c->n_nodes,
-                       c->d_err.as<uint32_t>());
-    c->launches++;
-    CU(cudaGetLastError());
-    return FYX_OK;
+    int32_t rc = stage_to_device(c, trs, (size_t)count * sizeof(fyx_trs), idx, idx ? (size_t)count * 4 : 0, false, &d_t, &d_i);
+    return rc ? rc : scatter_locals(c, c->stream, LOCALS_TRS, count, static_cast<const uint32_t *>(d_i), d_t);
 }
 
 extern "C" int32_t fyx_set_transform_statics(fyx_ctx *c, uint32_t count, const uint32_t *idx, const fyx_transform_statics *statics)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!statics) return fail(c, FYX_ERR_INVALID_ARGUMENT, "statics is NULL");
     CU(cudaSetDevice(c->device));
@@ -1146,8 +1154,7 @@ extern "C" int32_t fyx_set_transform_statics(fyx_ctx *c, uint32_t count, const u
 
 extern "C" int32_t fyx_set_flags(fyx_ctx *c, uint32_t count, const uint32_t *idx, const uint32_t *flags)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!flags) return fail(c, FYX_ERR_INVALID_ARGUMENT, "values are NULL");
     for (uint32_t i = 0; i < count; ++i)
@@ -1165,8 +1172,7 @@ extern "C" int32_t fyx_set_flags(fyx_ctx *c, uint32_t count, const uint32_t *idx
 
 extern "C" int32_t fyx_set_render_masks(fyx_ctx *c, uint32_t count, const uint32_t *idx, const uint32_t *mask)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!mask) return fail(c, FYX_ERR_INVALID_ARGUMENT, "values are NULL");
     CU(cudaSetDevice(c->device));
@@ -1175,8 +1181,7 @@ extern "C" int32_t fyx_set_render_masks(fyx_ctx *c, uint32_t count, const uint32
 
 extern "C" int32_t fyx_set_local_aabbs(fyx_ctx *c, uint32_t count, const uint32_t *idx, const float *aabb)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!aabb) return fail(c, FYX_ERR_INVALID_ARGUMENT, "aabb is NULL");
     CU(cudaSetDevice(c->device));
@@ -1240,7 +1245,7 @@ constexpr uint32_t kTileQuads = 2048; // up to 8192 vertices per tile (a 5k-vert
 int32_t commit_surfaces(fyx_ctx *c)
 {
     if (!c->tables_dirty) return FYX_OK;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     const size_t ns = c->surfaces.size();
     std::vector<uint32_t> bone_slot(c->n_entries);
     std::vector<SkinTile> tiles;
@@ -1368,8 +1373,7 @@ extern "C" int32_t fyx_add_skinned_surface(fyx_ctx *c, uint32_t mesh_node, uint3
                                            const float *inv_bind, uint32_t n_verts, const void *verts,
                                            const fyx_vertex_layout *layout, uint32_t *out_id)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (n_bones > FYX_MAX_BONES) return fail(c, FYX_ERR_INVALID_ARGUMENT, "n_bones %u > %u", n_bones, FYX_MAX_BONES);
     if (n_bones && (!bone_nodes || !inv_bind)) return fail(c, FYX_ERR_INVALID_ARGUMENT, "bone arrays are NULL");
     if (n_verts && (!verts || !layout)) return fail(c, FYX_ERR_INVALID_ARGUMENT, "verts/layout are NULL");
@@ -1524,61 +1528,86 @@ extern "C" int32_t fyx_commit_surfaces(fyx_ctx *c)
 }
 
 // --------------------------------------------------------------------------------------------
-// per frame
+// per frame.  Each stage is enqueued by one function that fyx_render_prep and the stage's own call share: scatter_locals,
+// animate_enqueue (fyx_anim.inl), update_cull_enqueue, palette_enqueue, skin_enqueue.  They record no events; their callers do.
 // --------------------------------------------------------------------------------------------
-extern "C" int32_t fyx_update_transforms(fyx_ctx *c, uint32_t update_flags)
+namespace {
+
+// Hierarchy + world boxes, and the cull of the `nf` frusta prepare_cull set up (nf = 0: no cull).  With a LOD filter / static
+// batches the cull cannot be fused into the level kernels: the pruning bits need every ancestor first.  side_fold_wanted: the
+// caller joins c->ev_fold_done before the boxes are read, so the skinned-mesh fold may run on c->fold_stream (run_update);
+// *side_fold tells whether it does.
+int32_t update_cull_enqueue(fyx_ctx *c, uint32_t update_flags, uint32_t nf, bool side_fold_wanted = false, bool *side_fold = nullptr)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
-    CU(cudaSetDevice(c->device));
-    int32_t rc = commit_surfaces(c);
+    static const bool side_fold_allowed = [] {
+        const char *e = getenv("FYX_SIDE_FOLD"); // 0: the fold always runs in order on the main stream (A/B measurements)
+        return !(e && *e == '0');
+    }();
+    const bool unf = unfused_cull(c, nf);
+    const bool side = side_fold_wanted && side_fold_allowed && !unf && c->fold.n;
+    if (side_fold) *side_fold = side;
+    int32_t rc = run_update(c, update_flags, (nf && !unf) ? &c->cp : nullptr, side ? c->fold_stream.h : nullptr);
     if (rc) return rc;
+    return unf ? cull_unfused(c, nf) : FYX_OK;
+}
+
+// the bones' skinning matrices (palettes)
+void palette_enqueue(fyx_ctx *c, cudaStream_t s)
+{
+    if (c->sk.n_entries) {
+        launch_palette(s, c->a, c->sk);
+        c->launches++;
+    }
+}
+
+void skin_enqueue(fyx_ctx *c, cudaStream_t s)
+{
+    if (c->n_tiles) {
+        launch_skin(s, c->sk, c->b_tiles.as<SkinTile>(), c->n_tiles, c->max_bones, c->any_blend_shapes);
+        c->launches++;
+    }
+}
+
+// A stand-alone stage call: the stage alone on the main stream, between EV_START and `ev_end`, synchronised; its time goes to `ms`.
+template <class Enqueue> int32_t run_timed(fyx_ctx *c, int ev_end, float &ms, Enqueue enqueue)
+{
     CU(cudaEventRecord(c->ev[EV_START], c->stream));
-    rc = run_update(c, update_flags, nullptr);
+    int32_t rc = enqueue();
     if (rc) return rc;
-    CU(cudaEventRecord(c->ev[EV_UPDATE], c->stream));
+    CU(cudaEventRecord(c->ev[ev_end], c->stream));
     rc = sync_and_check(c);
-    cudaEventElapsedTime(&c->timings.update_ms, c->ev[EV_START], c->ev[EV_UPDATE]);
+    cudaEventElapsedTime(&ms, c->ev[EV_START], c->ev[ev_end]);
     return rc;
 }
 
+} // namespace
+
+extern "C" int32_t fyx_update_transforms(fyx_ctx *c, uint32_t update_flags)
+{
+    int32_t rc;
+    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    return run_timed(c, EV_UPDATE, c->timings.update_ms, [&] { return update_cull_enqueue(c, update_flags, 0); });
+}
+
+// fyx_cull and fyx_update_and_cull prepare the cull even for nf = 0: a new, empty visible slot becomes the one fyx_get_visible reads
 extern "C" int32_t fyx_cull(fyx_ctx *c, uint32_t nf, const fyx_frustum *fr, const uint32_t *cam_mask, const uint32_t *pass_flags)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
-    CU(cudaSetDevice(c->device));
-    CU(cudaEventRecord(c->ev[EV_START], c->stream));
-    int32_t rc = prepare_cull(c, nf, fr, cam_mask, pass_flags);
-    if (rc) return rc;
-    if (nf && (rc = cull_unfused(c, nf))) return rc;
-    CU(cudaEventRecord(c->ev[EV_CULL], c->stream));
-    rc = sync_and_check(c);
-    cudaEventElapsedTime(&c->timings.cull_ms, c->ev[EV_START], c->ev[EV_CULL]);
-    return rc;
+    int32_t rc;
+    if ((rc = enter(c))) return rc;
+    return run_timed(c, EV_CULL, c->timings.cull_ms, [&] {
+        if ((rc = prepare_cull(c, nf, fr, cam_mask, pass_flags)) || !nf) return rc;
+        return cull_unfused(c, nf);
+    });
 }
 
 extern "C" int32_t fyx_update_and_cull(fyx_ctx *c, uint32_t update_flags, uint32_t nf, const fyx_frustum *fr,
                                        const uint32_t *cam_mask, const uint32_t *pass_flags)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
-    CU(cudaSetDevice(c->device));
-    int32_t rc = commit_surfaces(c);
-    if (rc) return rc;
-    CU(cudaEventRecord(c->ev[EV_START], c->stream));
-    rc = prepare_cull(c, nf, fr, cam_mask, pass_flags);
-    if (rc) return rc;
-    {
-        // with a LOD filter / static batches the cull cannot be fused into the level kernels: the pruning bits need every ancestor first
-        const bool unf = unfused_cull(c, nf);
-        rc = run_update(c, update_flags, (nf && !unf) ? &c->cp : nullptr);
-        if (rc) return rc;
-        if (unf && (rc = cull_unfused(c, nf))) return rc;
-    }
-    CU(cudaEventRecord(c->ev[EV_UPDATE], c->stream));
-    rc = sync_and_check(c);
-    cudaEventElapsedTime(&c->timings.update_ms, c->ev[EV_START], c->ev[EV_UPDATE]);
-    return rc;
+    int32_t rc;
+    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    return run_timed(c, EV_UPDATE, c->timings.update_ms, [&] {
+        return (rc = prepare_cull(c, nf, fr, cam_mask, pass_flags)) ? rc : update_cull_enqueue(c, update_flags, nf);
+    });
 }
 
 extern "C" int32_t fyx_get_visible(fyx_ctx *c, uint32_t f, const uint32_t **out_idx, uint32_t *out_count)
@@ -1607,38 +1636,22 @@ extern "C" int32_t fyx_get_visible_device(fyx_ctx *c, uint32_t f, const uint32_t
 
 extern "C" int32_t fyx_build_palettes(fyx_ctx *c)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
-    CU(cudaSetDevice(c->device));
-    int32_t rc = commit_surfaces(c);
-    if (rc) return rc;
-    CU(cudaEventRecord(c->ev[EV_START], c->stream));
-    if (c->sk.n_entries) {
-        launch_palette(c->stream, c->a, c->sk);
-        c->launches++;
-    }
-    CU(cudaEventRecord(c->ev[EV_PALETTE], c->stream));
-    rc = sync_and_check(c);
-    cudaEventElapsedTime(&c->timings.palette_ms, c->ev[EV_START], c->ev[EV_PALETTE]);
-    return rc;
+    int32_t rc;
+    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    return run_timed(c, EV_PALETTE, c->timings.palette_ms, [&] {
+        palette_enqueue(c, c->stream);
+        return FYX_OK;
+    });
 }
 
 extern "C" int32_t fyx_skin(fyx_ctx *c)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
-    CU(cudaSetDevice(c->device));
-    int32_t rc = commit_surfaces(c);
-    if (rc) return rc;
-    CU(cudaEventRecord(c->ev[EV_START], c->stream));
-    if (c->n_tiles) {
-        launch_skin(c->stream, c->sk, c->b_tiles.as<SkinTile>(), c->n_tiles, c->max_bones, c->any_blend_shapes);
-        c->launches++;
-    }
-    CU(cudaEventRecord(c->ev[EV_SKIN], c->stream));
-    rc = sync_and_check(c);
-    cudaEventElapsedTime(&c->timings.skin_ms, c->ev[EV_START], c->ev[EV_SKIN]);
-    return rc;
+    int32_t rc;
+    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    return run_timed(c, EV_SKIN, c->timings.skin_ms, [&] {
+        skin_enqueue(c, c->stream);
+        return FYX_OK;
+    });
 }
 
 static void frame_timings_from_events(fyx_ctx *c)
@@ -1657,14 +1670,67 @@ static void frame_timings_from_events(fyx_ctx *c)
     c->timings_pending = false;
 }
 
+// 1. of fyx_render_prep: the changed local transforms.  Pinned caller memory is DMA'd in place (the caller keeps it untouched
+//    until the frame is synchronised / waited for).  Async frames upload on the copy stream into alternating staging buffers,
+//    so the H2D of frame i+1 overlaps the kernels of frame i.
+static int32_t frame_upload(fyx_ctx *c, const fyx_frame_desc *fr, bool async)
+{
+    if (!fr->n_changed) return FYX_OK;
+    const LocalsForm form = fr->changed_rot ? LOCALS_ROT : (fr->changed_trs ? LOCALS_TRS : LOCALS_M16);
+    const void *payload = form == LOCALS_ROT ? static_cast<const void *>(fr->changed_rot)
+                          : (form == LOCALS_TRS ? static_cast<const void *>(fr->changed_trs) : static_cast<const void *>(fr->changed_m16));
+    if (!payload) return fail(c, FYX_ERR_INVALID_ARGUMENT, "changed_m16 / changed_trs / changed_rot is NULL");
+    const size_t mb = (size_t)fr->n_changed * (form == LOCALS_ROT ? 16 : (form == LOCALS_TRS ? sizeof(fyx_trs) : 64)),
+                 ib = fr->changed_idx ? (size_t)fr->n_changed * 4 : 0;
+    cudaStream_t s = c->stream;
+    int32_t rc;
+    if (!(async && is_pinned(payload) && (!fr->changed_idx || is_pinned(fr->changed_idx)))) {
+        void *d_m = nullptr, *d_i = nullptr;
+        rc = stage_to_device(c, payload, mb, fr->changed_idx, ib, true, &d_m, &d_i);
+        return rc ? rc : scatter_locals(c, s, form, fr->n_changed, static_cast<const uint32_t *>(d_i), d_m);
+    }
+    const int u = (c->upload_parity ^= 1);
+    if (c->slot_used[u]) CU(cudaEventSynchronize(c->ev_slot_free[u])); // its previous scatter has consumed it
+    const size_t off = (mb + 255) & ~size_t(255);
+    rc = dev_ensure(c, c->d_stage_frame[u], off + ib + 256);
+    if (rc) return rc;
+    char *base = c->d_stage_frame[u].as<char>();
+    const uint32_t *d_idx = ib ? reinterpret_cast<const uint32_t *>(base + off) : nullptr;
+    CU(cudaMemcpyAsync(base, payload, mb, cudaMemcpyHostToDevice, c->copy_stream));
+    if (ib) CU(cudaMemcpyAsync(base + off, fr->changed_idx, ib, cudaMemcpyHostToDevice, c->copy_stream));
+    // The scatter writes local matrices / TRS records / F_DIRTY_SELF of the changed nodes — columns nothing of the PREVIOUS
+    // frame reads once its level kernels and fold are done.  When that point is known (the previous frame recorded its
+    // cull event) and nothing else has been enqueued on the main stream since, the scatter runs on the copy stream, beside
+    // the previous frame's palette / skinning kernels, instead of in front of this frame's level kernels.  Nor may the
+    // scatter enqueue anything on the main stream itself: a TRS form's first upload fills the TRS column there.
+    static const bool side_allowed = [] {
+        const char *e = getenv("FYX_SIDE_SCATTER"); // 0: always scatter on the main stream (A/B measurements)
+        return !(e && *e == '0');
+    }();
+    const bool side = side_allowed && c->ev_levels_prev && c->launches == c->launches_at_frame_end &&
+                      (form == LOCALS_M16 || c->trs.live) && !(fr->struct_size >= sizeof(fyx_frame_desc) && fr->do_animate);
+    if (side) {
+        CU(cudaStreamWaitEvent(c->copy_stream, c->ev_levels_prev, 0));
+        if ((rc = scatter_locals(c, c->copy_stream, form, fr->n_changed, d_idx, base))) return rc;
+        CU(cudaEventRecord(c->ev_upload[u], c->copy_stream));
+        CU(cudaEventRecord(c->ev_slot_free[u], c->copy_stream));
+        CU(cudaStreamWaitEvent(s, c->ev_upload[u], 0));
+    } else {
+        CU(cudaEventRecord(c->ev_upload[u], c->copy_stream));
+        CU(cudaStreamWaitEvent(s, c->ev_upload[u], 0));
+        if ((rc = scatter_locals(c, s, form, fr->n_changed, d_idx, base))) return rc;
+        CU(cudaEventRecord(c->ev_slot_free[u], s));
+    }
+    c->slot_used[u] = true;
+    return FYX_OK;
+}
+
 extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
 {
     if (!c || !fr) return FYX_ERR_INVALID_ARGUMENT;
     if (fr->struct_size < offsetof(fyx_frame_desc, do_animate)) return fail(c, FYX_ERR_INVALID_ARGUMENT, "fyx_frame_desc.struct_size too small");
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
-    CU(cudaSetDevice(c->device));
-    int32_t rc = commit_surfaces(c);
-    if (rc) return rc;
+    int32_t rc;
+    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
     cudaStream_t s = c->stream;
     CU(cudaEventRecord(c->ev[EV_START], s));
     // 0. animation players tick before Graph::update (N2): curves are device-resident, nothing to upload
@@ -1679,86 +1745,16 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
     const bool stage_events = !async;
     c->stage_events_valid = stage_events;
     const bool pipelined = async && fr->readback_visible && fr->n_frusta; // read-back deferred to fyx_frame_wait
-    bool side_fold = false;
-    // 1. changed local matrices.  Pinned caller memory is DMA'd in place (the caller keeps it untouched until
-    //    the frame is synchronised / waited for).  Async frames upload on the copy stream into alternating
-    //    staging buffers, so the H2D of frame i+1 overlaps the kernels of frame i.
-    if (fr->n_changed) {
-        const bool as_rot = fr->changed_rot != nullptr, as_trs = !as_rot && fr->changed_trs != nullptr;
-        const void *payload = as_rot ? static_cast<const void *>(fr->changed_rot)
-                                     : (as_trs ? static_cast<const void *>(fr->changed_trs) : static_cast<const void *>(fr->changed_m16));
-        if (!payload) return fail(c, FYX_ERR_INVALID_ARGUMENT, "changed_m16 / changed_trs / changed_rot is NULL");
-        if (as_rot || as_trs) {
-            rc = c->trs.ensure(c);
-            if (rc) return rc;
-        }
-        const size_t mb = (size_t)fr->n_changed * (as_rot ? 16 : (as_trs ? sizeof(fyx_trs) : 64)), ib = fr->changed_idx ? (size_t)fr->n_changed * 4 : 0;
-        const fyx_transform_statics *st = c->statics.live ? c->statics.buf.as<fyx_transform_statics>() : nullptr;
-        auto scatter = [&](cudaStream_t ss, const void *d_p, const uint32_t *d_i) {
-            if (as_rot || as_trs)
-                launch_scatter_trs(ss, c->a, fr->n_changed, d_i, d_p, as_rot, c->trs.buf.as<fyx_trs>(), st, c->b_slot_of_node.as<uint32_t>(),
-                                   c->n_nodes, c->d_err.as<uint32_t>());
-            else
-                launch_scatter_locals(ss, c->a, fr->n_changed, d_i, static_cast<const float *>(d_p), c->b_slot_of_node.as<uint32_t>(),
-                                      c->n_nodes, c->d_err.as<uint32_t>());
-        };
-        if (async && is_pinned(payload) && (!fr->changed_idx || is_pinned(fr->changed_idx))) {
-            const int u = (c->upload_parity ^= 1);
-            if (c->slot_used[u]) CU(cudaEventSynchronize(c->ev_slot_free[u])); // its previous scatter has consumed it
-            const size_t off = (mb + 255) & ~size_t(255);
-            rc = dev_ensure(c, c->d_stage_frame[u], off + ib + 256);
-            if (rc) return rc;
-            char *base = c->d_stage_frame[u].as<char>();
-            CU(cudaMemcpyAsync(base, payload, mb, cudaMemcpyHostToDevice, c->copy_stream));
-            if (ib) CU(cudaMemcpyAsync(base + off, fr->changed_idx, ib, cudaMemcpyHostToDevice, c->copy_stream));
-            // The scatter writes local matrices / TRS records / F_DIRTY_SELF of the changed nodes — columns nothing of the PREVIOUS
-            // frame reads once its level kernels and fold are done.  When that point is known (the previous frame recorded its
-            // cull event) and nothing else has been enqueued on the main stream since, the scatter runs on the copy stream, beside
-            // the previous frame's palette / skinning kernels, instead of in front of this frame's level kernels.
-            static const bool side_allowed = [] {
-                const char *e = getenv("FYX_SIDE_SCATTER"); // 0: always scatter on the main stream (A/B measurements)
-                return !(e && *e == '0');
-            }();
-            const bool side = side_allowed && c->ev_levels_prev && c->launches == c->launches_at_frame_end &&
-                              !(fr->struct_size >= sizeof(fyx_frame_desc) && fr->do_animate);
-            if (side) {
-                CU(cudaStreamWaitEvent(c->copy_stream, c->ev_levels_prev, 0));
-                scatter(c->copy_stream, base, ib ? reinterpret_cast<const uint32_t *>(base + off) : nullptr);
-                CU(cudaEventRecord(c->ev_upload[u], c->copy_stream));
-                CU(cudaEventRecord(c->ev_slot_free[u], c->copy_stream));
-                CU(cudaStreamWaitEvent(s, c->ev_upload[u], 0));
-            } else {
-                CU(cudaEventRecord(c->ev_upload[u], c->copy_stream));
-                CU(cudaStreamWaitEvent(s, c->ev_upload[u], 0));
-                scatter(s, base, ib ? reinterpret_cast<const uint32_t *>(base + off) : nullptr);
-                CU(cudaEventRecord(c->ev_slot_free[u], s));
-            }
-            c->slot_used[u] = true;
-        } else {
-            void *d_m = nullptr, *d_i = nullptr;
-            rc = stage_to_device(c, payload, mb, fr->changed_idx, ib, true, &d_m, &d_i);
-            if (rc) return rc;
-            scatter(s, d_m, static_cast<const uint32_t *>(d_i));
-        }
-        c->launches++;
-    }
+    // 1. changed local transforms
+    if ((rc = frame_upload(c, fr, async))) return rc;
     if (stage_events) CU(cudaEventRecord(c->ev[EV_UPLOAD], s));
-    // 2. hierarchy + world boxes + cull
+    // 2. hierarchy + world boxes + cull; an asynchronous frame that goes on to skinning joins a fold on the side below
     if (fr->n_frusta) {
         rc = prepare_cull(c, fr->n_frusta, fr->frusta, fr->cam_mask, fr->pass_flags);
         if (rc) return rc;
     }
-    {
-        const bool unf = unfused_cull(c, fr->n_frusta);
-        static const bool side_fold_allowed = [] {
-            const char *e = getenv("FYX_SIDE_FOLD"); // 0: the fold always runs in order on the main stream (A/B measurements)
-            return !(e && *e == '0');
-        }();
-        side_fold = side_fold_allowed && async && !unf && c->fold.n && fr->do_skin && c->n_tiles;
-        rc = run_update(c, fr->update_flags, (fr->n_frusta && !unf) ? &c->cp : nullptr, side_fold ? c->fold_stream.h : nullptr);
-        if (rc) return rc;
-        if (unf && (rc = cull_unfused(c, fr->n_frusta))) return rc;
-    }
+    bool side_fold = false;
+    if ((rc = update_cull_enqueue(c, fr->update_flags, fr->n_frusta, async && fr->do_skin && c->n_tiles, &side_fold))) return rc;
     if (stage_events) CU(cudaEventRecord(c->ev[EV_UPDATE], s));
     c->ev_levels_prev = nullptr;
     if (fr->n_frusta && (async || (fr->flags & FYX_FRAME_ALLGATHER))) {
@@ -1778,15 +1774,9 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
         if (rc) return rc;
     }
     // 3. palettes, 4. skinning
-    if (fr->do_palettes && c->sk.n_entries) {
-        launch_palette(s, c->a, c->sk);
-        c->launches++;
-    }
+    if (fr->do_palettes) palette_enqueue(c, s);
     if (stage_events) CU(cudaEventRecord(c->ev[EV_PALETTE], s));
-    if (fr->do_skin && c->n_tiles) {
-        launch_skin(s, c->sk, c->b_tiles.as<SkinTile>(), c->n_tiles, c->max_bones, c->any_blend_shapes);
-        c->launches++;
-    }
+    if (fr->do_skin) skin_enqueue(c, s);
     if (stage_events) CU(cudaEventRecord(c->ev[EV_SKIN], s));
     CU(cudaGetLastError());
     if (side_fold) CU(cudaStreamWaitEvent(s, c->ev_fold_done, 0)); // join: whatever follows on the main stream sees the folded boxes and the complete lists
@@ -1880,8 +1870,7 @@ namespace {
 // gather `count` items of `item_bytes` through a gather launcher into caller memory
 template <class Launch> int32_t gather_out(fyx_ctx *c, uint32_t count, const uint32_t *idx, size_t item_bytes, void *out, Launch launch)
 {
-    if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (!c->have_topology) return fail(c, FYX_ERR_STATE, "fyx_set_topology has not been called");
+    if (int32_t rc = topology_check(c)) return rc;
     if (!count) return FYX_OK;
     if (!out) return fail(c, FYX_ERR_INVALID_ARGUMENT, "output pointer is NULL");
     CU(cudaSetDevice(c->device));
