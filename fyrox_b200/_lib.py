@@ -233,6 +233,7 @@ SYMBOLS = {
     "fyx_cull_shadow_casters": (C.c_int32, [ctx_p, C.c_uint32, f32p, C.POINTER(fyx_shadow_settings)]),
     "fyx_set_csm_options": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     "fyx_cull_shadow_casters_csm": (C.c_int32, [ctx_p, C.c_uint32, f32p, C.POINTER(fyx_shadow_settings), C.POINTER(fyx_csm_camera)]),
+    "fyx_cull_shadow_casters_pruned": (C.c_int32, [ctx_p, C.c_uint32, f32p, C.POINTER(fyx_shadow_settings), C.POINTER(fyx_csm_camera)]),
     "fyx_get_shadow_maps": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p)]),
     "fyx_get_shadow_maps_device": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p)]),
     "fyx_build_palettes": (C.c_int32, [ctx_p]),

@@ -366,15 +366,20 @@ class Context:
         return cam
 
     def cull_shadow_casters(self, camera_frustum: int, camera_translation, spot_shadows_distance: float = 10.0, point_shadows_distance: float = 10.0,
-                            spot_shadows_enabled: bool = True, point_shadows_enabled: bool = True, csm_camera=None):
+                            spot_shadows_enabled: bool = True, point_shadows_enabled: bool = True, csm_camera=None, prune: bool = False):
         """The shadow maps the deferred light renderer draws for frustum `camera_frustum` of the last cull, and their visible
         sets (renderer/light.rs:509-606, 695-782).  Defaults are QualitySettings::default() (renderer/settings.rs).  Spot and
         point maps always; the cascades of directional lights (renderer/shadow/csm.rs) when `csm_camera` (Context.csm_camera
-        or an fyx_csm_camera) is given, through fyx_cull_shadow_casters_csm."""
+        or an fyx_csm_camera) is given, through fyx_cull_shadow_casters_csm.  prune=True: every map's list with the map's own
+        LOD filter and static-batch pruning (fyx_cull_shadow_casters_pruned, with or without `csm_camera`); without it a scene
+        with LOD ranges or static batches is refused."""
         t = _f32(camera_translation)
         st = L.fyx_shadow_settings(float(spot_shadows_distance), float(point_shadows_distance), int(bool(spot_shadows_enabled)),
                                    int(bool(point_shadows_enabled)))
-        if csm_camera is None:
+        if prune:
+            cam = C.byref(csm_camera) if csm_camera is not None else None
+            self._chk(self._lib.fyx_cull_shadow_casters_pruned(self._h, camera_frustum, t.ctypes.data_as(L.f32p), C.byref(st), cam))
+        elif csm_camera is None:
             self._chk(self._lib.fyx_cull_shadow_casters(self._h, camera_frustum, t.ctypes.data_as(L.f32p), C.byref(st)))
         else:
             self._chk(self._lib.fyx_cull_shadow_casters_csm(self._h, camera_frustum, t.ctypes.data_as(L.f32p), C.byref(st), C.byref(csm_camera)))

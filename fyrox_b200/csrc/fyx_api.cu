@@ -27,6 +27,8 @@ namespace {
 
 thread_local std::string g_create_error;
 
+constexpr uint8_t kPrLod = 1, kPrBatch = 2; // fyx_ctx::pr_node
+
 // Owners of the context's CUDA resources.  Each is move-only and frees what it holds when it dies; a move assignment swaps,
 // so what the target held before dies with the moved-from source.  A failed allocation leaves the owner as it was.
 struct DevBuf {
@@ -377,6 +379,14 @@ struct fyx_ctx {
     DevBuf b_sh_slots, b_sh_views;
     bool sh_have_slots = false, sh_slots_stale = false;
     InstPack shi;
+    // per-map LOD filter and static-batch pruning (fyx_cull_shadow_casters_pruned).  pr_node: by node index, kPrLod | kPrBatch
+    // for a node with a LOD range / FYX_NODE_STATIC_BATCH (kept beside the device columns, so that a change is seen without
+    // reading them back).  The pruner column is rebuilt by the first pruned cull after such a change (pr_dirty).
+    std::vector<uint8_t> pr_node;
+    bool pr_dirty = true;
+    uint32_t n_pruners = 0;
+    std::vector<uint32_t> pr_level_off; // pruner ids per hierarchy level (pruners are numbered in slot order)
+    DevBuf b_pr_col, b_pr_slot, b_pr_anc, b_pr_rows, b_pr_obs;
 
     // N3 draw-prep (fyx_drawprep.inl)
     bool instances_enabled = false, rank_on_device = false;
@@ -546,6 +556,7 @@ int32_t check_device_errors(fyx_ctx *c)
     if (e & E_BAD_BONE_INDEX) return fail(c, FYX_ERR_INVALID_ARGUMENT, "a vertex references a bone index >= n_bones");
     if (e & E_NONFINITE_VERTEX) return fail(c, FYX_ERR_INVALID_ARGUMENT, "a vertex position is not finite");
     if (e & E_PEER_TIMEOUT) return fail(c, FYX_ERR_NCCL, "the peer exchange of the visible lists timed out: a rank did not take part in the frame");
+    if (e & E_SHADOW_LIST) return fail(c, FYX_ERR_CUDA, "internal: a pruned shadow map had more entries than its count pass found; its list is incomplete");
     return FYX_OK;
 }
 
@@ -571,6 +582,15 @@ int32_t enter(fyx_ctx *c)
     if (int32_t rc = topology_check(c)) return rc;
     CU(cudaSetDevice(c->device));
     return FYX_OK;
+}
+
+// a pruner mark (kPrLod / kPrBatch) of an alive node set or cleared; the pruner column is rebuilt when a mark changes
+void pr_mark(fyx_ctx *c, uint32_t node, uint8_t bit, bool on)
+{
+    if (node >= c->n_nodes || node >= c->pr_node.size() || c->slot_of_node[node] == FYX_NONE) return; // skipped by the scatter kernels too
+    const uint8_t m = on ? (c->pr_node[node] | bit) : (c->pr_node[node] & ~bit);
+    if (m != c->pr_node[node]) c->pr_dirty = true;
+    c->pr_node[node] = m;
 }
 
 void rebuild_node_arrays(fyx_ctx *c)
@@ -1011,6 +1031,19 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
         if (!carry) col->live = false; // nothing to carry over (first topology, or one side empty): the column starts afresh
         else if ((rc = col->carry(c, b_map.as<uint32_t>()))) return rc;
     }
+    // the pruner marks: a LOD range stays with a node alive before and after (as the column carries it), static batches come
+    // from the new flags
+    {
+        const size_t old_cap = c->slot_of_node.size();
+        c->pr_node.resize(capacity, 0);
+        for (uint32_t i = 0; i < capacity; ++i) {
+            const bool kept = carry && i < old_cap && c->slot_of_node[i] != FYX_NONE && slot_of_node[i] != FYX_NONE;
+            uint8_t m = kept ? (c->pr_node[i] & kPrLod) : 0;
+            if (slot_of_node[i] != FYX_NONE && (fl(i) & FYX_NODE_STATIC_BATCH)) m |= kPrBatch;
+            c->pr_node[i] = m;
+        }
+        c->pr_dirty = true;
+    }
     if (!carry) c->n_bundle_ids = 1;
 
     // device columns.  Everything is allocated before the fills below are launched: the planes the level kernels stream side by
@@ -1163,6 +1196,8 @@ extern "C" int32_t fyx_set_flags(fyx_ctx *c, uint32_t count, const uint32_t *idx
     void *d_v = nullptr, *d_i = nullptr;
     int32_t rc = stage_to_device(c, flags, (size_t)count * 4, idx, idx ? (size_t)count * 4 : 0, false, &d_v, &d_i);
     if (rc) return rc;
+    for (uint32_t i = 0; i < count; ++i) // the pruner marks, as k_scatter_flags resolves the nodes
+        pr_mark(c, idx ? idx[i] : i, kPrBatch, (flags[i] & FYX_NODE_STATIC_BATCH) != 0);
     launch_scatter_flags(c->stream, c->a.flags, count, static_cast<const uint32_t *>(d_i), static_cast<const uint32_t *>(d_v),
                          c->b_slot_of_node.as<uint32_t>(), c->n_nodes);
     c->launches++;

@@ -267,9 +267,31 @@ struct ShadowParams {
     uint32_t *entries;    // [total], sized by the host from the count pass
     uint32_t *entry_slot; // [total] the same entries as HBM slots; nullptr unless fyx_enable_instances
     CsmCameraDev csm;     // last, so that the node passes' parameter offsets do not move
+    // ---- per-map LOD filter and static-batch pruning (fyx_cull_shadow_casters_pruned; unused by the unpruned kernels).
+    // A pruner is a LOD object or an FYX_NODE_STATIC_BATCH node; pruners have dense ids in slot order.
+    struct Prune {
+        const uint32_t *col;    // per slot: the nearest pruner on the node's path (id | kPrSelf when the node is that pruner), FYX_NONE = none
+        const uint32_t *slot;   // per pruner: its slot
+        const uint32_t *anc;    // per pruner: the nearest strict pruner ancestor, FYX_NONE = none
+        const float2 *range;    // per slot: LOD range (begin NaN = none); nullptr = no node has one
+        uint32_t *rows;         // [pruner][2][words]: maps hiding the pruner itself, then maps hiding its children
+        uint32_t words;         // u32 words per row (ceil(max maps / 32))
+        float *obs;             // [max maps * 5]: the map's observer for the LOD filter (translation, z_near, z_far)
+        uint32_t *err;          // the context's error word (E_SHADOW_LIST)
+    } pr;
 };
+constexpr uint32_t kPrSelf = 1u << 31; // bit of ShadowParams::Prune::col: the node is the pruner itself
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp); // map table + frusta, count pass, scan
 void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);
+// the same with every map's LOD filter and static-batch pruning: map table + observers, the pruner table (one launch per entry
+// of pr_level_off that holds pruners, parents first), count pass, scan; then the emit pass
+void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
+                               uint64_t *launches);
+void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);
+// the pruner column ShadowParams::Prune::col / anc from the pruners' slots: col must hold FYX_NONE everywhere; then one launch per
+// hierarchy level [level_off[l], level_off[l + 1]) from level `first` on, parents first
+void launch_pruner_mark(cudaStream_t s, uint32_t n_pruners, const uint32_t *pr_slot, uint32_t *col);
+void launch_pruner_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, uint32_t *col, uint32_t *anc);
 void launch_fold_bones(cudaStream_t s, const NodeArrays &a, const FoldArrays &fa, const CullParams *cull);
 void launch_snapshot_bones(cudaStream_t s, const NodeArrays &a, uint32_t n_late, const uint32_t *late_slot, float4 *stale_pos);
 void launch_palette(cudaStream_t s, const NodeArrays &a, const SkinArrays &sk);
@@ -357,5 +379,6 @@ constexpr uint32_t E_NOT_AFFINE = 1u;
 constexpr uint32_t E_BAD_BONE_INDEX = 2u;
 constexpr uint32_t E_NONFINITE_VERTEX = 4u;
 constexpr uint32_t E_PEER_TIMEOUT = 8u; // a rank never showed up in the peer exchange (bounded spin, fyx_peer.cu)
+constexpr uint32_t E_SHADOW_LIST = 16u; // the pruned shadow emit pass found more entries for a map than its count pass (nothing written)
 
 } // namespace fyx

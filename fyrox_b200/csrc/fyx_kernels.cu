@@ -1538,10 +1538,17 @@ __device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uin
     else sp.frusta[m] = sp.fallback;
 }
 
+// the observer of a map's from_graph for the LOD filter (renderer/bundle.rs:873-916): translation, z_near, z_far
+__device__ __forceinline__ void map_observer(float *o, const float *t, const float z_near, const float z_far)
+{
+    o[0] = t[0]; o[1] = t[1]; o[2] = t[2]; o[3] = z_near; o[4] = z_far;
+}
+
 // cascade i of a directional light (renderer/shadow/csm.rs:195-249): the light-space box around slice i of the camera
-// frustum.  V = the map's look_at_lh, P = its orthographic projection.
+// frustum.  V = the map's look_at_lh, P = its orthographic projection.  obs != nullptr: the cascade's observer
+// (shadow/csm.rs:251-265: the look_at_lh eye, the slice's depths after the guard) goes there.
 __device__ __forceinline__ void csm_cascade(const CsmCameraDev &cam, const fyx_csm_options &opt, const uint32_t i, const float *light_dir,
-                                         const float *light_up, float *V, float *P)
+                                         const float *light_up, float *V, float *P, float *obs = nullptr)
 {
     // csm.rs:181-194: z_values = [z_near, far planes] (Absolute) or [z_near, z_far * fractions] (Relative)
     const float a = i == 0u ? cam.z_near : opt.relative ? FYX_MUL(cam.z_far, opt.splits[i - 1]) : opt.splits[i - 1];
@@ -1558,6 +1565,7 @@ __device__ __forceinline__ void csm_cascade(const CsmCameraDev &cam, const fyx_c
     float c[3];
     frustum_center(fr, c);
     const float eye[3] = {FYX_ADD(c[0], light_dir[0]), FYX_ADD(c[1], light_dir[1]), FYX_ADD(c[2], light_dir[2])};
+    if (obs) map_observer(obs, eye, z_near, z_far);
     look_at_lh(eye, c, light_up, V);
     // AxisAlignedBoundingBox::default + add_point of every light-space corner
     float mn[3] = {3.40282347e+38f, 3.40282347e+38f, 3.40282347e+38f}, mx[3] = {-3.40282347e+38f, -3.40282347e+38f, -3.40282347e+38f};
@@ -1575,6 +1583,8 @@ __device__ __forceinline__ void csm_cascade(const CsmCameraDev &cam, const fyx_c
     orthographic(mn[0], mx[0], mn[1], mx[1], mn[2], mx[2], P);
 }
 
+// PRUNE: each map's LOD observer goes to sp.pr.obs as well
+template <bool PRUNE>
 __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, const ShadowParams sp)
 {
     __shared__ uint32_t s_warp[kBlock / 32];
@@ -1667,11 +1677,13 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
                 try_normalize(lookv, zdir, up);
 #pragma unroll 1
                 for (uint32_t k = 0; k < 3u; ++k) {
-                    csm_cascade(sp.csm, csm_opt, k, dir, up, V, P);
+                    csm_cascade(sp.csm, csm_opt, k, dir, up, V, P, PRUNE ? sp.pr.obs + (size_t)(first + k) * 5 : nullptr);
                     shadow_map_out(sp, first + k, light, 0u, k, P, V);
                 }
             } else {
                 perspective(m22, 1.0f, 0.01f, radius, P); // z_near 0.01, z_far light_radius (light.rs:702-704, point.rs:167-170)
+                if (PRUNE) // light.rs:700-728, shadow/point.rs:162-190: the light's position, z_near 0.01, z_far light_radius
+                    for (uint32_t k = 0; k < (kind == FYX_LIGHT_SPOT ? 1u : 6u); ++k) map_observer(sp.pr.obs + (size_t)(first + k) * 5, pos, 0.01f, radius);
                 if (kind == FYX_LIGHT_SPOT) {
                     // light.rs:706-722: look_at_rh(pos, pos - emit_direction, look_vector normalised)
                     float emit[3], up[3];
@@ -1706,12 +1718,80 @@ __device__ __forceinline__ bool shadow_candidate(const uint32_t nf, const uint32
     return (nf & kShadowNeed) == kShadowNeed && (mask & sp.cam.cam_mask) != 0u;
 }
 
-// pass 2: every node read once (flags, mask, box: 32 B) and tested against every map; one atomic per (warp, map) with an entry
+// The one predicate of the count and emit passes (and of a static batch's "rendered" in the pruner table): the node is in
+// map m's list.  hrow (PRUNE only): the node's row of the pruner table, the maps in which the LOD filter or a static batch
+// above it hides it (nullptr = none); hword carries its word of the current 32 maps from one map to the next.
+template <bool PRUNE>
+__device__ __forceinline__ bool shadow_in_map(const FrustumDev *__restrict__ F, const uint32_t m, const bool cand, const bool test, const bool tame,
+                                              const float2 wx, const float2 wy, const float2 wz, const PackedConsts &kc,
+                                              const uint32_t *hrow, uint32_t &hword)
+{
+    bool ok = test ? frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame) : cand;
+    if (PRUNE && hrow) {
+        if ((m & 31u) == 0u) hword = hrow[m >> 5];
+        ok = ok && !((hword >> (m & 31u)) & 1u);
+    }
+    return ok;
+}
+
+// the node's row of the pruner table: its own (it is a pruner) or its nearest pruner ancestor's children row
+__device__ __forceinline__ const uint32_t *pruner_row(const ShadowParams &sp, const uint32_t pc)
+{
+    if (pc == FYX_NONE) return nullptr;
+    return sp.pr.rows + ((size_t)(pc & ~kPrSelf) * 2u + ((pc & kPrSelf) ? 0u : 1u)) * sp.pr.words;
+}
+
+// The pruner table of a shadow cull, one launch per hierarchy level's pruners [p_lo, p_hi) (parents first), one thread per
+// (pruner, word of 32 maps) — renderer/bundle.rs:898-916, 988-1004 with each map's observer, and Mesh::collect_render_data's
+// Break (scene/mesh/mod.rs:691-725):
+//   self_hidden[p]     = children_hidden[anc(p)] | (LOD object outside its range for the map's observer)
+//   children_hidden[p] = self_hidden[p] | (static batch rendered in the map)
+__global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, const ShadowParams sp, const uint32_t p_lo, const uint32_t p_hi)
+{
+    pdl_wait(); // the map table and its observers
+    const uint32_t W = sp.pr.words;
+    const uint64_t t = (uint64_t)blockIdx.x * kBlock + threadIdx.x;
+    if (t >= (uint64_t)(p_hi - p_lo) * W) return;
+    const uint32_t p = p_lo + (uint32_t)(t / W), w = (uint32_t)(t % W);
+    const uint32_t slot = sp.pr.slot[p], anc = sp.pr.anc[p];
+    uint32_t self = anc != FYX_NONE ? sp.pr.rows[((size_t)anc * 2u + 1u) * W + w] : 0u, rendered = 0u;
+    const uint32_t nf = a.flags[slot], mask = a.mask[slot];
+    const float2 r = sp.pr.range ? sp.pr.range[slot] : make_float2(NAN, NAN);
+    const bool lod = r.x == r.x, batch = (nf & FYX_NODE_STATIC_BATCH) != 0u;
+    const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
+    const float gx = a.G[0][slot].w, gy = a.G[1][slot].w, gz = a.G[2][slot].w; // global_position()
+    PackedConsts kc;
+    kc.one = make_float2(1.0f, 1.0f);
+    kc.negzero = make_float2(-0.0f, -0.0f);
+    const bool cand = shadow_candidate(nf, mask, sp);
+    const bool tame = cand && aabb_is_tame(wx, wy, wz);
+    const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
+    const uint32_t n_maps = *sp.n_maps;
+    uint32_t unused = 0u;
+    for (uint32_t b = 0; b < 32u; ++b) {
+        const uint32_t m = w * 32u + b;
+        if (m >= n_maps) break;
+        if (lod) { // k_lod_level's arithmetic with the map's observer
+            const float *o = sp.pr.obs + (size_t)m * 5;
+            const float dx = FYX_ADD(o[0], -gx), dy = FYX_ADD(o[1], -gy), dz = FYX_ADD(o[2], -gz);
+            const float dist = __fsqrt_rn(FYX_ADD(FYX_ADD(FYX_MUL(dx, dx), FYX_MUL(dy, dy)), FYX_MUL(dz, dz)));
+            const float normalized = __fdiv_rn(FYX_ADD(dist, -o[3]), FYX_ADD(o[4], -o[3]));
+            if (!((normalized >= r.x) && (normalized <= r.y))) self |= 1u << b;
+        }
+        if (batch && shadow_in_map<false>(sp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused)) rendered |= 1u << b;
+    }
+    sp.pr.rows[((size_t)p * 2u) * W + w] = self;
+    sp.pr.rows[((size_t)p * 2u + 1u) * W + w] = self | rendered;
+}
+
+// pass 2: every node read once (flags, mask, box: 32 B; with PRUNE its pruner id: 4 B more) and tested against every map;
+// one atomic per (warp, map) with an entry
+template <bool PRUNE>
 __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, const ShadowParams sp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
     const bool valid = slot < a.cap;
-    uint32_t nf = 0u, mask = 0u;
+    uint32_t nf = 0u, mask = 0u, pc = FYX_NONE;
     float2 wx = make_float2(0.f, 0.f), wy = wx, wz = wx;
     if (valid) {
         nf = a.flags[slot];
@@ -1719,6 +1799,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, con
         wx = ld_stream(a.wa[0] + slot);
         wy = ld_stream(a.wa[1] + slot);
         wz = ld_stream(a.wa[2] + slot);
+        if (PRUNE) pc = sp.pr.col[slot];
     }
     pdl_trigger();
     pdl_wait(); // the map table
@@ -1732,8 +1813,10 @@ __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, con
         const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
         const FrustumDev *__restrict__ F = sp.frusta;
         const uint32_t n_maps = *sp.n_maps;
+        const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
+        uint32_t hword = 0u;
         for (uint32_t m = 0; m < n_maps; ++m) {
-            const bool ok = test ? frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame) : cand;
+            const bool ok = shadow_in_map<PRUNE>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword);
             const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
             if (b && lane == 0u) atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
             any |= b;
@@ -1776,14 +1859,16 @@ __global__ void __launch_bounds__(1024) k_shadow_scan(const ShadowParams sp)
     if (tid == 0) *sp.total = s_base;
 }
 
-// pass 3: the warps that had an entry test again and write their node indices (and, with instances enabled, their slots)
+// pass 3: the warps that had an entry test again and write their node indices (and, with instances enabled, their slots).
+// PRUNE: a warp whose entries would reach past its map's list (first + count) writes nothing and raises E_SHADOW_LIST.
+template <bool PRUNE>
 __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const ShadowParams sp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
     pdl_wait();
     if (!sp.warp_any[slot >> 5]) return; // warp-uniform
     const bool valid = slot < a.cap;
-    uint32_t nf = 0u, mask = 0u, gi = 0u;
+    uint32_t nf = 0u, mask = 0u, gi = 0u, pc = FYX_NONE;
     float2 wx = make_float2(0.f, 0.f), wy = wx, wz = wx;
     if (valid) {
         nf = a.flags[slot];
@@ -1792,6 +1877,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
         wy = ld_stream(a.wa[1] + slot);
         wz = ld_stream(a.wa[2] + slot);
         gi = a.gidx[slot];
+        if (PRUNE) pc = sp.pr.col[slot];
     }
     const bool cand = valid && shadow_candidate(nf, mask, sp);
     PackedConsts kc;
@@ -1802,13 +1888,19 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
     const FrustumDev *__restrict__ F = sp.frusta;
     const uint32_t n_maps = *sp.n_maps;
     const uint32_t lt = (1u << lane) - 1u;
+    const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
+    uint32_t hword = 0u;
     for (uint32_t m = 0; m < n_maps; ++m) {
-        const bool ok = test ? frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame) : cand;
+        const bool ok = shadow_in_map<PRUNE>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword);
         const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
         if (!b) continue;
         uint32_t at = 0u;
         if (lane == 0u) at = atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
         at = __shfl_sync(0xFFFFFFFFu, at, 0);
+        if (PRUNE && at + (uint32_t)__popc(b) > sp.maps[m].first + sp.maps[m].count) { // warp-uniform
+            if (lane == 0u) atomicOr(sp.pr.err, E_SHADOW_LIST);
+            continue;
+        }
         if (ok) {
             sp.entries[at + __popc(b & lt)] = gi;
             if (sp.entry_slot) sp.entry_slot[at + __popc(b & lt)] = slot;
@@ -1818,14 +1910,69 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
 
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
 {
-    k_shadow_frusta<<<1, kBlock, 0, s>>>(a, sp);
-    if (a.cap) launch_pdl(k_shadow_count, grid_for(a.cap), kBlock, 0, s, a, sp);
+    k_shadow_frusta<false><<<1, kBlock, 0, s>>>(a, sp);
+    if (a.cap) launch_pdl(k_shadow_count<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
     launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
 }
 
 void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
 {
-    if (a.cap) launch_pdl(k_shadow_emit, grid_for(a.cap), kBlock, 0, s, a, sp);
+    if (a.cap) launch_pdl(k_shadow_emit<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+}
+
+void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
+                               uint64_t *launches)
+{
+    k_shadow_frusta<true><<<1, kBlock, 0, s>>>(a, sp);
+    ++*launches;
+    for (uint32_t l = 0; l < n_levels; ++l) {
+        const uint32_t lo = pr_level_off[l], hi = pr_level_off[l + 1];
+        if (hi <= lo) continue;
+        launch_pdl(k_shadow_pruners, grid_for((uint64_t)(hi - lo) * sp.pr.words), kBlock, 0, s, a, sp, lo, hi);
+        ++*launches;
+    }
+    if (a.cap) {
+        launch_pdl(k_shadow_count<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+        ++*launches;
+    }
+    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
+    ++*launches;
+}
+
+void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
+{
+    if (a.cap) launch_pdl(k_shadow_emit<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+}
+
+// the pruners mark their own slots of the column
+__global__ void __launch_bounds__(kBlock) k_pruner_mark(const uint32_t n, const uint32_t *pr_slot, uint32_t *col)
+{
+    const uint32_t p = blockIdx.x * kBlock + threadIdx.x;
+    if (p < n) col[pr_slot[p]] = p | kPrSelf;
+}
+
+// one hierarchy level: a node that is no pruner takes the nearest pruner on its parent's path; a pruner records it as its
+// nearest strict pruner ancestor
+__global__ void __launch_bounds__(kBlock) k_pruner_level(const NodeArrays a, const uint32_t lo, const uint32_t hi, uint32_t *col, uint32_t *anc)
+{
+    const uint32_t slot = lo + blockIdx.x * kBlock + threadIdx.x;
+    if (slot >= hi) return;
+    const uint32_t p = a.parent[slot];
+    const uint32_t pv = p != FYX_NONE ? col[p] : FYX_NONE;
+    const uint32_t up = pv != FYX_NONE ? (pv & ~kPrSelf) : FYX_NONE;
+    const uint32_t v = col[slot];
+    if (v != FYX_NONE) anc[v & ~kPrSelf] = up; // a pruner (the column holds nothing else yet)
+    else col[slot] = up;
+}
+
+void launch_pruner_mark(cudaStream_t s, uint32_t n_pruners, const uint32_t *pr_slot, uint32_t *col)
+{
+    if (n_pruners) k_pruner_mark<<<grid_for(n_pruners), kBlock, 0, s>>>(n_pruners, pr_slot, col);
+}
+
+void launch_pruner_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, uint32_t *col, uint32_t *anc)
+{
+    if (hi > lo) k_pruner_level<<<grid_for(hi - lo), kBlock, 0, s>>>(a, lo, hi, col, anc);
 }
 
 } // namespace fyx

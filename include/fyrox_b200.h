@@ -285,7 +285,27 @@ int32_t fyx_get_visible_lights(fyx_ctx *ctx, uint32_t frustum, const uint32_t **
  * pass), as for the spot and point maps; fyx_pack_shadow_instances sorts its instances by the map's look_at_lh.  The
  * perspective's 1 / tan(fov / 2) is evaluated here with the platform's tanf.  cam NULL or csm_enabled = 0: directional
  * lights get no maps.  Same refusals as fyx_cull_shadow_casters, plus FYX_ERR_INVALID_ARGUMENT for an unknown projection
- * kind.  Inputs for which the reference panics (superimposed planes, a collapsed light-space box) give a defined result. */
+ * kind.  Inputs for which the reference panics (superimposed planes, a collapsed light-space box) give a defined result.
+ *
+ * fyx_cull_shadow_casters_pruned: fyx_cull_shadow_casters_csm (same parameters, same map table: the same maps in the same
+ * order, view_projection bit for bit) where every map's list is from_graph with that map's own LOD filter and static-batch
+ * pruning, as the reference builds one RenderDataBundleStorage per map (renderer/bundle.rs:873-1009):
+ *   - LOD filter: the ranges of fyx_set_lod_ranges, whenever any node has one (fyx_set_observers takes no part: it
+ *     describes the frusta of fyx_cull).  The map's observer is the light's global position with z_near 0.01 and z_far
+ *     light_radius for a spot map and each cube face of a point light (light.rs:700-728, shadow/point.rs:162-190), and for
+ *     cascade i the look_at_lh eye center + light_direction with the slice's z_near and guarded z_far (shadow/csm.rs:195-270).
+ *     A LOD object whose normalised distance (dist − z_near) / (z_far − z_near) lies outside its [begin, end] hides itself
+ *     and its whole sub-tree in that map only.
+ *   - Static batches: an FYX_NODE_STATIC_BATCH node that is in a map's list (frustum, camera mask, cast_shadows) hides its
+ *     sub-tree in that map (Mesh::collect_render_data's Break, scene/mesh/mod.rs:691-725); where it is not in the list its
+ *     children are visited as usual.
+ * A static batch's shadow instance carries the identity world matrix (fyx_pack_shadow_instances), as on the camera path.
+ * The per-map state grows with the pruners (LOD objects and static batches), not with nodes x maps: one u32 per slot (the
+ * nearest pruner on the node's path, rebuilt by the first pruned cull after fyx_set_topology, fyx_set_lod_ranges or a
+ * fyx_set_flags that changes an FYX_NODE_STATIC_BATCH bit) and two rows of ceil(maps / 32) words per pruner.  On a context
+ * with no LOD range and no static batch it runs exactly the kernels of fyx_cull_shadow_casters_csm; fyx_cull_shadow_casters_csm
+ * equals fyx_cull_shadow_casters_pruned on such a context and refuses (FYX_ERR_STATE) on any other.  Refusals otherwise as
+ * fyx_cull_shadow_casters_csm; FYX_ERR_OUT_OF_MEMORY when the pruner table does not fit. */
 #define FYX_LIGHT_UNKNOWN 0u
 #define FYX_LIGHT_SPOT 1u
 #define FYX_LIGHT_POINT 2u
@@ -327,6 +347,8 @@ typedef struct fyx_csm_camera {
 int32_t fyx_set_csm_options(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const fyx_csm_options *opts);
 int32_t fyx_cull_shadow_casters_csm(fyx_ctx *ctx, uint32_t camera_frustum, const float camera_translation[3], const fyx_shadow_settings *settings,
                                     const fyx_csm_camera *cam);
+int32_t fyx_cull_shadow_casters_pruned(fyx_ctx *ctx, uint32_t camera_frustum, const float camera_translation[3],
+                                       const fyx_shadow_settings *settings, const fyx_csm_camera *cam /* NULL = no cascades */);
 /* Result of the last fyx_cull_shadow_casters: pinned host copies ... */
 int32_t fyx_get_shadow_maps(fyx_ctx *ctx, const fyx_shadow_map **out_maps, uint32_t *out_n_maps, const uint32_t **out_entries);
 /* ... or the device arrays (*out_n_maps is a host value). */
