@@ -191,6 +191,28 @@ class fyx_csm_camera(C.Structure):
                 ("frame_size", C.c_float * 2), ("view_matrix", C.c_float * 16), ("csm_enabled", C.c_uint32)]
 
 
+PROJECTION_NONE = 0xFFFFFFFF
+PROBE_UPDATE_ONCE, PROBE_UPDATE_EACH_FRAME = 0, 1
+OBSERVER_PROBE_FACE, OBSERVER_CAMERA = 0, 1
+
+
+class fyx_camera(C.Structure):
+    _fields_ = [("enabled", C.c_uint32), ("projection", C.c_uint32), ("fov_or_vertical_size", C.c_float), ("z_near", C.c_float),
+                ("z_far", C.c_float), ("frame_size", C.c_float * 2)]
+
+
+class fyx_reflection_probe(C.Structure):
+    _fields_ = [("present", C.c_uint32), ("update_mode", C.c_uint32), ("z_near", C.c_float), ("z_far", C.c_float),
+                ("rendering_position", C.c_float * 3)]
+
+
+class fyx_scene_observer(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("node", "kind", "face", "render_mask", "first", "count", "lights_first", "lights_count",
+                                          "environment_map")] + [
+        ("translation", C.c_float * 3), ("z_near", C.c_float), ("z_far", C.c_float), ("view", C.c_float * 16),
+        ("projection", C.c_float * 16), ("view_projection", C.c_float * 16)]
+
+
 # every symbol include/fyrox_b200.h declares: name -> (restype, argtypes)
 ctx_p = C.c_void_p
 SYMBOLS = {
@@ -277,6 +299,19 @@ SYMBOLS = {
     "fyx_pack_shadow_bone_matrices": (C.c_int32, [ctx_p]),
     "fyx_get_shadow_bone_matrix_blocks_device": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
     "fyx_get_shadow_bone_matrix_block": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
+    "fyx_set_cameras": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "fyx_set_reflection_probes": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "fyx_force_reflection_probe_update": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
+    "fyx_cull_scene_observers": (C.c_int32, [ctx_p, f32p]),
+    "fyx_get_scene_observers": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
+    "fyx_get_scene_observers_device": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
+    "fyx_pack_scene_observer_instances": (C.c_int32, [ctx_p]),
+    "fyx_get_scene_observer_instances": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),
+    "fyx_get_scene_observer_instances_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),
+    "fyx_get_scene_observer_instance_surfaces": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(u32p)]),
+    "fyx_pack_scene_observer_bone_matrices": (C.c_int32, [ctx_p]),
+    "fyx_get_scene_observer_bone_matrix_blocks_device": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
+    "fyx_get_scene_observer_bone_matrix_block": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     "fyx_set_blend_shapes": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p]),
     "fyx_set_blend_shape_weights": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "fyx_allgather_visible": (C.c_int32, [ctx_p]),

@@ -404,6 +404,75 @@ class Context:
         self._chk(self._lib.fyx_get_shadow_maps_device(self._h, C.byref(pm), C.byref(n), C.byref(pe)))
         return pm.value, n.value, pe.value
 
+    # ---- N4 (scene observers) ----
+    CAMERA_DTYPE = np.dtype([("enabled", "<u4"), ("projection", "<u4"), ("fov_or_vertical_size", "<f4"), ("z_near", "<f4"), ("z_far", "<f4"),
+                             ("frame_size", "<f4", 2)])
+    PROBE_DTYPE = np.dtype([("present", "<u4"), ("update_mode", "<u4"), ("z_near", "<f4"), ("z_far", "<f4"), ("rendering_position", "<f4", 3)])
+    SCENE_OBSERVER_DTYPE = np.dtype([(n, "<u4") for n in ("node", "kind", "face", "render_mask", "first", "count", "lights_first", "lights_count",
+                                                          "environment_map")]
+                                    + [("translation", "<f4", 3), ("z_near", "<f4"), ("z_far", "<f4"), ("view", "<f4", 16),
+                                       ("projection", "<f4", 16), ("view_projection", "<f4", 16)])
+
+    def set_cameras(self, idx, cameras):
+        """Camera records (CAMERA_DTYPE) of the nodes `idx`; projection PROJECTION_NONE removes a node's record."""
+        idx = _u32(idx)
+        recs = np.ascontiguousarray(cameras, self.CAMERA_DTYPE)
+        self._chk(self._lib.fyx_set_cameras(self._h, recs.size, _ptr(idx), recs.ctypes.data))
+
+    def set_reflection_probes(self, idx, probes):
+        """Reflection-probe records (PROBE_DTYPE) of the nodes `idx`; present 0 removes a node's record."""
+        idx = _u32(idx)
+        recs = np.ascontiguousarray(probes, self.PROBE_DTYPE)
+        self._chk(self._lib.fyx_set_reflection_probes(self._h, recs.size, _ptr(idx), recs.ctypes.data))
+
+    def force_reflection_probe_update(self, idx):
+        idx = _u32(idx)
+        self._chk(self._lib.fyx_force_reflection_probe_update(self._h, idx.size, _ptr(idx)))
+
+    def cull_scene_observers(self, frame_size):
+        """ObserversCollection::from_scene and one from_graph per observer (fyx_cull_scene_observers)."""
+        fs = np.ascontiguousarray(frame_size, np.float32).reshape(2)
+        self._chk(self._lib.fyx_cull_scene_observers(self._h, fs.ctypes.data_as(L.f32p)))
+
+    def get_scene_observers(self):
+        """(table, entries, light_entries): table is a SCENE_OBSERVER_DTYPE array; observer o's visible set is
+        entries[first:first + count], its lights light_entries[lights_first:lights_first + lights_count]."""
+        pt, pe, pl = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        n = C.c_uint32()
+        self._chk(self._lib.fyx_get_scene_observers(self._h, C.byref(pt), C.byref(n), C.byref(pe), C.byref(pl)))
+        if not n.value:
+            return np.empty(0, self.SCENE_OBSERVER_DTYPE), np.empty(0, np.uint32), np.empty(0, np.uint32)
+        table = np.frombuffer((C.c_char * (n.value * self.SCENE_OBSERVER_DTYPE.itemsize)).from_address(pt.value), self.SCENE_OBSERVER_DTYPE).copy()
+        total = int(table["first"][-1]) + int(table["count"][-1])
+        ltotal = int(table["lights_first"][-1]) + int(table["lights_count"][-1])
+        entries = np.ctypeslib.as_array(C.cast(pe.value, L.u32p), shape=(max(total, 1),))[:total].copy()
+        lights = np.ctypeslib.as_array(C.cast(pl.value, L.u32p), shape=(max(ltotal, 1),))[:ltotal].copy()
+        return table, entries, lights
+
+    def get_scene_observers_device(self):
+        """(device pointer of the table, number of observers, device pointers of the entries and light entries)."""
+        pt, pe, pl = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        n = C.c_uint32()
+        self._chk(self._lib.fyx_get_scene_observers_device(self._h, C.byref(pt), C.byref(n), C.byref(pe), C.byref(pl)))
+        return pt.value, n.value, pe.value, pl.value
+
+    def pack_scene_observer_instances(self):
+        """Pack the instances of every observer of the last cull_scene_observers (made with enable_instances) in one call."""
+        self._chk(self._lib.fyx_pack_scene_observer_instances(self._h))
+
+    def get_scene_observer_instances(self, observer: int) -> dict:
+        """Instances of observer `observer`: the same dict as pack_instances, for its view and view_projection."""
+        out = L.fyx_instances()
+        self._chk(self._lib.fyx_get_scene_observer_instances(self._h, observer, C.byref(out)))
+        return self._instances_dict(out, self._instance_surfaces(self._lib.fyx_get_scene_observer_instance_surfaces, observer, out.count))
+
+    def pack_scene_observer_bone_matrices(self):
+        self._chk(self._lib.fyx_pack_scene_observer_bone_matrices(self._h))
+
+    def get_scene_observer_bone_matrix_block(self, observer: int, instance: int):
+        """(255,16) f32 block of instance `instance` of observer `observer`, or None for an unskinned instance."""
+        return self._bone_matrix_block(self._lib.fyx_get_scene_observer_bone_matrix_block, observer, instance)
+
     # ---- N2: animation sampling on the device ----
     KEY_DTYPE = np.dtype([("location", "<f4"), ("value", "<f4"), ("kind", "<u4"), ("left_tangent", "<f4"), ("right_tangent", "<f4")])
     TRACK_DTYPE = np.dtype([("target_node", "<u4"), ("binding", "<u4"), ("value_kind", "<u4"), ("enabled", "<u4"), ("n_curves", "<u4"),

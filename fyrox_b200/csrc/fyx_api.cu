@@ -388,6 +388,22 @@ struct fyx_ctx {
     std::vector<uint32_t> pr_level_off; // pruner ids per hierarchy level (pruners are numbered in slot order)
     DevBuf b_pr_col, b_pr_slot, b_pr_anc, b_pr_rows, b_pr_obs;
 
+    // N4 scene observers (fyx_drawprep.inl): camera and reflection-probe records by node index, their device table (due
+    // probes, then cameras, each in pool order; rebuilt when a record or the topology changes), the observer cull's outputs
+    std::vector<fyx_camera> cam_src;            // projection FYX_PROJECTION_NONE = no record
+    std::vector<float> cam_m22;                 // 1 / tan(fov / 2) or vertical_size
+    std::vector<fyx_reflection_probe> probe_src; // present 0 = no record
+    std::vector<uint8_t> probe_due;             // set or forced since the table was built: its rendered bit starts at 0
+    std::vector<uint32_t> ob_rec_node;          // node of each record of the device table
+    bool obs_table_dirty = false;
+    uint32_t n_ob_recs = 0;
+    DevBuf b_ob_recs, b_ob_table, b_ob_scratch, b_ob_frusta, b_ob_maps, b_ob_views, b_ob_counts, b_ob_warp_any, b_ob_small, b_ob_entries,
+        b_ob_slots, b_ob_lcounts, b_ob_best, b_ob_lraw, b_ob_lights;
+    PinnedBuf h_ob_small, h_ob_table, h_ob_entries, h_ob_lights; // n_obs, total, light total; host copies of the results
+    uint32_t ob_n = 0, ob_total = 0, ob_light_total = 0;
+    bool ob_valid = false, ob_on_host = false, ob_have_slots = false, ob_slots_stale = false;
+    InstPack obi; // their instances, a segment per observer
+
     // N3 draw-prep (fyx_drawprep.inl)
     bool instances_enabled = false, rank_on_device = false;
     uint32_t n_bundle_ids = 1;
@@ -1102,6 +1118,13 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     if (!same_capacity) c->dfs_rank.clear(); // indexed by node: stays valid while the pool capacity does
     c->rank_on_device = false; // re-derived from dfs_rank in the new slot order
     c->sh_slots_stale = true;  // the last shadow cull's entry slots
+    c->ob_slots_stale = true;  // and the last observer cull's
+    // camera and probe records stay with their node indices; a node that is not alive any more drops its record
+    for (size_t i = 0; i < c->cam_src.size(); ++i)
+        if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->cam_src[i].projection = FYX_PROJECTION_NONE;
+    for (size_t i = 0; i < c->probe_src.size(); ++i)
+        if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->probe_src[i].present = 0u;
+    c->obs_table_dirty = true;
     c->ms_dirty = c->have_ms;  // the per-slot surface table too (the CSR itself is by node)
     if (c->ms_of_node.size() < capacity) c->ms_of_node.resize(capacity, make_uint2(0u, 0u));
     c->anim_csr_dirty = true; // animated nodes are addressed by slot

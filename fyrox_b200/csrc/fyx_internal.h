@@ -235,6 +235,18 @@ struct ShadowLightDev {
     float distance_or_radius;
     fyx_csm_options csm; // directional lights: the cascades' FrustumSplitOptions
 };
+// one camera or reflection probe of fyx_cull_scene_observers, in the order of the observers they give
+struct ObserverRecDev {
+    uint32_t slot;
+    uint32_t kind;              // FYX_OBSERVER_*
+    uint32_t mode;              // camera: FYX_PROJECTION_*; probe: FYX_PROBE_UPDATE_*
+    uint32_t enabled;           // camera: Camera::is_enabled
+    uint32_t rendered;          // probe: emitted since its record was set or its update forced
+    uint32_t emitted;           // probe: emitted by the current call (k_observer_views); folded into `rendered` once it succeeds
+    float m22_or_vertical_size; // camera: 1 / tan(fov / 2) (evaluated on the host) or vertical_size
+    float z_near, z_far;
+    float v[3];                 // camera: frame size (0,0 = the call's); probe: rendering_position
+};
 // the camera of the cascaded shadow maps (fyx_cull_shadow_casters_csm); enabled = 0: directional lights get no maps
 struct CsmCameraDev {
     uint32_t enabled;
@@ -280,6 +292,21 @@ struct ShadowParams {
         uint32_t *err;          // the context's error word (E_SHADOW_LIST)
     } pr;
 };
+// The scene's observers (fyx_cull_scene_observers).  The node passes take the observers as their maps: ShadowParams' `maps` /
+// `frusta` / `views` / `counts` / `entries` hold one per observer, each frustum with its observer's cam_mask, and the node
+// test takes each observer's mask and no cast_shadows (shadow_in_map<.., OBS>).  What only the observer kernels read:
+struct ObserverParams {
+    ObserverRecDev *recs;       // [n_recs] due probes' and cameras' records: probes in pool order, then cameras
+    uint32_t n_recs;
+    float frame_size[2];        // the call's frame size
+    float probe_m22;            // 1 / tan(FRAC_PI_2 / 2), evaluated on the host
+    fyx_scene_observer *table;  // [max observers]
+    uint32_t *light_counts;     // [max observers * kCountStride]: light-list counts, then write cursors
+    uint32_t *best;             // [max observers]: environment map node + 1 (0 = none)
+    uint32_t *light_total;      // one u32
+    uint32_t *light_raw;        // [light_total] the light lists in emission order
+    uint32_t *light_entries;    // [light_total] the same, each list in ascending node index
+};
 constexpr uint32_t kPrSelf = 1u << 31; // bit of ShadowParams::Prune::col: the node is the pruner itself
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp); // map table + frusta, count pass, scan
 void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);
@@ -288,6 +315,15 @@ void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams 
 void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
                                uint64_t *launches);
 void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);
+// fyx_cull_scene_observers: the observer table (one CTA), the pruner table when pr_level_off is given (as the pruned shadow
+// cull), the count pass over the observers' frusta, the scan, the light counts and environment maps, the light scan
+void launch_observers(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, const uint32_t *pr_level_off,
+                      uint32_t n_levels, uint64_t *launches);
+// then the lists: the emit pass, the light emit pass and the light lists' sort (one CTA per observer)
+void launch_observers_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, bool pruned, uint32_t n_obs,
+                           uint64_t *launches);
+// after a call that succeeded: the probes it emitted count as rendered (probe.rs `updated`)
+void launch_observers_commit(cudaStream_t s, ObserverRecDev *recs, uint32_t n_recs);
 // the pruner column ShadowParams::Prune::col / anc from the pruners' slots: col must hold FYX_NONE everywhere; then one launch per
 // hierarchy level [level_off[l], level_off[l + 1]) from level `first` on, parents first
 void launch_pruner_mark(cudaStream_t s, uint32_t n_pruners, const uint32_t *pr_slot, uint32_t *col);

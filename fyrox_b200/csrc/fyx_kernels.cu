@@ -1712,21 +1712,31 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
 }
 
 // the node's part of from_graph for a shadow map, minus the frustum test: alive, renderable, reachable, globally visible and
-// enabled, cast_shadows, render mask against the camera's (every map carries the camera's mask)
+// enabled, cast_shadows, render mask against the camera's (every map carries the camera's mask).  OBS (the scene's observers,
+// fyx_cull_scene_observers): no shadow pass, so no cast_shadows, and each observer's own mask, tested per map by shadow_in_map.
+template <bool OBS>
 __device__ __forceinline__ bool shadow_candidate(const uint32_t nf, const uint32_t mask, const ShadowParams &sp)
 {
+    if (OBS) return (nf & kNeedBits) == kNeedBits;
     return (nf & kShadowNeed) == kShadowNeed && (mask & sp.cam.cam_mask) != 0u;
 }
 
 // The one predicate of the count and emit passes (and of a static batch's "rendered" in the pruner table): the node is in
 // map m's list.  hrow (PRUNE only): the node's row of the pruner table, the maps in which the LOD filter or a static batch
-// above it hides it (nullptr = none); hword carries its word of the current 32 maps from one map to the next.
-template <bool PRUNE>
+// above it hides it (nullptr = none); hword carries its word of the current 32 maps from one map to the next.  OBS: the
+// node's render mask against map m's (should_be_rendered, scene/node/mod.rs:231-256).
+template <bool PRUNE, bool OBS>
 __device__ __forceinline__ bool shadow_in_map(const FrustumDev *__restrict__ F, const uint32_t m, const bool cand, const bool test, const bool tame,
                                               const float2 wx, const float2 wy, const float2 wz, const PackedConsts &kc,
-                                              const uint32_t *hrow, uint32_t &hword)
+                                              const uint32_t *hrow, uint32_t &hword, const uint32_t mask)
 {
-    bool ok = test ? frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame) : cand;
+    bool ok;
+    if (OBS) {
+        ok = cand && (mask & F[m].cam_mask) != 0u;
+        if (ok && test) ok = frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame);
+    } else {
+        ok = test ? frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame) : cand;
+    }
     if (PRUNE && hrow) {
         if ((m & 31u) == 0u) hword = hrow[m >> 5];
         ok = ok && !((hword >> (m & 31u)) & 1u);
@@ -1746,6 +1756,7 @@ __device__ __forceinline__ const uint32_t *pruner_row(const ShadowParams &sp, co
 // Break (scene/mesh/mod.rs:691-725):
 //   self_hidden[p]     = children_hidden[anc(p)] | (LOD object outside its range for the map's observer)
 //   children_hidden[p] = self_hidden[p] | (static batch rendered in the map)
+template <bool OBS>
 __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, const ShadowParams sp, const uint32_t p_lo, const uint32_t p_hi)
 {
     pdl_wait(); // the map table and its observers
@@ -1763,7 +1774,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, c
     PackedConsts kc;
     kc.one = make_float2(1.0f, 1.0f);
     kc.negzero = make_float2(-0.0f, -0.0f);
-    const bool cand = shadow_candidate(nf, mask, sp);
+    const bool cand = shadow_candidate<OBS>(nf, mask, sp);
     const bool tame = cand && aabb_is_tame(wx, wy, wz);
     const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
     const uint32_t n_maps = *sp.n_maps;
@@ -1778,7 +1789,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, c
             const float normalized = __fdiv_rn(FYX_ADD(dist, -o[3]), FYX_ADD(o[4], -o[3]));
             if (!((normalized >= r.x) && (normalized <= r.y))) self |= 1u << b;
         }
-        if (batch && shadow_in_map<false>(sp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused)) rendered |= 1u << b;
+        if (batch && shadow_in_map<false, OBS>(sp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused, mask)) rendered |= 1u << b;
     }
     sp.pr.rows[((size_t)p * 2u) * W + w] = self;
     sp.pr.rows[((size_t)p * 2u + 1u) * W + w] = self | rendered;
@@ -1786,7 +1797,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, c
 
 // pass 2: every node read once (flags, mask, box: 32 B; with PRUNE its pruner id: 4 B more) and tested against every map;
 // one atomic per (warp, map) with an entry
-template <bool PRUNE>
+template <bool PRUNE, bool OBS>
 __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, const ShadowParams sp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
@@ -1803,7 +1814,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, con
     }
     pdl_trigger();
     pdl_wait(); // the map table
-    const bool cand = valid && shadow_candidate(nf, mask, sp);
+    const bool cand = valid && shadow_candidate<OBS>(nf, mask, sp);
     uint32_t any = 0u;
     if (__any_sync(0xFFFFFFFFu, cand)) {
         PackedConsts kc;
@@ -1816,7 +1827,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, con
         const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
         uint32_t hword = 0u;
         for (uint32_t m = 0; m < n_maps; ++m) {
-            const bool ok = shadow_in_map<PRUNE>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword);
+            const bool ok = shadow_in_map<PRUNE, OBS>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
             const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
             if (b && lane == 0u) atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
             any |= b;
@@ -1861,7 +1872,7 @@ __global__ void __launch_bounds__(1024) k_shadow_scan(const ShadowParams sp)
 
 // pass 3: the warps that had an entry test again and write their node indices (and, with instances enabled, their slots).
 // PRUNE: a warp whose entries would reach past its map's list (first + count) writes nothing and raises E_SHADOW_LIST.
-template <bool PRUNE>
+template <bool PRUNE, bool OBS>
 __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const ShadowParams sp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
@@ -1879,7 +1890,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
         gi = a.gidx[slot];
         if (PRUNE) pc = sp.pr.col[slot];
     }
-    const bool cand = valid && shadow_candidate(nf, mask, sp);
+    const bool cand = valid && shadow_candidate<OBS>(nf, mask, sp);
     PackedConsts kc;
     kc.one = make_float2(1.0f, 1.0f);
     kc.negzero = make_float2(-0.0f, -0.0f);
@@ -1891,7 +1902,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
     const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
     uint32_t hword = 0u;
     for (uint32_t m = 0; m < n_maps; ++m) {
-        const bool ok = shadow_in_map<PRUNE>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword);
+        const bool ok = shadow_in_map<PRUNE, OBS>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
         const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
         if (!b) continue;
         uint32_t at = 0u;
@@ -1911,13 +1922,26 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
 {
     k_shadow_frusta<false><<<1, kBlock, 0, s>>>(a, sp);
-    if (a.cap) launch_pdl(k_shadow_count<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    if (a.cap) launch_pdl(k_shadow_count<false, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
     launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
 }
 
 void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
 {
-    if (a.cap) launch_pdl(k_shadow_emit<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    if (a.cap) launch_pdl(k_shadow_emit<false, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+}
+
+// the pruner table, one launch per hierarchy level that holds pruners (parents first)
+template <bool OBS>
+static void launch_pruner_table(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
+                                uint64_t *launches)
+{
+    for (uint32_t l = 0; l < n_levels; ++l) {
+        const uint32_t lo = pr_level_off[l], hi = pr_level_off[l + 1];
+        if (hi <= lo) continue;
+        launch_pdl(k_shadow_pruners<OBS>, grid_for((uint64_t)(hi - lo) * sp.pr.words), kBlock, 0, s, a, sp, lo, hi);
+        ++*launches;
+    }
 }
 
 void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
@@ -1925,14 +1949,9 @@ void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const Shadow
 {
     k_shadow_frusta<true><<<1, kBlock, 0, s>>>(a, sp);
     ++*launches;
-    for (uint32_t l = 0; l < n_levels; ++l) {
-        const uint32_t lo = pr_level_off[l], hi = pr_level_off[l + 1];
-        if (hi <= lo) continue;
-        launch_pdl(k_shadow_pruners, grid_for((uint64_t)(hi - lo) * sp.pr.words), kBlock, 0, s, a, sp, lo, hi);
-        ++*launches;
-    }
+    launch_pruner_table<false>(s, a, sp, pr_level_off, n_levels, launches);
     if (a.cap) {
-        launch_pdl(k_shadow_count<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+        launch_pdl(k_shadow_count<true, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
         ++*launches;
     }
     launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
@@ -1941,7 +1960,248 @@ void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const Shadow
 
 void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
 {
-    if (a.cap) launch_pdl(k_shadow_emit<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    if (a.cap) launch_pdl(k_shadow_emit<true, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+}
+
+// ------------------------------------------------------------------------------------------------
+// N4 scene observers (fyx_cull_scene_observers): ObserversCollection::from_scene (renderer/observer.rs:88-153) with
+// Camera::calculate_matrices (scene/camera.rs:454-462), then one from_graph per observer (renderer/mod.rs:1034-1047) through
+// the shadow maps' node passes: the observers are the maps.
+// ------------------------------------------------------------------------------------------------
+// one observer: its table row, its map row (what k_shadow_scan and the pack read), its frustum with the node's render mask,
+// its view matrix and its LOD observer (translation, z_near, z_far)
+__device__ __forceinline__ void observer_out(const ShadowParams &sp, const ObserverParams &op, const uint32_t m, const uint32_t node, const uint32_t kind, const uint32_t face,
+                                             const uint32_t mask, const float *t, const float z_near, const float z_far, const float *P,
+                                             const float *V)
+{
+    float VP[16];
+    mat4_mul(P, V, VP);
+    fyx_scene_observer &o = op.table[m];
+    o.node = node;
+    o.kind = kind;
+    o.face = face;
+    o.render_mask = mask;
+    o.first = o.count = o.lights_first = o.lights_count = 0u;
+    o.environment_map = FYX_NONE;
+    for (int k = 0; k < 3; ++k) o.translation[k] = t[k];
+    o.z_near = z_near;
+    o.z_far = z_far;
+    for (int k = 0; k < 16; ++k) {
+        o.view[k] = V[k];
+        o.projection[k] = P[k];
+        o.view_projection[k] = VP[k];
+        sp.views[(size_t)m * 16 + k] = V[k];
+    }
+    fyx_shadow_map &mp = sp.maps[m];
+    mp.light = node;
+    mp.face = face;
+    mp.cascade = 0u;
+    mp.first = mp.count = 0u;
+    for (int k = 0; k < 16; ++k) mp.view_projection[k] = VP[k];
+    // renderer/bundle.rs:893-896: from_view_projection_matrix(..).unwrap_or_default()
+    if (!frustum_from_view_projection(VP, sp.scratch[m])) sp.scratch[m] = sp.csm.fallback;
+    to_dev_frustum(sp.scratch[m], mask, 0u, sp.frusta[m]);
+    if (sp.pr.obs) map_observer(sp.pr.obs + (size_t)m * 5, t, z_near, z_far);
+}
+
+// One CTA: the records in order (due probes' six faces, then cameras), the same ordered block scan as k_shadow_frusta
+__global__ void __launch_bounds__(kBlock) k_observer_views(const NodeArrays a, const ShadowParams sp, const ObserverParams op)
+{
+    __shared__ uint32_t s_warp[kBlock / 32];
+    __shared__ uint32_t s_base;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    pdl_trigger();
+    if (tid == 0) s_base = 0u;
+    for (uint32_t base = 0; base < op.n_recs; base += kBlock) {
+        const uint32_t i = base + tid;
+        uint32_t n_obs = 0u;
+        ObserverRecDev R{};
+        if (i < op.n_recs) {
+            R = op.recs[i];
+            const uint32_t nf = a.flags[R.slot];
+            constexpr uint32_t need = FYX_NODE_ALIVE | FYX_NODE_GLOBAL_ENABLED; // observer.rs:91
+            if ((nf & need) == need) {
+                if (R.kind == FYX_OBSERVER_CAMERA) n_obs = R.enabled ? 1u : 0u;
+                else if (R.mode == FYX_PROBE_UPDATE_EACH_FRAME || !R.rendered) n_obs = 6u; // probe.rs:276-290, observer.rs:99-102
+            }
+            // observer.rs:102 marks the probe updated; here that waits for the call to succeed (k_observer_commit), so a call
+            // that fails leaves the probe due
+            op.recs[i].emitted = R.kind == FYX_OBSERVER_PROBE_FACE && n_obs ? 1u : 0u;
+        }
+        uint32_t incl = n_obs;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= (uint32_t)o) incl += v;
+        }
+        if (lane == 31u) s_warp[warp] = incl;
+        __syncthreads();
+        uint32_t first = s_base + incl - n_obs;
+        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
+        if (n_obs) {
+            const uint32_t slot = R.slot, node = a.gidx[slot], mask = a.mask[slot];
+            const float4 r0 = a.G[0][slot], r1 = a.G[1][slot], r2 = a.G[2][slot];
+            const float pos[3] = {r0.w, r1.w, r2.w};
+            float P[16], V[16];
+            if (R.kind == FYX_OBSERVER_CAMERA) {
+                // camera.rs:454-462: look = column 2, up = column 1, both as they are
+                const float target[3] = {FYX_ADD(pos[0], r0.z), FYX_ADD(pos[1], r1.z), FYX_ADD(pos[2], r2.z)};
+                const float up[3] = {r0.y, r1.y, r2.y};
+                look_at_rh(pos, target, up, V);
+                const bool own = R.v[0] != 0.0f || R.v[1] != 0.0f; // a render target's size (camera.rs:813-826)
+                camera_projection(R.mode, R.m22_or_vertical_size, R.z_near, R.z_far, own ? R.v[0] : op.frame_size[0],
+                                  own ? R.v[1] : op.frame_size[1], P);
+                observer_out(sp, op, first, node, FYX_OBSERVER_CAMERA, 0u, mask, pos, R.z_near, R.z_far, P, V);
+            } else {
+                // observer.rs:104-145: perspective fov 90°, aspect 1 (a cube face); translation = global_rendering_position
+                const float t[3] = {FYX_ADD(pos[0], R.v[0]), FYX_ADD(pos[1], R.v[1]), FYX_ADD(pos[2], R.v[2])};
+                camera_projection(FYX_PROJECTION_PERSPECTIVE, op.probe_m22, R.z_near, R.z_far, 1.0f, 1.0f, P);
+#pragma unroll 1
+                for (uint32_t k = 0; k < 6u; ++k) {
+                    const float target[3] = {FYX_ADD(t[0], c_face_look[k][0]), FYX_ADD(t[1], c_face_look[k][1]), FYX_ADD(t[2], c_face_look[k][2])};
+                    const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
+                    look_at_rh(t, target, up, V);
+                    observer_out(sp, op, first + k, node, FYX_OBSERVER_PROBE_FACE, k, mask, t, R.z_near, R.z_far, P, V);
+                }
+            }
+        }
+        __syncthreads();
+        if (tid == kBlock - 1) s_base = first + n_obs;
+        __syncthreads();
+    }
+    if (tid == 0) *sp.n_maps = s_base;
+}
+
+// The light lists and environment maps of every observer in one pass over the flag column (k_cull_lights and
+// k_select_probes for any number of observers): EMIT = false counts each observer's lights and picks its environment map,
+// EMIT = true writes the lights at the cursors of k_observer_light_scan.
+template <bool EMIT>
+__global__ void __launch_bounds__(kBlock) k_observer_lights(const NodeArrays a, const ShadowParams sp, const ObserverParams op)
+{
+    const uint32_t slot = blockIdx.x * kBlock + threadIdx.x;
+    pdl_wait();
+    if (slot >= a.cap) return;
+    const uint32_t nf = a.flags[slot];
+    constexpr uint32_t need = FYX_NODE_ALIVE | FYX_NODE_LIGHT | FYX_NODE_GLOBAL_VISIBILITY | FYX_NODE_GLOBAL_ENABLED;
+    constexpr uint32_t probe = FYX_NODE_ALIVE | FYX_NODE_REFLECTION_PROBE;
+    const bool light = (nf & need) == need, env = !EMIT && (nf & probe) == probe;
+    if (!light && !env) return;
+    const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
+    PackedConsts kc;
+    kc.one = make_float2(1.0f, 1.0f);
+    kc.negzero = make_float2(-0.0f, -0.0f);
+    const bool tame = aabb_is_tame(wx, wy, wz);
+    const uint32_t gi = a.gidx[slot];
+    const uint32_t n = *sp.n_maps;
+    for (uint32_t m = 0; m < n; ++m) {
+        if (light && frustum_intersects_aabb(sp.frusta[m], wx, wy, wz, kc, tame)) {
+            uint32_t *c = op.light_counts + (size_t)m * kCountStride;
+            if (EMIT) op.light_raw[atomicAdd(c, 1u)] = gi;
+            else atomicAdd(c, 1u);
+        }
+        // renderer/bundle.rs:918-925 (cameras only, renderer/mod.rs:1045-1047): the last probe in pool order containing the observer
+        if (env && op.table[m].kind == FYX_OBSERVER_CAMERA) {
+            const float px = op.table[m].translation[0], py = op.table[m].translation[1], pz = op.table[m].translation[2];
+            if (px >= wx.x && px <= wx.y && py >= wy.x && py <= wy.y && pz >= wz.x && pz <= wz.y) atomicMax(op.best + m, gi + 1u);
+        }
+    }
+}
+
+// One CTA: the table's lists (from the map rows of k_shadow_scan), the light lists' places, the environment maps
+__global__ void __launch_bounds__(1024) k_observer_light_scan(const ShadowParams sp, const ObserverParams op)
+{
+    __shared__ uint32_t s_warp[32];
+    __shared__ uint32_t s_base;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    pdl_wait();
+    if (tid == 0) s_base = 0u;
+    const uint32_t n = *sp.n_maps;
+    for (uint32_t base = 0; base < n; base += 1024u) {
+        const uint32_t m = base + tid;
+        const uint32_t c = m < n ? op.light_counts[(size_t)m * kCountStride] : 0u;
+        uint32_t incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= (uint32_t)o) incl += v;
+        }
+        if (lane == 31u) s_warp[warp] = incl;
+        __syncthreads();
+        uint32_t first = s_base + incl - c;
+        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
+        if (m < n) {
+            fyx_scene_observer &o = op.table[m];
+            o.first = sp.maps[m].first;
+            o.count = sp.maps[m].count;
+            o.lights_first = first;
+            o.lights_count = c;
+            o.environment_map = op.best[m] ? op.best[m] - 1u : FYX_NONE;
+            op.light_counts[(size_t)m * kCountStride] = first;
+        }
+        __syncthreads();
+        if (tid == 1023u) s_base = first + c;
+        __syncthreads();
+    }
+    if (tid == 0) *op.light_total = s_base;
+}
+
+// One CTA per observer: its light list into ascending node index (pool order, as the reference's pair_iter).  Node
+// indices are distinct, so an entry's place is the number of smaller entries.  That is n² compares for a list of n lights,
+// n² / 256 per thread: it assumes lists of at most a few thousand lights (4 096 lights = 65 536 compares per thread, tens of µs;
+// the observer benchmark's scene has 8 per observer).  A scene whose observers each see far more lights wants a segmented
+// radix sort here.
+__global__ void __launch_bounds__(kBlock) k_observer_light_sort(const ObserverParams op)
+{
+    pdl_wait();
+    const fyx_scene_observer &o = op.table[blockIdx.x];
+    const uint32_t f = o.lights_first, n = o.lights_count;
+    const uint32_t *src = op.light_raw + f;
+    for (uint32_t i = threadIdx.x; i < n; i += kBlock) {
+        const uint32_t v = src[i];
+        uint32_t r = 0u;
+        for (uint32_t j = 0; j < n; ++j) r += src[j] < v ? 1u : 0u;
+        op.light_entries[f + r] = v;
+    }
+}
+
+__global__ void __launch_bounds__(kBlock) k_observer_commit(ObserverRecDev *recs, const uint32_t n)
+{
+    const uint32_t i = blockIdx.x * kBlock + threadIdx.x;
+    if (i < n && recs[i].emitted) recs[i].rendered = 1u;
+}
+
+void launch_observers_commit(cudaStream_t s, ObserverRecDev *recs, uint32_t n_recs)
+{
+    if (n_recs) k_observer_commit<<<grid_for(n_recs), kBlock, 0, s>>>(recs, n_recs);
+}
+
+void launch_observers(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, const uint32_t *pr_level_off,
+                      uint32_t n_levels, uint64_t *launches)
+{
+    k_observer_views<<<1, kBlock, 0, s>>>(a, sp, op);
+    ++*launches;
+    const bool pruned = pr_level_off != nullptr;
+    if (pruned) launch_pruner_table<true>(s, a, sp, pr_level_off, n_levels, launches);
+    if (a.cap) {
+        if (pruned) launch_pdl(k_shadow_count<true, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+        else launch_pdl(k_shadow_count<false, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+        launch_pdl(k_observer_lights<false>, grid_for(a.cap), kBlock, 0, s, a, sp, op);
+        *launches += 2;
+    }
+    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
+    launch_pdl(k_observer_light_scan, 1, 1024, 0, s, sp, op);
+    *launches += 2;
+}
+
+void launch_observers_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, bool pruned, uint32_t n_obs,
+                           uint64_t *launches)
+{
+    if (!a.cap || !n_obs) return;
+    if (pruned) launch_pdl(k_shadow_emit<true, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    else launch_pdl(k_shadow_emit<false, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    launch_pdl(k_observer_lights<true>, grid_for(a.cap), kBlock, 0, s, a, sp, op);
+    launch_pdl(k_observer_light_sort, n_obs, kBlock, 0, s, op);
+    *launches += 3;
 }
 
 // the pruners mark their own slots of the column

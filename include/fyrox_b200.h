@@ -371,6 +371,78 @@ typedef struct fyx_observer {
 int32_t fyx_set_lod_ranges(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const float *begin_end);
 int32_t fyx_set_observers(fyx_ctx *ctx, uint32_t count, const fyx_observer *observers);
 
+/* N4 (scene observers) — ObserversCollection::from_scene (renderer/observer.rs:88-153) and one from_graph per observer
+ * (renderer/mod.rs:1034-1047, 1364-1400), on the device, in one call.
+ *
+ * fyx_set_cameras / fyx_set_reflection_probes: the Camera / ReflectionProbe data of `count` nodes (idx NULL = nodes
+ * 0..count-1) that the global transform does not give.  A record with projection FYX_PROJECTION_NONE (camera) or present 0
+ * (probe) removes the node's record.  Records are kept by node index, carried over by fyx_set_topology; a node that a
+ * topology removes drops its record.  The perspective's one transcendental, 1 / tan(fov / 2), is evaluated here with the
+ * platform's tanf (a probe's fov is 90f32.to_radians() = FRAC_PI_2, the point lights' value).  Setting a probe's record
+ * makes it due, as does fyx_force_reflection_probe_update (ReflectionProbe::force_update, scene/probe.rs:215-218).
+ *
+ * fyx_cull_scene_observers: the observers of the scene, in the reference's order — first the six faces of every due
+ * reflection probe (probes in pool order, faces in CubeMapFaceDescriptor::cube_faces() order), then every camera in pool
+ * order — each with its matrices, its visible list, its light list and its environment map.
+ *   - A node counts when it is alive and FYX_NODE_GLOBAL_ENABLED after the last update (observer.rs:91); a camera also
+ *     needs `enabled`.  A probe is due when its mode is FYX_PROBE_UPDATE_EACH_FRAME, or when it has not been emitted since
+ *     its record was set or its update forced (probe.rs:276-290, observer.rs:99-102); every call that emits a probe and
+ *     succeeds marks it rendered (a call that fails leaves it due).  That bit lives on the device and survives fyx_set_topology.
+ *   - Camera (scene/camera.rs:454-462, observer.rs:64-74): view = look_at_rh(pos, pos + look, up) with the global
+ *     matrix's translation, column 2 and column 1 as they are (not normalised); projection = Projection::matrix(frame
+ *     size) with its guards (camera.rs:89-173), the frame size being the record's when it is not 0,0 (a render target),
+ *     else the call's; translation = the global position, z_near / z_far the record's raw values.
+ *   - Probe face (observer.rs:104-145): translation = global position + rendering_position; projection = the guarded
+ *     perspective of fov FRAC_PI_2 and aspect 1; view = look_at_rh(t, t + face.look, face.up).
+ *   - Frustum: from_view_projection_matrix(projection · view).unwrap_or_default() (renderer/bundle.rs:893-896).
+ *   - Visible list: from_graph without the shadow pass: alive, renderable, reachable, should_be_rendered with the node's
+ *     render mask against the observer's (render_mask = the camera's or probe's node mask), the LOD filter of
+ *     fyx_set_lod_ranges with the observer's translation and z range, and static-batch Break (scene/mesh/mod.rs:691-725)
+ *     — always honoured.  Order inside a list is unspecified.
+ *   - Light list: fyx_cull_lights' rule for the observer's frustum, in pool order.  Environment map: for a camera
+ *     fyx_select_reflection_probes' rule for its translation; FYX_NONE for a probe face (renderer/mod.rs:1045-1047).
+ * One pass over the nodes counts every observer's list; the call is synchronous.  FYX_ERR_STATE on a sharded context, while
+ * a frame is in flight, or before fyx_set_topology; FYX_ERR_INVALID_ARGUMENT for a NULL or non-positive frame_size.
+ * fyx_set_* return FYX_ERR_INVALID_ARGUMENT for an unknown projection kind or update mode or a node out of range. */
+#define FYX_PROJECTION_NONE 0xFFFFFFFFu
+typedef struct fyx_camera {             /* Camera fields, scene/camera.rs */
+    uint32_t enabled;                   /* Camera::is_enabled */
+    uint32_t projection;                /* FYX_PROJECTION_PERSPECTIVE / _ORTHOGRAPHIC; FYX_PROJECTION_NONE removes the record */
+    float fov_or_vertical_size;         /* PerspectiveProjection::fov (radians) or OrthographicProjection::vertical_size */
+    float z_near, z_far;                /* the projection's own values */
+    float frame_size[2];                /* the render target's size (camera.rs:813-826); 0,0 = the call's frame size */
+} fyx_camera;
+int32_t fyx_set_cameras(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const fyx_camera *cameras);
+#define FYX_PROBE_UPDATE_ONCE 0u
+#define FYX_PROBE_UPDATE_EACH_FRAME 1u
+typedef struct fyx_reflection_probe {   /* ReflectionProbe fields, scene/probe.rs */
+    uint32_t present;                   /* 0 removes the record */
+    uint32_t update_mode;               /* FYX_PROBE_UPDATE_* */
+    float z_near, z_far;
+    float rendering_position[3];        /* added to the global position: global_rendering_position, probe.rs:221-223 */
+} fyx_reflection_probe;
+int32_t fyx_set_reflection_probes(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const fyx_reflection_probe *probes);
+int32_t fyx_force_reflection_probe_update(fyx_ctx *ctx, uint32_t count, const uint32_t *idx);
+#define FYX_OBSERVER_PROBE_FACE 0u
+#define FYX_OBSERVER_CAMERA 1u
+typedef struct fyx_scene_observer {
+    uint32_t node, kind, face;          /* FYX_OBSERVER_PROBE_FACE (face 0..5) or FYX_OBSERVER_CAMERA (face 0) */
+    uint32_t render_mask;               /* Observer::render_mask: the node's render mask */
+    uint32_t first, count;              /* visible list: entries[first, first + count), order unspecified */
+    uint32_t lights_first, lights_count;/* light list: light_entries[lights_first, + lights_count), ascending node index */
+    uint32_t environment_map;           /* reflection-probe node, FYX_NONE = none */
+    float translation[3], z_near, z_far;/* ObserverPosition */
+    float view[16], projection[16], view_projection[16]; /* column-major */
+} fyx_scene_observer;
+int32_t fyx_cull_scene_observers(fyx_ctx *ctx, const float frame_size[2]);
+/* Result of the last fyx_cull_scene_observers: pinned host copies, valid until the next call ... */
+int32_t fyx_get_scene_observers(fyx_ctx *ctx, const fyx_scene_observer **out_table, uint32_t *out_n, const uint32_t **out_entries,
+                                const uint32_t **out_light_entries);
+/* ... or the device arrays (*out_n is a host value). */
+int32_t fyx_get_scene_observers_device(fyx_ctx *ctx, const fyx_scene_observer **d_table, uint32_t *out_n, const uint32_t **d_entries,
+                                       const uint32_t **d_light_entries);
+/* Instances of the observers: fyx_pack_scene_observer_instances, below with the shadow maps' pack. */
+
 /* ---- N4: blend shapes (morph targets) ahead of the skinning ------------------------------------------------ */
 /* The standard shader adds, for every blend shape i of the surface in order, offsets.position * weight to the vertex
  * position and offsets.normal * weight to the normal BEFORE skinning (fyrox-material/src/shader/standard/opengl/
@@ -622,6 +694,20 @@ int32_t fyx_get_shadow_instance_surfaces(fyx_ctx *ctx, uint32_t map, const uint3
 int32_t fyx_pack_shadow_bone_matrices(fyx_ctx *ctx);
 int32_t fyx_get_shadow_bone_matrix_blocks_device(fyx_ctx *ctx, uint32_t map, fyx_bone_blocks *out);
 int32_t fyx_get_shadow_bone_matrix_block(fyx_ctx *ctx, uint32_t map, uint32_t instance, float *out_255x16, uint32_t *out_has_block);
+
+/* The same for every observer of the last fyx_cull_scene_observers (made with fyx_enable_instances), in one call: observer o
+ * is packed exactly as fyx_pack_instances packs a frustum for (view[o], view_projection[o]).  The getters and the bone
+ * blocks (one per fyx surface) work as those of the shadow maps, with the observer in place of the map.  FYX_ERR_STATE when
+ * there is no observer cull, it was made without fyx_enable_instances, fyx_set_topology has run since it or a frame is
+ * still in flight. */
+int32_t fyx_pack_scene_observer_instances(fyx_ctx *ctx);
+int32_t fyx_get_scene_observer_instances(fyx_ctx *ctx, uint32_t observer, fyx_instances *out);
+int32_t fyx_get_scene_observer_instances_device(fyx_ctx *ctx, uint32_t observer, fyx_instances *out);
+int32_t fyx_get_scene_observer_instance_surfaces(fyx_ctx *ctx, uint32_t observer, const uint32_t **out_ordinal);
+int32_t fyx_pack_scene_observer_bone_matrices(fyx_ctx *ctx);
+int32_t fyx_get_scene_observer_bone_matrix_blocks_device(fyx_ctx *ctx, uint32_t observer, fyx_bone_blocks *out);
+int32_t fyx_get_scene_observer_bone_matrix_block(fyx_ctx *ctx, uint32_t observer, uint32_t instance, float *out_255x16,
+                                                 uint32_t *out_has_block);
 
 /* ---- multi-GPU: one context per GPU, one process per GPU ------------------------------------- */
 /* The node array is sharded (sub-trees + replicated ancestors, SURVEY §8e); each context culls its
