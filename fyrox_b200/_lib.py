@@ -213,6 +213,10 @@ class fyx_scene_observer(C.Structure):
         ("projection", C.c_float * 16), ("view_projection", C.c_float * 16)]
 
 
+class fyx_scene_shadow_map(C.Structure):
+    _fields_ = [("observer", C.c_uint32), ("map", C.c_uint32)]
+
+
 # every symbol include/fyrox_b200.h declares: name -> (restype, argtypes)
 ctx_p = C.c_void_p
 SYMBOLS = {
@@ -305,6 +309,9 @@ SYMBOLS = {
     "fyx_cull_scene_observers": (C.c_int32, [ctx_p, f32p]),
     "fyx_get_scene_observers": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
     "fyx_get_scene_observers_device": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
+    "fyx_cull_scene_shadow_casters": (C.c_int32, [ctx_p, C.POINTER(fyx_shadow_settings), C.c_uint32]),
+    "fyx_get_scene_shadow_maps": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p]),
+    "fyx_get_scene_shadow_maps_device": (C.c_int32, [ctx_p, C.POINTER(C.c_void_p), u32p]),
     "fyx_pack_scene_observer_instances": (C.c_int32, [ctx_p]),
     "fyx_get_scene_observer_instances": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),
     "fyx_get_scene_observer_instances_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),

@@ -456,6 +456,33 @@ class Context:
         self._chk(self._lib.fyx_get_scene_observers_device(self._h, C.byref(pt), C.byref(n), C.byref(pe), C.byref(pl)))
         return pt.value, n.value, pe.value, pl.value
 
+    SCENE_SHADOW_MAP_DTYPE = np.dtype([("observer", "<u4"), ("map", "<u4")])
+
+    def cull_scene_shadow_casters(self, spot_shadows_distance: float = 10.0, point_shadows_distance: float = 10.0, spot_shadows_enabled: bool = True,
+                                  point_shadows_enabled: bool = True, csm_enabled: bool = True):
+        """The shadow maps every observer of the last cull_scene_observers renders (fyx_cull_scene_shadow_casters): the map
+        table and lists of get_shadow_maps, spot and point maps shared between observers, and the refs of
+        get_scene_shadow_maps.  Defaults are QualitySettings::default() (renderer/settings.rs)."""
+        st = L.fyx_shadow_settings(float(spot_shadows_distance), float(point_shadows_distance), int(bool(spot_shadows_enabled)),
+                                   int(bool(point_shadows_enabled)))
+        self._chk(self._lib.fyx_cull_scene_shadow_casters(self._h, C.byref(st), int(bool(csm_enabled))))
+
+    def get_scene_shadow_maps(self) -> np.ndarray:
+        """SCENE_SHADOW_MAP_DTYPE refs (observer, map) in render order: `map` is a row of get_shadow_maps' table."""
+        p = C.c_void_p()
+        n = C.c_uint32()
+        self._chk(self._lib.fyx_get_scene_shadow_maps(self._h, C.byref(p), C.byref(n)))
+        if not n.value:
+            return np.empty(0, self.SCENE_SHADOW_MAP_DTYPE)
+        return np.frombuffer((C.c_char * (n.value * self.SCENE_SHADOW_MAP_DTYPE.itemsize)).from_address(p.value), self.SCENE_SHADOW_MAP_DTYPE).copy()
+
+    def get_scene_shadow_maps_device(self):
+        """(device pointer of the refs, number of refs)."""
+        p = C.c_void_p()
+        n = C.c_uint32()
+        self._chk(self._lib.fyx_get_scene_shadow_maps_device(self._h, C.byref(p), C.byref(n)))
+        return p.value, n.value
+
     def pack_scene_observer_instances(self):
         """Pack the instances of every observer of the last cull_scene_observers (made with enable_instances) in one call."""
         self._chk(self._lib.fyx_pack_scene_observer_instances(self._h))

@@ -403,6 +403,16 @@ struct fyx_ctx {
     uint32_t ob_n = 0, ob_total = 0, ob_light_total = 0;
     bool ob_valid = false, ob_on_host = false, ob_have_slots = false, ob_slots_stale = false;
     InstPack obi; // their instances, a segment per observer
+    float ob_frame[2] = {0.f, 0.f}; // the frame size of the last observer cull
+    uint64_t ob_epoch = 0;          // hier_epoch at the last observer cull
+
+    // N4 shadow maps of the scene's observers (fyx_drawprep.inl): the map table and lists are the shadow cull's (sh_*); the
+    // refs (observer, map), with the map-table kernel's scratch
+    DevBuf b_ssh_refs, b_ssh_cand, b_ssh_hash, b_ssh_csm;
+    PinnedBuf h_ssh_refs;
+    uint32_t ssh_n_refs = 0;
+    bool ssh_valid = false, ssh_on_host = false;
+    uint64_t hier_epoch = 0; // counts fyx_set_topology and hierarchy updates: a table of another frame is refused
 
     // N3 draw-prep (fyx_drawprep.inl)
     bool instances_enabled = false, rank_on_device = false;
@@ -670,6 +680,7 @@ int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cu
 {
     const bool all = (update_flags & FYX_UPDATE_ALL) || !c->updated_once;
     const size_t nl = c->level_off.size() ? c->level_off.size() - 1 : 0;
+    ++c->hier_epoch;
     if (c->n_late) {
         launch_snapshot_bones(c->stream, c->a, c->n_late, c->b_late_slot.as<uint32_t>(), c->b_stale_pos.as<float4>());
         c->launches++;
@@ -1119,6 +1130,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     c->rank_on_device = false; // re-derived from dfs_rank in the new slot order
     c->sh_slots_stale = true;  // the last shadow cull's entry slots
     c->ob_slots_stale = true;  // and the last observer cull's
+    ++c->hier_epoch;
     // camera and probe records stay with their node indices; a node that is not alive any more drops its record
     for (size_t i = 0; i < c->cam_src.size(); ++i)
         if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->cam_src[i].projection = FYX_PROJECTION_NONE;

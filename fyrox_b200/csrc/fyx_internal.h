@@ -307,14 +307,47 @@ struct ObserverParams {
     uint32_t *light_raw;        // [light_total] the light lists in emission order
     uint32_t *light_entries;    // [light_total] the same, each list in ascending node index
 };
+// The shadow maps of the scene's observers (fyx_cull_scene_shadow_casters).  ShadowParams holds the map table and lists as
+// for one camera (its `cam`, `cam_t` and `csm` camera unused but for csm.fallback); each map's frustum carries the render mask
+// of its observers.  What only the map-table kernel reads and writes:
+struct SceneShadowCand {   // one (observer, light-list entry)
+    uint32_t observer;     // its row of the observer table
+    uint32_t light;        // its row of the light table, FYX_NONE = no record
+    uint32_t n_maps, cascade;
+    uint32_t hslot;        // spot or point with maps: its key's hash slot; else FYX_NONE
+    uint32_t row;          // first map row, when it is the first of its key
+};
+struct SceneShadowParams {
+    const fyx_scene_observer *table; // [n_obs] the observer table of the last fyx_cull_scene_observers
+    uint32_t n_obs;
+    const FrustumDev *frusta;        // [n_obs] the observers' frusta
+    const uint32_t *light_entries;   // [n_cand] the observers' light lists, one after the other in table order
+    uint32_t n_cand;
+    const ObserverRecDev *recs;      // [n_recs] the records the table was built from
+    uint32_t n_recs;
+    float frame_size[2];             // the frame size of that call
+    float probe_m22;
+    uint32_t csm_enabled;
+    CsmCameraDev *csm_cams;          // [n_obs] scratch: each observer's cascade camera
+    SceneShadowCand *cand;           // [n_cand] scratch
+    uint32_t *hash;                  // [hash_mask + 1] FYX_NONE-filled: the smallest candidate of each key
+    uint32_t hash_mask;
+    fyx_scene_shadow_map *refs;      // [6 n_cand] (observer, map) in render order
+    uint32_t *n_refs;                // one u32
+};
 constexpr uint32_t kPrSelf = 1u << 31; // bit of ShadowParams::Prune::col: the node is the pruner itself
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp); // map table + frusta, count pass, scan
-void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);
+// the emit pass; scene: the form of fyx_cull_scene_shadow_casters (each map's own mask)
+void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene);
 // the same with every map's LOD filter and static-batch pruning: map table + observers, the pruner table (one launch per entry
 // of pr_level_off that holds pruners, parents first), count pass, scan; then the emit pass
 void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
                                uint64_t *launches);
-void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp);
+void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene);
+// fyx_cull_scene_shadow_casters: the map table and refs (one CTA), the pruner table when pr_level_off is given, the count pass
+// and the scan; then launch_shadow_emit[_pruned](scene = true)
+void launch_scene_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const SceneShadowParams &ss, const uint32_t *pr_level_off,
+                              uint32_t n_levels, uint64_t *launches);
 // fyx_cull_scene_observers: the observer table (one CTA), the pruner table when pr_level_off is given (as the pruned shadow
 // cull), the count pass over the observers' frusta, the scan, the light counts and environment maps, the light scan
 void launch_observers(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, const uint32_t *pr_level_off,

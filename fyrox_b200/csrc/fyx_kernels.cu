@@ -1520,9 +1520,10 @@ __device__ __forceinline__ void try_normalize(const float *v, const float *fallb
 __constant__ float c_face_look[6][3] = {{1.f, 0.f, 0.f}, {-1.f, 0.f, 0.f}, {0.f, 1.f, 0.f}, {0.f, -1.f, 0.f}, {0.f, 0.f, 1.f}, {0.f, 0.f, -1.f}};
 __constant__ float c_face_up[6][3] = {{0.f, -1.f, 0.f}, {0.f, -1.f, 0.f}, {0.f, 0.f, 1.f}, {0.f, 0.f, -1.f}, {0.f, -1.f, 0.f}, {0.f, -1.f, 0.f}};
 
-// one map: view_projection = P · V, its frustum (Frustum::default if the matrix has none, renderer/bundle.rs:893-896)
+// one map: view_projection = P · V, its frustum (Frustum::default if the matrix has none, renderer/bundle.rs:893-896) with
+// the render mask of the observer that renders it
 __device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uint32_t m, const uint32_t light, const uint32_t face, const uint32_t cascade,
-                               const float *P, const float *V)
+                               const float *P, const float *V, const uint32_t mask)
 {
     float VP[16];
     mat4_mul(P, V, VP);
@@ -1534,8 +1535,12 @@ __device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uin
     o.count = 0u;
     for (int k = 0; k < 16; ++k) o.view_projection[k] = VP[k];
     for (int k = 0; k < 16; ++k) sp.views[(size_t)m * 16 + k] = V[k]; // the observer's view_matrix of the map's instances
-    if (frustum_from_view_projection(VP, sp.scratch[m])) to_dev_frustum(sp.scratch[m], sp.cam.cam_mask, FYX_PASS_SHADOW, sp.frusta[m]);
-    else sp.frusta[m] = sp.fallback;
+    if (frustum_from_view_projection(VP, sp.scratch[m])) {
+        to_dev_frustum(sp.scratch[m], mask, FYX_PASS_SHADOW, sp.frusta[m]);
+    } else {
+        sp.frusta[m] = sp.fallback;
+        sp.frusta[m].cam_mask = mask;
+    }
 }
 
 // the observer of a map's from_graph for the LOD filter (renderer/bundle.rs:873-916): translation, z_near, z_far
@@ -1583,6 +1588,114 @@ __device__ __forceinline__ void csm_cascade(const CsmCameraDev &cam, const fyx_c
     orthographic(mn[0], mx[0], mn[1], mx[1], mn[2], mx[2], P);
 }
 
+// What one light of an observer's light list needs for its maps (shadow_light_gate)
+struct ShadowLightGate {
+    uint32_t cascade;
+    float pos[3], upv[3], lookv[3], radius;
+};
+
+// The shadow loop's gates for one light record and one observer — its frustum `cam` and translation cam_t
+// (renderer/light.rs:509-606): in the observer's light list (renderer/bundle.rs:926-974, as k_cull_lights), cast_shadows,
+// the distance gate, is_intersects_sphere, the cascade index; directional lights need csm_enabled.  Returns the light's
+// number of maps: 0, 1 (spot), 6 (point: cube faces) or 3 (directional: cascades).
+__device__ __forceinline__ uint32_t shadow_light_gate(const NodeArrays &a, const ShadowParams &sp, const ShadowLightDev &L, const FrustumDev &cam,
+                                                      const float *cam_t, const bool csm_enabled, const PackedConsts &kc, ShadowLightGate &g)
+{
+    const uint32_t slot = L.slot, kind = L.kind;
+    const uint32_t nf = a.flags[slot];
+    constexpr uint32_t need = FYX_NODE_ALIVE | FYX_NODE_LIGHT | FYX_NODE_GLOBAL_VISIBILITY | FYX_NODE_GLOBAL_ENABLED;
+    const bool dir = kind == FYX_LIGHT_DIRECTIONAL;
+    bool ok = (nf & need) == need && (kind == FYX_LIGHT_SPOT || kind == FYX_LIGHT_POINT || (dir && csm_enabled));
+    if (ok) {
+        const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
+        ok = frustum_intersects_aabb(cam, wx, wy, wz, kc, aabb_is_tame(wx, wy, wz));
+    }
+    if (!ok) return 0u;
+    const float4 r0 = a.G[0][slot], r1 = a.G[1][slot], r2 = a.G[2][slot];
+    float *pos = g.pos;
+    pos[0] = r0.w; pos[1] = r1.w; pos[2] = r2.w;          // global_position
+    g.upv[0] = r0.y; g.upv[1] = r1.y; g.upv[2] = r2.y;    // up_vector: column 1
+    g.lookv[0] = r0.z; g.lookv[1] = r1.z; g.lookv[2] = r2.z; // look_vector: column 2
+    // light.rs:510: (light.position - observer.position.translation).norm()
+    const float d[3] = {FYX_SUB(pos[0], cam_t[0]), FYX_SUB(pos[1], cam_t[1]), FYX_SUB(pos[2], cam_t[2])};
+    const float dist = sqrtf(dot3(d, d));
+    const bool spot = kind == FYX_LIGHT_SPOT;
+    const float sd = spot ? sp.spot_distance : sp.point_distance;
+    // light.rs:529-532, 547-549: cast_shadows && distance_to_camera <= shadows_distance && enabled;
+    // light.rs:555-565 (directional): cast_shadows && csm_settings.enabled (checked above), raw radius f32::MAX
+    ok = (nf & FYX_NODE_CAST_SHADOWS) && (dir || (dist <= sd && (spot ? sp.spot_enabled : sp.point_enabled)));
+    // light.rs:570-572: max(local scale) * raw radius
+    float sx = 1.f, sy = 1.f, sz = 1.f;
+    if (sp.trs) {
+        sx = sp.trs[slot].scale[0];
+        sy = sp.trs[slot].scale[1];
+        sz = sp.trs[slot].scale[2];
+    }
+    const float radius = FYX_MUL(fmaxf(fmaxf(sx, sy), sz), dir ? 3.40282347e+38f : L.distance_or_radius);
+    g.radius = radius;
+    // light.rs:585-587, Frustum::is_intersects_sphere (fyrox-math/src/frustum.rs:336-347)
+    bool sphere = true;
+    for (int p = 0; p < 6; ++p) {
+        const float4 pl = cam.plane[p];
+        const float n[3] = {pl.x, pl.y, pl.z};
+        const float dd = FYX_ADD(dot3(n, pos), pl.w);
+        if (dd < -radius) { sphere = false; break; }
+        if (fabsf(dd) < radius) break;
+    }
+    ok = ok && sphere;
+    // light.rs:589-602 (a distance equal to b1 is neither < b1 nor > b1: cascade 2)
+    const float b1 = FYX_MUL(sd, 0.2f), b2 = FYX_MUL(sd, 0.4f);
+    const float e[3] = {FYX_SUB(cam_t[0], pos[0]), FYX_SUB(cam_t[1], pos[1]), FYX_SUB(cam_t[2], pos[2])};
+    const float metric = sqrtf(dot3(e, e));
+    g.cascade = (dist < b1 || metric <= radius) ? 0u : (dist > b1 && dist < b2) ? 1u : 2u;
+    return ok ? (dir ? 3u : spot ? 1u : 6u) : 0u;
+}
+
+// The maps of one light that passed shadow_light_gate, at rows first.. of the map table, each with the render mask `mask`:
+// the cascades of `csm` for a directional light, else the spot map or the six cube faces.  obs != nullptr: each map's LOD
+// observer goes there as well (sp.pr.obs).
+__device__ __forceinline__ void shadow_light_maps(const ShadowParams &sp, const ShadowLightDev &L, const ShadowLightGate &g, const CsmCameraDev &csm,
+                                                  const uint32_t light, const uint32_t first, const uint32_t mask, float *obs)
+{
+    const float zdir[3] = {0.f, 0.f, 1.f}, ydir[3] = {0.f, 1.f, 0.f};
+    const float *pos = g.pos;
+    float P[16], V[16];
+    if (L.kind == FYX_LIGHT_DIRECTIONAL) {
+        // shadow/csm.rs:170-179: light_direction = -up (normalised, else y), light_up = look (normalised, else z)
+        float dir[3], up[3];
+        try_normalize(g.upv, ydir, dir);
+        dir[0] = -dir[0]; dir[1] = -dir[1]; dir[2] = -dir[2];
+        try_normalize(g.lookv, zdir, up);
+#pragma unroll 1
+        for (uint32_t k = 0; k < 3u; ++k) {
+            csm_cascade(csm, L.csm, k, dir, up, V, P, obs ? obs + (size_t)(first + k) * 5 : nullptr);
+            shadow_map_out(sp, first + k, light, 0u, k, P, V, mask);
+        }
+    } else {
+        perspective(L.m22, 1.0f, 0.01f, g.radius, P); // z_near 0.01, z_far light_radius (light.rs:702-704, point.rs:167-170)
+        if (obs) // light.rs:700-728, shadow/point.rs:162-190: the light's position, z_near 0.01, z_far light_radius
+            for (uint32_t k = 0; k < (L.kind == FYX_LIGHT_SPOT ? 1u : 6u); ++k) map_observer(obs + (size_t)(first + k) * 5, pos, 0.01f, g.radius);
+        if (L.kind == FYX_LIGHT_SPOT) {
+            // light.rs:706-722: look_at_rh(pos, pos - emit_direction, look_vector normalised)
+            float emit[3], up[3];
+            try_normalize(g.upv, zdir, emit);
+            try_normalize(g.lookv, ydir, up);
+            const float target[3] = {FYX_SUB(pos[0], emit[0]), FYX_SUB(pos[1], emit[1]), FYX_SUB(pos[2], emit[2])};
+            look_at_rh(pos, target, up, V);
+            shadow_map_out(sp, first, light, 0u, g.cascade, P, V, mask);
+        } else {
+            // shadow/point.rs:172-180: one map per cube face
+#pragma unroll 1
+            for (uint32_t k = 0; k < 6u; ++k) {
+                const float target[3] = {FYX_ADD(pos[0], c_face_look[k][0]), FYX_ADD(pos[1], c_face_look[k][1]), FYX_ADD(pos[2], c_face_look[k][2])};
+                const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
+                look_at_rh(pos, target, up, V);
+                shadow_map_out(sp, first + k, light, k, g.cascade, P, V, mask);
+            }
+        }
+    }
+}
+
 // PRUNE: each map's LOD observer goes to sp.pr.obs as well
 template <bool PRUNE>
 __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, const ShadowParams sp)
@@ -1597,62 +1710,12 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
     kc.negzero = make_float2(-0.0f, -0.0f);
     for (uint32_t base = 0; base < sp.n_lights; base += kBlock) {
         const uint32_t i = base + tid;
-        uint32_t n_maps = 0u, cascade = 0u, slot = 0u, kind = FYX_LIGHT_UNKNOWN;
-        float pos[3] = {0.f, 0.f, 0.f}, upv[3] = {0.f, 0.f, 0.f}, lookv[3] = {0.f, 0.f, 0.f}, radius = 0.f, m22 = 0.f;
-        fyx_csm_options csm_opt{0u, {0.f, 0.f, 0.f}};
+        uint32_t n_maps = 0u;
+        ShadowLightDev L{};
+        ShadowLightGate g;
         if (i < sp.n_lights) {
-            const ShadowLightDev L = sp.lights[i];
-            slot = L.slot;
-            kind = L.kind;
-            m22 = L.m22;
-            csm_opt = L.csm;
-            const uint32_t nf = a.flags[slot];
-            // in the camera's light list (renderer/bundle.rs:926-974, as k_cull_lights)
-            constexpr uint32_t need = FYX_NODE_ALIVE | FYX_NODE_LIGHT | FYX_NODE_GLOBAL_VISIBILITY | FYX_NODE_GLOBAL_ENABLED;
-            const bool dir = kind == FYX_LIGHT_DIRECTIONAL;
-            bool ok = (nf & need) == need && (kind == FYX_LIGHT_SPOT || kind == FYX_LIGHT_POINT || (dir && sp.csm.enabled));
-            if (ok) {
-                const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
-                ok = frustum_intersects_aabb(sp.cam, wx, wy, wz, kc, aabb_is_tame(wx, wy, wz));
-            }
-            if (ok) {
-                const float4 r0 = a.G[0][slot], r1 = a.G[1][slot], r2 = a.G[2][slot];
-                pos[0] = r0.w; pos[1] = r1.w; pos[2] = r2.w;    // global_position
-                upv[0] = r0.y; upv[1] = r1.y; upv[2] = r2.y;    // up_vector: column 1
-                lookv[0] = r0.z; lookv[1] = r1.z; lookv[2] = r2.z; // look_vector: column 2
-                // light.rs:510: (light.position - observer.position.translation).norm()
-                const float d[3] = {FYX_SUB(pos[0], sp.cam_t[0]), FYX_SUB(pos[1], sp.cam_t[1]), FYX_SUB(pos[2], sp.cam_t[2])};
-                const float dist = sqrtf(dot3(d, d));
-                const bool spot = kind == FYX_LIGHT_SPOT;
-                const float sd = spot ? sp.spot_distance : sp.point_distance;
-                // light.rs:529-532, 547-549: cast_shadows && distance_to_camera <= shadows_distance && enabled;
-                // light.rs:555-565 (directional): cast_shadows && csm_settings.enabled (checked above), raw radius f32::MAX
-                ok = (nf & FYX_NODE_CAST_SHADOWS) && (dir || (dist <= sd && (spot ? sp.spot_enabled : sp.point_enabled)));
-                // light.rs:570-572: max(local scale) * raw radius
-                float sx = 1.f, sy = 1.f, sz = 1.f;
-                if (sp.trs) {
-                    sx = sp.trs[slot].scale[0];
-                    sy = sp.trs[slot].scale[1];
-                    sz = sp.trs[slot].scale[2];
-                }
-                radius = FYX_MUL(fmaxf(fmaxf(sx, sy), sz), dir ? 3.40282347e+38f : L.distance_or_radius);
-                // light.rs:585-587, Frustum::is_intersects_sphere (fyrox-math/src/frustum.rs:336-347)
-                bool sphere = true;
-                for (int p = 0; p < 6; ++p) {
-                    const float4 pl = sp.cam.plane[p];
-                    const float n[3] = {pl.x, pl.y, pl.z};
-                    const float dd = FYX_ADD(dot3(n, pos), pl.w);
-                    if (dd < -radius) { sphere = false; break; }
-                    if (fabsf(dd) < radius) break;
-                }
-                ok = ok && sphere;
-                // light.rs:589-602 (a distance equal to b1 is neither < b1 nor > b1: cascade 2)
-                const float b1 = FYX_MUL(sd, 0.2f), b2 = FYX_MUL(sd, 0.4f);
-                const float e[3] = {FYX_SUB(sp.cam_t[0], pos[0]), FYX_SUB(sp.cam_t[1], pos[1]), FYX_SUB(sp.cam_t[2], pos[2])};
-                const float metric = sqrtf(dot3(e, e));
-                cascade = (dist < b1 || metric <= radius) ? 0u : (dist > b1 && dist < b2) ? 1u : 2u;
-                n_maps = ok ? (dir ? 3u : spot ? 1u : 6u) : 0u;
-            }
+            L = sp.lights[i];
+            n_maps = shadow_light_gate(a, sp, L, sp.cam, sp.cam_t, sp.csm.enabled, kc, g);
         }
         // ordered compaction: maps in light (pool) order
         uint32_t incl = n_maps;
@@ -1665,45 +1728,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
         __syncthreads();
         uint32_t first = s_base + incl - n_maps;
         for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
-        if (n_maps) {
-            const uint32_t light = a.gidx[slot];
-            const float zdir[3] = {0.f, 0.f, 1.f}, ydir[3] = {0.f, 1.f, 0.f};
-            float P[16], V[16];
-            if (kind == FYX_LIGHT_DIRECTIONAL) {
-                // shadow/csm.rs:170-179: light_direction = -up (normalised, else y), light_up = look (normalised, else z)
-                float dir[3], up[3];
-                try_normalize(upv, ydir, dir);
-                dir[0] = -dir[0]; dir[1] = -dir[1]; dir[2] = -dir[2];
-                try_normalize(lookv, zdir, up);
-#pragma unroll 1
-                for (uint32_t k = 0; k < 3u; ++k) {
-                    csm_cascade(sp.csm, csm_opt, k, dir, up, V, P, PRUNE ? sp.pr.obs + (size_t)(first + k) * 5 : nullptr);
-                    shadow_map_out(sp, first + k, light, 0u, k, P, V);
-                }
-            } else {
-                perspective(m22, 1.0f, 0.01f, radius, P); // z_near 0.01, z_far light_radius (light.rs:702-704, point.rs:167-170)
-                if (PRUNE) // light.rs:700-728, shadow/point.rs:162-190: the light's position, z_near 0.01, z_far light_radius
-                    for (uint32_t k = 0; k < (kind == FYX_LIGHT_SPOT ? 1u : 6u); ++k) map_observer(sp.pr.obs + (size_t)(first + k) * 5, pos, 0.01f, radius);
-                if (kind == FYX_LIGHT_SPOT) {
-                    // light.rs:706-722: look_at_rh(pos, pos - emit_direction, look_vector normalised)
-                    float emit[3], up[3];
-                    try_normalize(upv, zdir, emit);
-                    try_normalize(lookv, ydir, up);
-                    const float target[3] = {FYX_SUB(pos[0], emit[0]), FYX_SUB(pos[1], emit[1]), FYX_SUB(pos[2], emit[2])};
-                    look_at_rh(pos, target, up, V);
-                    shadow_map_out(sp, first, light, 0u, cascade, P, V);
-                } else {
-                    // shadow/point.rs:172-180: one map per cube face
-#pragma unroll 1
-                    for (uint32_t k = 0; k < 6u; ++k) {
-                        const float target[3] = {FYX_ADD(pos[0], c_face_look[k][0]), FYX_ADD(pos[1], c_face_look[k][1]), FYX_ADD(pos[2], c_face_look[k][2])};
-                        const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
-                        look_at_rh(pos, target, up, V);
-                        shadow_map_out(sp, first + k, light, k, cascade, P, V);
-                    }
-                }
-            }
-        }
+        if (n_maps) shadow_light_maps(sp, L, g, sp.csm, a.gidx[L.slot], first, sp.cam.cam_mask, PRUNE ? sp.pr.obs : nullptr);
         __syncthreads();
         if (tid == kBlock - 1) s_base = first + n_maps;
         __syncthreads();
@@ -1711,27 +1736,34 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
     if (tid == 0) *sp.n_maps = s_base;
 }
 
-// the node's part of from_graph for a shadow map, minus the frustum test: alive, renderable, reachable, globally visible and
-// enabled, cast_shadows, render mask against the camera's (every map carries the camera's mask).  OBS (the scene's observers,
-// fyx_cull_scene_observers): no shadow pass, so no cast_shadows, and each observer's own mask, tested per map by shadow_in_map.
-template <bool OBS>
+// The three forms of the node passes' one predicate:
+//   kFormShadow (fyx_cull_shadow_casters*): every map carries the camera's mask, tested once per node;
+//   kFormObservers (fyx_cull_scene_observers): the observers as maps, no shadow pass, each observer's own mask;
+//   kFormSceneShadow (fyx_cull_scene_shadow_casters): the shadow pass, each map with its observer's own mask.
+enum ShadowForm { kFormShadow, kFormObservers, kFormSceneShadow };
+
+// the node's part of from_graph for a map, minus the frustum test: alive, renderable, reachable, globally visible and
+// enabled; the shadow forms add cast_shadows, and kFormShadow the render mask against the camera's.  The other forms test
+// each map's mask in shadow_in_map.
+template <int FORM>
 __device__ __forceinline__ bool shadow_candidate(const uint32_t nf, const uint32_t mask, const ShadowParams &sp)
 {
-    if (OBS) return (nf & kNeedBits) == kNeedBits;
+    if (FORM == kFormObservers) return (nf & kNeedBits) == kNeedBits;
+    if (FORM == kFormSceneShadow) return (nf & kShadowNeed) == kShadowNeed;
     return (nf & kShadowNeed) == kShadowNeed && (mask & sp.cam.cam_mask) != 0u;
 }
 
 // The one predicate of the count and emit passes (and of a static batch's "rendered" in the pruner table): the node is in
 // map m's list.  hrow (PRUNE only): the node's row of the pruner table, the maps in which the LOD filter or a static batch
-// above it hides it (nullptr = none); hword carries its word of the current 32 maps from one map to the next.  OBS: the
-// node's render mask against map m's (should_be_rendered, scene/node/mod.rs:231-256).
-template <bool PRUNE, bool OBS>
+// above it hides it (nullptr = none); hword carries its word of the current 32 maps from one map to the next.  Forms other
+// than kFormShadow: the node's render mask against map m's (should_be_rendered, scene/node/mod.rs:231-256).
+template <bool PRUNE, int FORM>
 __device__ __forceinline__ bool shadow_in_map(const FrustumDev *__restrict__ F, const uint32_t m, const bool cand, const bool test, const bool tame,
                                               const float2 wx, const float2 wy, const float2 wz, const PackedConsts &kc,
                                               const uint32_t *hrow, uint32_t &hword, const uint32_t mask)
 {
     bool ok;
-    if (OBS) {
+    if (FORM != kFormShadow) {
         ok = cand && (mask & F[m].cam_mask) != 0u;
         if (ok && test) ok = frustum_intersects_aabb(F[m], wx, wy, wz, kc, tame);
     } else {
@@ -1756,8 +1788,9 @@ __device__ __forceinline__ const uint32_t *pruner_row(const ShadowParams &sp, co
 // Break (scene/mesh/mod.rs:691-725):
 //   self_hidden[p]     = children_hidden[anc(p)] | (LOD object outside its range for the map's observer)
 //   children_hidden[p] = self_hidden[p] | (static batch rendered in the map)
-template <bool OBS>
-__global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, const ShadowParams sp, const uint32_t p_lo, const uint32_t p_hi)
+// The bodies of the node-pass kernels take the form; each kernel is one form of them.
+template <int FORM>
+__device__ __forceinline__ void shadow_pruners(const NodeArrays &a, const ShadowParams &sp, const uint32_t p_lo, const uint32_t p_hi)
 {
     pdl_wait(); // the map table and its observers
     const uint32_t W = sp.pr.words;
@@ -1774,7 +1807,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, c
     PackedConsts kc;
     kc.one = make_float2(1.0f, 1.0f);
     kc.negzero = make_float2(-0.0f, -0.0f);
-    const bool cand = shadow_candidate<OBS>(nf, mask, sp);
+    const bool cand = shadow_candidate<FORM>(nf, mask, sp);
     const bool tame = cand && aabb_is_tame(wx, wy, wz);
     const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
     const uint32_t n_maps = *sp.n_maps;
@@ -1789,16 +1822,27 @@ __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, c
             const float normalized = __fdiv_rn(FYX_ADD(dist, -o[3]), FYX_ADD(o[4], -o[3]));
             if (!((normalized >= r.x) && (normalized <= r.y))) self |= 1u << b;
         }
-        if (batch && shadow_in_map<false, OBS>(sp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused, mask)) rendered |= 1u << b;
+        if (batch && shadow_in_map<false, FORM>(sp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused, mask)) rendered |= 1u << b;
     }
     sp.pr.rows[((size_t)p * 2u) * W + w] = self;
     sp.pr.rows[((size_t)p * 2u + 1u) * W + w] = self | rendered;
 }
 
+template <bool OBS>
+__global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, const ShadowParams sp, const uint32_t p_lo, const uint32_t p_hi)
+{
+    shadow_pruners<OBS ? kFormObservers : kFormShadow>(a, sp, p_lo, p_hi);
+}
+
+__global__ void __launch_bounds__(kBlock) k_scene_shadow_pruners(const NodeArrays a, const ShadowParams sp, const uint32_t p_lo, const uint32_t p_hi)
+{
+    shadow_pruners<kFormSceneShadow>(a, sp, p_lo, p_hi);
+}
+
 // pass 2: every node read once (flags, mask, box: 32 B; with PRUNE its pruner id: 4 B more) and tested against every map;
 // one atomic per (warp, map) with an entry
-template <bool PRUNE, bool OBS>
-__global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, const ShadowParams sp)
+template <bool PRUNE, int FORM>
+__device__ __forceinline__ void shadow_count(const NodeArrays &a, const ShadowParams &sp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
     const bool valid = slot < a.cap;
@@ -1814,7 +1858,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, con
     }
     pdl_trigger();
     pdl_wait(); // the map table
-    const bool cand = valid && shadow_candidate<OBS>(nf, mask, sp);
+    const bool cand = valid && shadow_candidate<FORM>(nf, mask, sp);
     uint32_t any = 0u;
     if (__any_sync(0xFFFFFFFFu, cand)) {
         PackedConsts kc;
@@ -1827,13 +1871,25 @@ __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, con
         const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
         uint32_t hword = 0u;
         for (uint32_t m = 0; m < n_maps; ++m) {
-            const bool ok = shadow_in_map<PRUNE, OBS>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
+            const bool ok = shadow_in_map<PRUNE, FORM>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
             const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
             if (b && lane == 0u) atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
             any |= b;
         }
     }
     if (lane == 0u) sp.warp_any[slot >> 5] = any;
+}
+
+template <bool PRUNE, bool OBS>
+__global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, const ShadowParams sp)
+{
+    shadow_count<PRUNE, OBS ? kFormObservers : kFormShadow>(a, sp);
+}
+
+template <bool PRUNE>
+__global__ void __launch_bounds__(kBlock) k_scene_shadow_count(const NodeArrays a, const ShadowParams sp)
+{
+    shadow_count<PRUNE, kFormSceneShadow>(a, sp);
 }
 
 // the lists' places: maps[m].first / count, counts[m] becomes map m's write cursor, total = all entries
@@ -1872,8 +1928,8 @@ __global__ void __launch_bounds__(1024) k_shadow_scan(const ShadowParams sp)
 
 // pass 3: the warps that had an entry test again and write their node indices (and, with instances enabled, their slots).
 // PRUNE: a warp whose entries would reach past its map's list (first + count) writes nothing and raises E_SHADOW_LIST.
-template <bool PRUNE, bool OBS>
-__global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const ShadowParams sp)
+template <bool PRUNE, int FORM>
+__device__ __forceinline__ void shadow_emit(const NodeArrays &a, const ShadowParams &sp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
     pdl_wait();
@@ -1890,7 +1946,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
         gi = a.gidx[slot];
         if (PRUNE) pc = sp.pr.col[slot];
     }
-    const bool cand = valid && shadow_candidate<OBS>(nf, mask, sp);
+    const bool cand = valid && shadow_candidate<FORM>(nf, mask, sp);
     PackedConsts kc;
     kc.one = make_float2(1.0f, 1.0f);
     kc.negzero = make_float2(-0.0f, -0.0f);
@@ -1902,7 +1958,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
     const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
     uint32_t hword = 0u;
     for (uint32_t m = 0; m < n_maps; ++m) {
-        const bool ok = shadow_in_map<PRUNE, OBS>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
+        const bool ok = shadow_in_map<PRUNE, FORM>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
         const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
         if (!b) continue;
         uint32_t at = 0u;
@@ -1919,6 +1975,18 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
     }
 }
 
+template <bool PRUNE, bool OBS>
+__global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const ShadowParams sp)
+{
+    shadow_emit<PRUNE, OBS ? kFormObservers : kFormShadow>(a, sp);
+}
+
+template <bool PRUNE>
+__global__ void __launch_bounds__(kBlock) k_scene_shadow_emit(const NodeArrays a, const ShadowParams sp)
+{
+    shadow_emit<PRUNE, kFormSceneShadow>(a, sp);
+}
+
 void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
 {
     k_shadow_frusta<false><<<1, kBlock, 0, s>>>(a, sp);
@@ -1926,20 +1994,21 @@ void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams 
     launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
 }
 
-void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
+void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene)
 {
-    if (a.cap) launch_pdl(k_shadow_emit<false, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    if (!a.cap) return;
+    if (scene) launch_pdl(k_scene_shadow_emit<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    else launch_pdl(k_shadow_emit<false, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
 }
 
-// the pruner table, one launch per hierarchy level that holds pruners (parents first)
-template <bool OBS>
-static void launch_pruner_table(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
-                                uint64_t *launches)
+// the pruner table, one launch of `kernel` (a form of k_shadow_pruners) per hierarchy level that holds pruners (parents first)
+static void launch_pruner_table(void (*kernel)(NodeArrays, ShadowParams, uint32_t, uint32_t), cudaStream_t s, const NodeArrays &a,
+                                const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels, uint64_t *launches)
 {
     for (uint32_t l = 0; l < n_levels; ++l) {
         const uint32_t lo = pr_level_off[l], hi = pr_level_off[l + 1];
         if (hi <= lo) continue;
-        launch_pdl(k_shadow_pruners<OBS>, grid_for((uint64_t)(hi - lo) * sp.pr.words), kBlock, 0, s, a, sp, lo, hi);
+        launch_pdl(kernel, grid_for((uint64_t)(hi - lo) * sp.pr.words), kBlock, 0, s, a, sp, lo, hi);
         ++*launches;
     }
 }
@@ -1949,7 +2018,7 @@ void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const Shadow
 {
     k_shadow_frusta<true><<<1, kBlock, 0, s>>>(a, sp);
     ++*launches;
-    launch_pruner_table<false>(s, a, sp, pr_level_off, n_levels, launches);
+    launch_pruner_table(k_shadow_pruners<false>, s, a, sp, pr_level_off, n_levels, launches);
     if (a.cap) {
         launch_pdl(k_shadow_count<true, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
         ++*launches;
@@ -1958,9 +2027,198 @@ void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const Shadow
     ++*launches;
 }
 
-void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
+void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene)
 {
-    if (a.cap) launch_pdl(k_shadow_emit<true, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    if (!a.cap) return;
+    if (scene) launch_pdl(k_scene_shadow_emit<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    else launch_pdl(k_shadow_emit<true, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+}
+
+// ------------------------------------------------------------------------------------------------
+// N4 shadow maps of the scene's observers (fyx_cull_scene_shadow_casters): the shadow loop of renderer/light.rs:509-782 for
+// every observer of the last fyx_cull_scene_observers (render_scene_observer, renderer/mod.rs:964-1120), through the shadow
+// maps' node passes in kFormSceneShadow.  A candidate is one (observer, entry of its light list); candidate p is entry p of
+// the observers' light lists, which lie one after the other in table order.
+// ------------------------------------------------------------------------------------------------
+// the observer whose light list holds entry p: the last one whose list starts at or before p (observers with an empty list
+// start where the next one does)
+__device__ __forceinline__ uint32_t candidate_observer(const SceneShadowParams &ss, const uint32_t p)
+{
+    uint32_t lo = 0u, hi = ss.n_obs; // table[lo].lights_first <= p < table[hi].lights_first
+    while (hi - lo > 1u) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (ss.table[mid].lights_first <= p) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// the row of the light table (pool order) that holds node's record, FYX_NONE = none
+__device__ __forceinline__ uint32_t light_record(const NodeArrays &a, const ShadowParams &sp, const uint32_t node)
+{
+    uint32_t lo = 0u, hi = sp.n_lights;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        const uint32_t n = a.gidx[sp.lights[mid].slot];
+        if (n == node) return mid;
+        if (n < node) lo = mid + 1u;
+        else hi = mid;
+    }
+    return FYX_NONE;
+}
+
+// the hash of a sharing key (light record, cascade, render mask): spot and point maps with equal keys are equal maps
+__device__ __forceinline__ uint32_t share_hash(const uint32_t light, const uint32_t cascade, const uint32_t mask)
+{
+    uint32_t h = light * 0x9E3779B1u ^ (mask * 0x85EBCA77u + cascade * 0xC2B2AE3Du);
+    h ^= h >> 15;
+    h *= 0x2C1B3C6Du;
+    return h ^ (h >> 13);
+}
+
+// The camera of observer m's cascades (shadow/csm.rs:179-270 with the observer's projection, view and frame size).  A
+// camera's record is found by (kind, node): the records are the probes in pool order, then the cameras in pool order.
+__device__ __forceinline__ void observer_csm_camera(const NodeArrays &a, const ShadowParams &sp, const SceneShadowParams &ss, const uint32_t m,
+                                                    CsmCameraDev &cam)
+{
+    const fyx_scene_observer &o = ss.table[m];
+    cam.enabled = ss.csm_enabled;
+    cam.z_near = o.z_near;
+    cam.z_far = o.z_far;
+    for (int k = 0; k < 16; ++k) cam.view[k] = o.view[k];
+    cam.fallback = sp.csm.fallback;
+    if (o.kind == FYX_OBSERVER_CAMERA) {
+        const uint64_t want = (1ull << 32) | o.node;
+        uint32_t lo = 0u, hi = ss.n_recs;
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi) >> 1;
+            const ObserverRecDev &r = ss.recs[mid];
+            const uint64_t k = ((uint64_t)(r.kind == FYX_OBSERVER_CAMERA) << 32) | a.gidx[r.slot];
+            if (k < want) lo = mid + 1u;
+            else hi = mid;
+        }
+        const ObserverRecDev &R = ss.recs[lo];
+        const bool own = R.v[0] != 0.0f || R.v[1] != 0.0f; // a render target's size
+        cam.projection = R.mode;
+        cam.m22_or_vertical_size = R.m22_or_vertical_size;
+        cam.frame_size[0] = own ? R.v[0] : ss.frame_size[0];
+        cam.frame_size[1] = own ? R.v[1] : ss.frame_size[1];
+    } else {
+        // a cube face is square: Projection::matrix uses only w / h (camera.rs:89-106)
+        cam.projection = FYX_PROJECTION_PERSPECTIVE;
+        cam.m22_or_vertical_size = ss.probe_m22;
+        cam.frame_size[0] = cam.frame_size[1] = 1.0f;
+    }
+}
+
+// One CTA builds the map table and the refs.
+//   1. every observer's cascade camera (ss.csm_cams) and every candidate's gate (shadow_light_gate with the observer's
+//      frustum and translation);
+//   2. a spot or point candidate that gets maps enters its key into the hash (open addressing, linear probing; a slot keeps
+//      the smallest candidate of its key);
+//   3. in candidate order, the same ordered block scan as k_shadow_frusta over (new maps, refs): a candidate that is the first
+//      of its key, or a directional light, builds its maps; every candidate writes its refs, to its own maps or its key's.
+// The work grows with the candidates (observers x lights in their lists; the benchmark scene has 26 x 17 = 442), twice
+// 256 at a time: it assumes at most some tens of thousands of candidates, as a one-CTA pass.
+__global__ void __launch_bounds__(kBlock) k_scene_shadow_maps(const NodeArrays a, const ShadowParams sp, const SceneShadowParams ss)
+{
+    __shared__ uint32_t s_warp[kBlock / 32];
+    __shared__ uint32_t s_maps, s_refs;
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    pdl_trigger(); // the node pass loads its columns meanwhile
+    if (tid == 0) s_maps = s_refs = 0u;
+    PackedConsts kc;
+    kc.one = make_float2(1.0f, 1.0f);
+    kc.negzero = make_float2(-0.0f, -0.0f);
+    for (uint32_t m = tid; m < ss.n_obs; m += kBlock) observer_csm_camera(a, sp, ss, m, ss.csm_cams[m]);
+    for (uint32_t p = tid; p < ss.n_cand; p += kBlock) {
+        SceneShadowCand &C = ss.cand[p];
+        const uint32_t m = candidate_observer(ss, p), node = ss.light_entries[p], row = light_record(a, sp, node);
+        const fyx_scene_observer &o = ss.table[m];
+        C.observer = m;
+        C.light = row;
+        C.n_maps = C.cascade = 0u;
+        C.hslot = FYX_NONE;
+        if (row == FYX_NONE) continue; // no record: Unknown (light.rs:560-568)
+        ShadowLightGate g;
+        C.n_maps = shadow_light_gate(a, sp, sp.lights[row], ss.frusta[m], o.translation, ss.csm_enabled != 0u, kc, g);
+        C.cascade = g.cascade;
+    }
+    __syncthreads();
+    for (uint32_t p = tid; p < ss.n_cand; p += kBlock) {
+        SceneShadowCand &C = ss.cand[p];
+        if (!C.n_maps || sp.lights[C.light].kind == FYX_LIGHT_DIRECTIONAL) continue; // cascades are never shared
+        const uint32_t mask = ss.table[C.observer].render_mask;
+        for (uint32_t h = share_hash(C.light, C.cascade, mask) & ss.hash_mask;; h = (h + 1u) & ss.hash_mask) {
+            const uint32_t q = atomicCAS(ss.hash + h, FYX_NONE, p);
+            const SceneShadowCand &Q = ss.cand[q == FYX_NONE ? p : q];
+            if (Q.light == C.light && Q.cascade == C.cascade && ss.table[Q.observer].render_mask == mask) {
+                if (q != FYX_NONE) atomicMin(ss.hash + h, p);
+                C.hslot = h;
+                break;
+            }
+        }
+    }
+    __syncthreads();
+    for (uint32_t base = 0; base < ss.n_cand; base += kBlock) {
+        const uint32_t p = base + tid;
+        uint32_t n_refs = 0u, n_new = 0u, src = p;
+        if (p < ss.n_cand) {
+            const SceneShadowCand &C = ss.cand[p];
+            n_refs = C.n_maps;
+            if (C.hslot != FYX_NONE) src = ss.hash[C.hslot];
+            n_new = src == p ? n_refs : 0u;
+        }
+        // one scan of (new maps << 16 | refs): at most 6 x 256 of either per round
+        const uint32_t v = n_new << 16 | n_refs;
+        uint32_t incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= (uint32_t)o) incl += t;
+        }
+        if (lane == 31u) s_warp[warp] = incl;
+        __syncthreads();
+        uint32_t excl = incl - v;
+        for (uint32_t w = 0; w < warp; ++w) excl += s_warp[w];
+        const uint32_t first_map = s_maps + (excl >> 16), first_ref = s_refs + (excl & 0xFFFFu);
+        if (n_new) {
+            const SceneShadowCand &C = ss.cand[p];
+            const ShadowLightDev &L = sp.lights[C.light];
+            ShadowLightGate g;
+            shadow_light_gate(a, sp, L, ss.frusta[C.observer], ss.table[C.observer].translation, ss.csm_enabled != 0u, kc, g);
+            shadow_light_maps(sp, L, g, ss.csm_cams[C.observer], ss.light_entries[p], first_map, ss.table[C.observer].render_mask, sp.pr.obs);
+            ss.cand[p].row = first_map;
+        }
+        __syncthreads(); // the rows of this round's first candidates
+        for (uint32_t k = 0; k < n_refs; ++k) ss.refs[first_ref + k] = fyx_scene_shadow_map{ss.cand[p].observer, ss.cand[src].row + k};
+        __syncthreads();
+        if (tid == kBlock - 1) {
+            s_maps = first_map + n_new;
+            s_refs = first_ref + n_refs;
+        }
+        __syncthreads();
+    }
+    if (tid == 0) {
+        *sp.n_maps = s_maps;
+        *ss.n_refs = s_refs;
+    }
+}
+
+void launch_scene_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const SceneShadowParams &ss, const uint32_t *pr_level_off,
+                              uint32_t n_levels, uint64_t *launches)
+{
+    k_scene_shadow_maps<<<1, kBlock, 0, s>>>(a, sp, ss);
+    ++*launches;
+    const bool pruned = pr_level_off != nullptr;
+    if (pruned) launch_pruner_table(k_scene_shadow_pruners, s, a, sp, pr_level_off, n_levels, launches);
+    if (a.cap) {
+        if (pruned) launch_pdl(k_scene_shadow_count<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
+        else launch_pdl(k_scene_shadow_count<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+        ++*launches;
+    }
+    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
+    ++*launches;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2181,7 +2439,7 @@ void launch_observers(cudaStream_t s, const NodeArrays &a, const ShadowParams &s
     k_observer_views<<<1, kBlock, 0, s>>>(a, sp, op);
     ++*launches;
     const bool pruned = pr_level_off != nullptr;
-    if (pruned) launch_pruner_table<true>(s, a, sp, pr_level_off, n_levels, launches);
+    if (pruned) launch_pruner_table(k_shadow_pruners<true>, s, a, sp, pr_level_off, n_levels, launches);
     if (a.cap) {
         if (pruned) launch_pdl(k_shadow_count<true, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
         else launch_pdl(k_shadow_count<false, true>, grid_for(a.cap), kBlock, 0, s, a, sp);

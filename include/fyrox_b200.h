@@ -441,7 +441,43 @@ int32_t fyx_get_scene_observers(fyx_ctx *ctx, const fyx_scene_observer **out_tab
 /* ... or the device arrays (*out_n is a host value). */
 int32_t fyx_get_scene_observers_device(fyx_ctx *ctx, const fyx_scene_observer **d_table, uint32_t *out_n, const uint32_t **d_entries,
                                        const uint32_t **d_light_entries);
-/* Instances of the observers: fyx_pack_scene_observer_instances, below with the shadow maps' pack. */
+/* Instances of the observers: fyx_pack_scene_observer_instances, below with the shadow maps' pack.
+ *
+ * fyx_cull_scene_shadow_casters: the shadow maps every observer of the last successful fyx_cull_scene_observers renders
+ * (render_scene_observer runs the deferred light renderer for each observer, probe faces included: renderer/mod.rs:964-1120,
+ * renderer/light.rs:509-782), and their lists, in one call.
+ *   - For every observer in table order and every light of its light list (pool order), the gates of
+ *     fyx_cull_shadow_casters_csm with the observer as the camera: a light with no fyx_set_light_sources record is skipped
+ *     (Unknown); cast_shadows; the distance gate against the observer's translation; is_intersects_sphere against its
+ *     frustum; the cascade index from that distance; directional lights need csm_enabled.
+ *   - A directional light's three cascades take the observer's projection kind, 1 / tan(fov / 2) or vertical size (for a
+ *     probe face the FRAC_PI_2 value), raw z_near / z_far, view matrix, and frame size: for a camera its render target's
+ *     size when it is not 0,0, else the frame size of that fyx_cull_scene_observers call; for a probe face aspect 1 (a cube
+ *     face is square; Projection::matrix uses only w / h, camera.rs:89-106).
+ *   - Every map carries its observer's render_mask: a node is in a map's list when it passes the shadow pass (cast_shadows),
+ *     that mask and the map's frustum.  Each map's LOD filter (its own observer: the light's position, 0.01 and the radius
+ *     for spot and point maps; the look_at_lh eye and the slice's depths for cascades) and static-batch Break (with the
+ *     map's mask) are always honoured, as in fyx_cull_shadow_casters_pruned.
+ *   - Spot and point maps with equal (light, face, cascade, render mask) are one row of the map table, culled and listed
+ *     once: their frustum, LOD observer and list do not depend on the observer (light.rs:700-728, shadow/point.rs:162-190).
+ *     Cascades are never shared.  Rows are numbered in order of first reference, and every field of a row holds for every
+ *     observer that references it.
+ *   - The refs list every (observer, map) pair in the reference's render order: observers in table order, then lights in
+ *     list order, then faces 0..5 or cascades 0..2.
+ * The result replaces the last shadow cull's: fyx_get_shadow_maps[_device], fyx_pack_shadow_instances, the shadow instance
+ * getters and fyx_pack_shadow_bone_matrices work on its map table unchanged; a later fyx_cull_shadow_casters* makes
+ * fyx_get_scene_shadow_maps return FYX_ERR_STATE.  The call is synchronous.  FYX_ERR_INVALID_ARGUMENT for a NULL ctx or
+ * settings; FYX_ERR_STATE before a successful fyx_cull_scene_observers, after fyx_set_topology or any hierarchy update
+ * since that call (its table describes another frame), on a sharded context, or while a frame is in flight. */
+typedef struct fyx_scene_shadow_map {   /* one shadow map an observer renders */
+    uint32_t observer;                  /* row of the last fyx_cull_scene_observers table */
+    uint32_t map;                       /* row of fyx_get_shadow_maps' table: light, face, cascade, list, view_projection */
+} fyx_scene_shadow_map;
+int32_t fyx_cull_scene_shadow_casters(fyx_ctx *ctx, const fyx_shadow_settings *settings, uint32_t csm_enabled);
+/* The refs of the last fyx_cull_scene_shadow_casters: a pinned host copy, valid until the next call ... */
+int32_t fyx_get_scene_shadow_maps(fyx_ctx *ctx, const fyx_scene_shadow_map **out_refs, uint32_t *out_n);
+/* ... or the device array (*out_n is a host value). */
+int32_t fyx_get_scene_shadow_maps_device(fyx_ctx *ctx, const fyx_scene_shadow_map **d_refs, uint32_t *out_n);
 
 /* ---- N4: blend shapes (morph targets) ahead of the skinning ------------------------------------------------ */
 /* The standard shader adds, for every blend shape i of the surface in order, offsets.position * weight to the vertex
