@@ -233,6 +233,27 @@ struct InstPack {
     uint32_t segments() const { return (uint32_t)inst_first.size() - 1; }
 };
 
+// N4: what a many-map cull leaves (fyx_drawprep.inl; MapParams in fyx_internal.h): the map table, the lists, their pinned
+// copies and the maps' instance pack, a segment per map.  A call takes prepare, its own table kernel, the count pass and
+// the scan (with what else it counts and scans), lists, the emit pass, commit.
+struct MapCull {
+    DevBuf b_scratch, b_frusta, b_maps, b_views, b_counts, b_warp_any;
+    DevBuf b_small; // n, total, then words of the caller's (a third count it reads back with them)
+    DevBuf b_entries, b_slots; // the lists as node indices and (with instances enabled) as HBM slots
+    PinnedBuf h_small, h_maps, h_entries;
+    uint32_t n = 0, total = 0; // maps, entries of all maps: set by lists, before the call has succeeded, so like every
+                               // result here they may be read only behind `valid`
+    bool valid = false, on_host = false, have_slots = false, slots_stale = false;
+    InstPack pack;
+    void invalidate() { valid = pack.valid = false; }
+    void topology_changed() { slots_stale = true; } // the entries' slots are the old order's
+    // buffers for up to max_maps maps, the node passes' parameters (the pruner table's too when pruned), counts cleared
+    int32_t prepare(fyx_ctx *c, size_t max_maps, bool pruned, MapParams &mp);
+    // waits for the scan, reads n, total (and the caller's words: n_small in all) and sizes the lists
+    int32_t lists(fyx_ctx *c, MapParams &mp, uint32_t n_small);
+    void commit(const fyx_ctx *c); // the call succeeded: the results are the context's
+};
+
 // Scratch of the instance packs, shared by all of them: per bin (histogram, first key, offset), per entry (sort index), per
 // segment (instances, first instance, first bundle), the device-wide scan's tile sums, and the totals with a pinned copy
 struct PackScratch {
@@ -369,16 +390,8 @@ struct fyx_ctx {
     std::vector<fyx_csm_options> csm_opts; // by node index; missing = FrustumSplitOptions::default()
     bool light_table_dirty = false;
     uint32_t n_light_table = 0;
-    DevBuf b_light_table, b_sh_scratch, b_sh_frusta, b_sh_maps, b_sh_counts, b_sh_warp_any, b_sh_small, b_sh_entries;
-    PinnedBuf h_sh_small; // n_maps, total
-    PinnedBuf h_sh_maps, h_sh_entries;
-    uint32_t sh_n_maps = 0, sh_total = 0;
-    bool sh_valid = false, sh_on_host = false;
-    // the shadow maps' instances (fyx_pack_shadow_instances): the shadow cull also records slots (with instances enabled)
-    // and view matrices; one pack for all maps, a segment per map; bone blocks per surface
-    DevBuf b_sh_slots, b_sh_views;
-    bool sh_have_slots = false, sh_slots_stale = false;
-    InstPack shi;
+    DevBuf b_light_table;
+    MapCull shadow_cull; // the last shadow cull: of one camera, or of the scene's observers
     // per-map LOD filter and static-batch pruning (fyx_cull_shadow_casters_pruned).  pr_node: by node index, kPrLod | kPrBatch
     // for a node with a LOD range / FYX_NODE_STATIC_BATCH (kept beside the device columns, so that a change is seen without
     // reading them back).  The pruner column is rebuilt by the first pruned cull after such a change (pr_dirty).
@@ -397,17 +410,15 @@ struct fyx_ctx {
     std::vector<uint32_t> ob_rec_node;          // node of each record of the device table
     bool obs_table_dirty = false;
     uint32_t n_ob_recs = 0;
-    DevBuf b_ob_recs, b_ob_table, b_ob_scratch, b_ob_frusta, b_ob_maps, b_ob_views, b_ob_counts, b_ob_warp_any, b_ob_small, b_ob_entries,
-        b_ob_slots, b_ob_lcounts, b_ob_best, b_ob_lraw, b_ob_lights;
-    PinnedBuf h_ob_small, h_ob_table, h_ob_entries, h_ob_lights; // n_obs, total, light total; host copies of the results
-    uint32_t ob_n = 0, ob_total = 0, ob_light_total = 0;
-    bool ob_valid = false, ob_on_host = false, ob_have_slots = false, ob_slots_stale = false;
-    InstPack obi; // their instances, a segment per observer
+    MapCull observer_cull; // a map per observer; its third small word is the light total
+    DevBuf b_ob_recs, b_ob_table, b_ob_lcounts, b_ob_best, b_ob_lraw, b_ob_lights;
+    PinnedBuf h_ob_table, h_ob_lights; // host copies of the table and the light lists
+    uint32_t ob_light_total = 0;
     float ob_frame[2] = {0.f, 0.f}; // the frame size of the last observer cull
     uint64_t ob_epoch = 0;          // hier_epoch at the last observer cull
 
-    // N4 shadow maps of the scene's observers (fyx_drawprep.inl): the map table and lists are the shadow cull's (sh_*); the
-    // refs (observer, map), with the map-table kernel's scratch
+    // N4 shadow maps of the scene's observers (fyx_drawprep.inl): the map table and lists are the shadow cull's (`shadow_cull`);
+    // the refs (observer, map), with the map-table kernel's scratch
     DevBuf b_ssh_refs, b_ssh_cand, b_ssh_hash, b_ssh_csm;
     PinnedBuf h_ssh_refs;
     uint32_t ssh_n_refs = 0;
@@ -1128,8 +1139,8 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     c->updated_once = false;
     if (!same_capacity) c->dfs_rank.clear(); // indexed by node: stays valid while the pool capacity does
     c->rank_on_device = false; // re-derived from dfs_rank in the new slot order
-    c->sh_slots_stale = true;  // the last shadow cull's entry slots
-    c->ob_slots_stale = true;  // and the last observer cull's
+    c->shadow_cull.topology_changed();
+    c->observer_cull.topology_changed();
     ++c->hier_epoch;
     // camera and probe records stay with their node indices; a node that is not alive any more drops its record
     for (size_t i = 0; i < c->cam_src.size(); ++i)

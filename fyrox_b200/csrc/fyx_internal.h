@@ -257,29 +257,25 @@ struct CsmCameraDev {
     float view[16];
     fyx_frustum fallback; // Frustum::default() as planes + corners: a cascade slice's unwrap_or_default (shadow/csm.rs:215-219)
 };
-struct ShadowParams {
-    const ShadowLightDev *lights;
-    uint32_t n_lights;
-    FrustumDev cam;      // the camera frustum of the last cull (planes + cam_mask)
-    FrustumDev fallback; // Frustum::default(): from_view_projection_matrix(..).unwrap_or_default() (renderer/bundle.rs:893-896)
-    float cam_t[3];
-    float spot_distance, point_distance;
-    uint32_t spot_enabled, point_enabled;
-    const fyx_trs *trs; // the node's last TRS record per slot; nullptr = none sent (identity scale)
-    // outputs of pass 1 (map table), read by the node pass
+// A many-map cull (the shadow maps of one camera, the scene's observers, the observers' shadow maps): a one-CTA table kernel
+// writes up to `max maps` map rows with their frusta; the count pass reads every node once and counts its entries per map;
+// the scan places the lists; the emit pass re-tests the warps that had an entry and writes them.  MapParams is what the node
+// passes, the scan and the pruner table read, and what the table kernels write.
+struct MapParams {
+    // the map table
     fyx_frustum *scratch; // [max maps] the map frusta as planes + corners
-    FrustumDev *frusta;   // [max maps]
+    FrustumDev *frusta;   // [max maps] each with the render mask of what renders the map
     fyx_shadow_map *maps; // [max maps]
-    float *views;         // [max maps * 16] the maps' view matrices (look_at_rh), for fyx_pack_shadow_instances
+    float *views;         // [max maps * 16] the maps' view matrices, for the instance pack
     uint32_t *n_maps;     // one u32
-    // node pass: per-map counts (each on its own 128 B line), then the lists
+    // node passes: per-map counts (each on its own 128 B line), then the lists
     uint32_t *counts;     // [max maps * kCountStride]
     uint32_t *warp_any;   // [warps]: the warp's nodes are in at least one map (written by the count pass, read by the emit pass)
     uint32_t *total;      // one u32: entries of all maps
     uint32_t *entries;    // [total], sized by the host from the count pass
     uint32_t *entry_slot; // [total] the same entries as HBM slots; nullptr unless fyx_enable_instances
-    CsmCameraDev csm;     // last, so that the node passes' parameter offsets do not move
-    // ---- per-map LOD filter and static-batch pruning (fyx_cull_shadow_casters_pruned; unused by the unpruned kernels).
+    uint32_t cam_mask;    // kFormShadow: the one camera's render mask, tested once per node (the other forms: frusta[m].cam_mask)
+    // ---- per-map LOD filter and static-batch pruning (unused by the unpruned kernels).
     // A pruner is a LOD object or an FYX_NODE_STATIC_BATCH node; pruners have dense ids in slot order.
     struct Prune {
         const uint32_t *col;    // per slot: the nearest pruner on the node's path (id | kPrSelf when the node is that pruner), FYX_NONE = none
@@ -292,14 +288,27 @@ struct ShadowParams {
         uint32_t *err;          // the context's error word (E_SHADOW_LIST)
     } pr;
 };
-// The scene's observers (fyx_cull_scene_observers).  The node passes take the observers as their maps: ShadowParams' `maps` /
-// `frusta` / `views` / `counts` / `entries` hold one per observer, each frustum with its observer's cam_mask, and the node
-// test takes each observer's mask and no cast_shadows (shadow_in_map<.., OBS>).  What only the observer kernels read:
+// What only the table kernels of the shadow culls read (k_shadow_frusta, k_scene_shadow_maps): the light table and the
+// shadow loop's settings; for one camera also that camera and its cascades
+struct ShadowParams {
+    const ShadowLightDev *lights;
+    uint32_t n_lights;
+    FrustumDev cam;      // fyx_cull_shadow_casters*: the camera frustum of the last cull (planes + cam_mask)
+    FrustumDev fallback; // Frustum::default(): from_view_projection_matrix(..).unwrap_or_default() (renderer/bundle.rs:893-896)
+    float cam_t[3];      // fyx_cull_shadow_casters*: the camera's translation
+    float spot_distance, point_distance;
+    uint32_t spot_enabled, point_enabled;
+    const fyx_trs *trs; // the node's last TRS record per slot; nullptr = none sent (identity scale)
+    CsmCameraDev csm;   // fyx_cull_shadow_casters*: the cascades' camera; the scene form takes its `fallback` for every observer's
+};
+// The scene's observers (fyx_cull_scene_observers): a many-map cull with one map per observer, in kFormObservers (each
+// observer's own mask, no cast_shadows).  What only the observer kernels read:
 struct ObserverParams {
     ObserverRecDev *recs;       // [n_recs] due probes' and cameras' records: probes in pool order, then cameras
     uint32_t n_recs;
     float frame_size[2];        // the call's frame size
     float probe_m22;            // 1 / tan(FRAC_PI_2 / 2), evaluated on the host
+    fyx_frustum fallback;       // Frustum::default(): from_view_projection_matrix(..).unwrap_or_default()
     fyx_scene_observer *table;  // [max observers]
     uint32_t *light_counts;     // [max observers * kCountStride]: light-list counts, then write cursors
     uint32_t *best;             // [max observers]: environment map node + 1 (0 = none)
@@ -307,9 +316,8 @@ struct ObserverParams {
     uint32_t *light_raw;        // [light_total] the light lists in emission order
     uint32_t *light_entries;    // [light_total] the same, each list in ascending node index
 };
-// The shadow maps of the scene's observers (fyx_cull_scene_shadow_casters).  ShadowParams holds the map table and lists as
-// for one camera (its `cam`, `cam_t` and `csm` camera unused but for csm.fallback); each map's frustum carries the render mask
-// of its observers.  What only the map-table kernel reads and writes:
+// The shadow maps of the scene's observers (fyx_cull_scene_shadow_casters): a many-map cull in kFormSceneShadow (each map's
+// frustum carries the render mask of its observers).  Beside ShadowParams, what only its table kernel reads and writes:
 struct SceneShadowCand {   // one (observer, light-list entry)
     uint32_t observer;     // its row of the observer table
     uint32_t light;        // its row of the light table, FYX_NONE = no record
@@ -335,29 +343,31 @@ struct SceneShadowParams {
     fyx_scene_shadow_map *refs;      // [6 n_cand] (observer, map) in render order
     uint32_t *n_refs;                // one u32
 };
-constexpr uint32_t kPrSelf = 1u << 31; // bit of ShadowParams::Prune::col: the node is the pruner itself
-void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp); // map table + frusta, count pass, scan
-// the emit pass; scene: the form of fyx_cull_scene_shadow_casters (each map's own mask)
-void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene);
-// the same with every map's LOD filter and static-batch pruning: map table + observers, the pruner table (one launch per entry
-// of pr_level_off that holds pruners, parents first), count pass, scan; then the emit pass
-void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
-                               uint64_t *launches);
-void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene);
-// fyx_cull_scene_shadow_casters: the map table and refs (one CTA), the pruner table when pr_level_off is given, the count pass
-// and the scan; then launch_shadow_emit[_pruned](scene = true)
-void launch_scene_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const SceneShadowParams &ss, const uint32_t *pr_level_off,
-                              uint32_t n_levels, uint64_t *launches);
-// fyx_cull_scene_observers: the observer table (one CTA), the pruner table when pr_level_off is given (as the pruned shadow
-// cull), the count pass over the observers' frusta, the scan, the light counts and environment maps, the light scan
-void launch_observers(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, const uint32_t *pr_level_off,
-                      uint32_t n_levels, uint64_t *launches);
-// then the lists: the emit pass, the light emit pass and the light lists' sort (one CTA per observer)
-void launch_observers_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, bool pruned, uint32_t n_obs,
-                           uint64_t *launches);
+constexpr uint32_t kPrSelf = 1u << 31; // bit of MapParams::Prune::col: the node is the pruner itself
+// The three forms of the node passes' one predicate:
+//   kFormShadow (fyx_cull_shadow_casters*): every map carries the camera's mask, tested once per node;
+//   kFormObservers (fyx_cull_scene_observers): the observers as maps, no shadow pass, each observer's own mask;
+//   kFormSceneShadow (fyx_cull_scene_shadow_casters): the shadow pass, each map with its observer's own mask.
+enum ShadowForm { kFormShadow, kFormObservers, kFormSceneShadow };
+static_assert(kFormSceneShadow == 2, "tools/scene_shadow_bench.py finds that call's node passes by this value in their names (<.., 2>)");
+// Every launcher returns the number of kernels it launched.
+// The table kernels, one CTA each (pruned: the maps' LOD observers go to mp.pr.obs as well; the other two look at mp.pr.obs)
+uint32_t launch_shadow_frusta(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ShadowParams &sp, bool pruned);
+uint32_t launch_scene_shadow_maps(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ShadowParams &sp, const SceneShadowParams &ss);
+uint32_t launch_observer_views(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ObserverParams &op);
+// after the table kernel: the pruner table when pr_level_off is given (one launch per entry of pr_level_off that holds
+// pruners, parents first), then the count pass; then the scan; then, once the host has sized the lists, the emit pass
+uint32_t launch_map_count(cudaStream_t s, const NodeArrays &a, const MapParams &mp, ShadowForm form, const uint32_t *pr_level_off, uint32_t n_levels);
+uint32_t launch_map_scan(cudaStream_t s, const MapParams &mp);
+uint32_t launch_map_emit(cudaStream_t s, const NodeArrays &a, const MapParams &mp, ShadowForm form, bool pruned);
+// fyx_cull_scene_observers' own passes: the light counts and environment maps (emit = false) or the light lists (emit = true);
+// the light scan; the light lists' sort (one CTA per observer)
+uint32_t launch_observer_lights(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ObserverParams &op, bool emit);
+uint32_t launch_observer_light_scan(cudaStream_t s, const MapParams &mp, const ObserverParams &op);
+uint32_t launch_observer_light_sort(cudaStream_t s, const ObserverParams &op, uint32_t n_obs);
 // after a call that succeeded: the probes it emitted count as rendered (probe.rs `updated`)
-void launch_observers_commit(cudaStream_t s, ObserverRecDev *recs, uint32_t n_recs);
-// the pruner column ShadowParams::Prune::col / anc from the pruners' slots: col must hold FYX_NONE everywhere; then one launch per
+uint32_t launch_observers_commit(cudaStream_t s, ObserverRecDev *recs, uint32_t n_recs);
+// the pruner column MapParams::Prune::col / anc from the pruners' slots: col must hold FYX_NONE everywhere; then one launch per
 // hierarchy level [level_off[l], level_off[l + 1]) from level `first` on, parents first
 void launch_pruner_mark(cudaStream_t s, uint32_t n_pruners, const uint32_t *pr_slot, uint32_t *col);
 void launch_pruner_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, uint32_t *col, uint32_t *anc);

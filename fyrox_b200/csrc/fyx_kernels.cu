@@ -89,9 +89,7 @@ template <int NFT>
 __device__ __forceinline__ uint32_t cull_warp(const bool cand, const uint32_t nf, const uint32_t mask, const float2 wx, const float2 wy,
                                               const float2 wz, const CullParams &cp)
 {
-    PackedConsts kc;
-    kc.one = make_float2(cp.one, cp.one);
-    kc.negzero = make_float2(cp.negzero, cp.negzero);
+    const PackedConsts kc = packed_consts(cp.one, cp.negzero);
     const bool ok = cand && (nf & kNeedBits) == kNeedBits;
     const bool tame = ok && aabb_is_tame(wx, wy, wz);
     return ok ? cull_bits<NFT>(nf, mask, wx, wy, wz, cp, kc, tame, 0xFFFFFFFFu) : 0u;
@@ -436,9 +434,7 @@ __global__ void __launch_bounds__(kBlock) k_cull_lights(const NodeArrays a, cons
     constexpr uint32_t need = FYX_NODE_ALIVE | FYX_NODE_LIGHT | FYX_NODE_GLOBAL_VISIBILITY | FYX_NODE_GLOBAL_ENABLED;
     if ((nf & need) != need) return;
     const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
-    PackedConsts kc;
-    kc.one = make_float2(cp.one, cp.one);
-    kc.negzero = make_float2(cp.negzero, cp.negzero);
+    const PackedConsts kc = packed_consts(cp.one, cp.negzero);
     const bool tame = aabb_is_tame(wx, wy, wz);
     const uint32_t gi = a.gidx[slot];
     for (int f = 0; f < cp.nf; ++f)
@@ -560,9 +556,7 @@ __global__ void __launch_bounds__(kBlock) k_fold_bones(const NodeArrays a, const
     uint32_t vis_bits = 0u, gi = 0u, slot = 0u;
     const uint32_t m = blockIdx.x * kWarps + lane; // lane l of warp 0 culls the mesh of warp l
     if (lane < kWarps && m < fa.n) {
-        PackedConsts kc;
-        kc.one = make_float2(cp.one, cp.one);
-        kc.negzero = make_float2(cp.negzero, cp.negzero);
+        const PackedConsts kc = packed_consts(cp.one, cp.negzero);
         slot = fa.node_slot[m];
         const float2 bx = s_box[0][lane], by = s_box[1][lane], bz = s_box[2][lane];
         vis_bits = cull_bits<(NFT > 0 ? NFT : 0)>(s_nf[lane], a.mask[slot], bx, by, bz, cp, kc, aabb_is_tame(bx, by, bz), 0xFFFFFFFFu);
@@ -853,9 +847,7 @@ __global__ void __launch_bounds__(kBlock, MINB) k_skin(const SkinArrays sk, cons
     constexpr int PAL = 3 * S * (1 << LOG2C);
     extern __shared__ float4 smem[];
     float4 *const s_pal = smem;
-    PackedConsts kc;
-    kc.one = make_float2(one, one);
-    kc.negzero = make_float2(negzero, negzero);
+    const PackedConsts kc = packed_consts(one, negzero);
     const SkinTile T = tiles[blockIdx.x];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     float4 *const stage = smem + PAL + warp * kSkinStageF4;
@@ -1502,8 +1494,44 @@ void launch_compact_gathered(cudaStream_t s, const uint32_t *pad, uint32_t maxc,
 // shadow/point.rs:162-180, shadow/csm.rs:251-265).  Pass 1 (one CTA) builds the map table: 1 map per spot light, 6 per
 // point light, 3 cascades per directional light; pass 2 reads every node once and counts its entries in
 // every map; a one-CTA scan places the lists; pass 3 re-tests the warps that had an entry and writes the lists.
+// The passes after the table are those of every many-map cull (MapParams): the observers and their shadow maps bring
+// their own table kernel and a form of the node passes' predicate.
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t kShadowNeed = kNeedBits | FYX_NODE_CAST_SHADOWS;
+
+// The ordered scan of a one-CTA kernel of BLOCK threads, in shared memory.  excl: every thread gives v and gets the sum of
+// the v of the threads before it (plus *from, read after the barrier), so what the threads place at their offsets keeps
+// thread order.  place: the same over rounds, offsets counted from `base`, which it carries from round to round: thread 0
+// clears it before the first round, with no barrier of its own, because `base` is only ever read after excl's barrier;
+// after the last round it is the sum of all.  A kernel that carries bases of its own (k_scene_shadow_maps) uses excl
+// alone and leaves `base` unused.
+template <uint32_t BLOCK> struct BlockScan {
+    uint32_t warp[BLOCK / 32u];
+    uint32_t base;
+    __device__ __forceinline__ uint32_t excl(const uint32_t v, const uint32_t *from = nullptr)
+    {
+        const uint32_t lane = threadIdx.x & 31u, w_self = threadIdx.x >> 5;
+        uint32_t incl = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= (uint32_t)o) incl += t;
+        }
+        if (lane == 31u) warp[w_self] = incl;
+        __syncthreads();
+        uint32_t e = from ? *from + incl - v : incl - v;
+        for (uint32_t w = 0; w < w_self; ++w) e += warp[w];
+        return e;
+    }
+    __device__ __forceinline__ uint32_t place(const uint32_t v)
+    {
+        const uint32_t first = excl(v, &base);
+        __syncthreads();
+        if (threadIdx.x == BLOCK - 1u) base = first + v;
+        __syncthreads();
+        return first;
+    }
+};
 
 // Vector3::try_normalize(f32::EPSILON).unwrap_or(fallback): norm <= eps ⇒ the fallback, else each component / norm
 __device__ __forceinline__ void try_normalize(const float *v, const float *fallback, float *out)
@@ -1522,24 +1550,24 @@ __constant__ float c_face_up[6][3] = {{0.f, -1.f, 0.f}, {0.f, -1.f, 0.f}, {0.f, 
 
 // one map: view_projection = P · V, its frustum (Frustum::default if the matrix has none, renderer/bundle.rs:893-896) with
 // the render mask of the observer that renders it
-__device__ __forceinline__ void shadow_map_out(const ShadowParams &sp, const uint32_t m, const uint32_t light, const uint32_t face, const uint32_t cascade,
-                               const float *P, const float *V, const uint32_t mask)
+__device__ __forceinline__ void shadow_map_out(const MapParams &mp, const FrustumDev &fallback, const uint32_t m, const uint32_t light, const uint32_t face,
+                                               const uint32_t cascade, const float *P, const float *V, const uint32_t mask)
 {
     float VP[16];
     mat4_mul(P, V, VP);
-    fyx_shadow_map &o = sp.maps[m];
+    fyx_shadow_map &o = mp.maps[m];
     o.light = light;
     o.face = face;
     o.cascade = cascade;
     o.first = 0u;
     o.count = 0u;
     for (int k = 0; k < 16; ++k) o.view_projection[k] = VP[k];
-    for (int k = 0; k < 16; ++k) sp.views[(size_t)m * 16 + k] = V[k]; // the observer's view_matrix of the map's instances
-    if (frustum_from_view_projection(VP, sp.scratch[m])) {
-        to_dev_frustum(sp.scratch[m], mask, FYX_PASS_SHADOW, sp.frusta[m]);
+    for (int k = 0; k < 16; ++k) mp.views[(size_t)m * 16 + k] = V[k]; // the observer's view_matrix of the map's instances
+    if (frustum_from_view_projection(VP, mp.scratch[m])) {
+        to_dev_frustum(mp.scratch[m], mask, FYX_PASS_SHADOW, mp.frusta[m]);
     } else {
-        sp.frusta[m] = sp.fallback;
-        sp.frusta[m].cam_mask = mask;
+        mp.frusta[m] = fallback;
+        mp.frusta[m].cam_mask = mask;
     }
 }
 
@@ -1653,9 +1681,9 @@ __device__ __forceinline__ uint32_t shadow_light_gate(const NodeArrays &a, const
 
 // The maps of one light that passed shadow_light_gate, at rows first.. of the map table, each with the render mask `mask`:
 // the cascades of `csm` for a directional light, else the spot map or the six cube faces.  obs != nullptr: each map's LOD
-// observer goes there as well (sp.pr.obs).
-__device__ __forceinline__ void shadow_light_maps(const ShadowParams &sp, const ShadowLightDev &L, const ShadowLightGate &g, const CsmCameraDev &csm,
-                                                  const uint32_t light, const uint32_t first, const uint32_t mask, float *obs)
+// observer goes there as well (mp.pr.obs).
+__device__ __forceinline__ void shadow_light_maps(const MapParams &mp, const FrustumDev &fallback, const ShadowLightDev &L, const ShadowLightGate &g,
+                                                  const CsmCameraDev &csm, const uint32_t light, const uint32_t first, const uint32_t mask, float *obs)
 {
     const float zdir[3] = {0.f, 0.f, 1.f}, ydir[3] = {0.f, 1.f, 0.f};
     const float *pos = g.pos;
@@ -1669,7 +1697,7 @@ __device__ __forceinline__ void shadow_light_maps(const ShadowParams &sp, const 
 #pragma unroll 1
         for (uint32_t k = 0; k < 3u; ++k) {
             csm_cascade(csm, L.csm, k, dir, up, V, P, obs ? obs + (size_t)(first + k) * 5 : nullptr);
-            shadow_map_out(sp, first + k, light, 0u, k, P, V, mask);
+            shadow_map_out(mp, fallback, first + k, light, 0u, k, P, V, mask);
         }
     } else {
         perspective(L.m22, 1.0f, 0.01f, g.radius, P); // z_near 0.01, z_far light_radius (light.rs:702-704, point.rs:167-170)
@@ -1682,7 +1710,7 @@ __device__ __forceinline__ void shadow_light_maps(const ShadowParams &sp, const 
             try_normalize(g.lookv, ydir, up);
             const float target[3] = {FYX_SUB(pos[0], emit[0]), FYX_SUB(pos[1], emit[1]), FYX_SUB(pos[2], emit[2])};
             look_at_rh(pos, target, up, V);
-            shadow_map_out(sp, first, light, 0u, g.cascade, P, V, mask);
+            shadow_map_out(mp, fallback, first, light, 0u, g.cascade, P, V, mask);
         } else {
             // shadow/point.rs:172-180: one map per cube face
 #pragma unroll 1
@@ -1690,24 +1718,21 @@ __device__ __forceinline__ void shadow_light_maps(const ShadowParams &sp, const 
                 const float target[3] = {FYX_ADD(pos[0], c_face_look[k][0]), FYX_ADD(pos[1], c_face_look[k][1]), FYX_ADD(pos[2], c_face_look[k][2])};
                 const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
                 look_at_rh(pos, target, up, V);
-                shadow_map_out(sp, first + k, light, k, g.cascade, P, V, mask);
+                shadow_map_out(mp, fallback, first + k, light, k, g.cascade, P, V, mask);
             }
         }
     }
 }
 
-// PRUNE: each map's LOD observer goes to sp.pr.obs as well
+// PRUNE: each map's LOD observer goes to mp.pr.obs as well
 template <bool PRUNE>
-__global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, const ShadowParams sp)
+__global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, const MapParams mp, const ShadowParams sp)
 {
-    __shared__ uint32_t s_warp[kBlock / 32];
-    __shared__ uint32_t s_base;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    __shared__ BlockScan<kBlock> s_scan;
+    const uint32_t tid = threadIdx.x;
     pdl_trigger(); // the node pass loads its columns meanwhile
-    if (tid == 0) s_base = 0u;
-    PackedConsts kc;
-    kc.one = make_float2(1.0f, 1.0f);
-    kc.negzero = make_float2(-0.0f, -0.0f);
+    if (tid == 0) s_scan.base = 0u;
+    const PackedConsts kc = packed_consts();
     for (uint32_t base = 0; base < sp.n_lights; base += kBlock) {
         const uint32_t i = base + tid;
         uint32_t n_maps = 0u;
@@ -1718,39 +1743,21 @@ __global__ void __launch_bounds__(kBlock) k_shadow_frusta(const NodeArrays a, co
             n_maps = shadow_light_gate(a, sp, L, sp.cam, sp.cam_t, sp.csm.enabled, kc, g);
         }
         // ordered compaction: maps in light (pool) order
-        uint32_t incl = n_maps;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if (lane >= (uint32_t)o) incl += v;
-        }
-        if (lane == 31u) s_warp[warp] = incl;
-        __syncthreads();
-        uint32_t first = s_base + incl - n_maps;
-        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
-        if (n_maps) shadow_light_maps(sp, L, g, sp.csm, a.gidx[L.slot], first, sp.cam.cam_mask, PRUNE ? sp.pr.obs : nullptr);
-        __syncthreads();
-        if (tid == kBlock - 1) s_base = first + n_maps;
-        __syncthreads();
+        const uint32_t first = s_scan.place(n_maps);
+        if (n_maps) shadow_light_maps(mp, sp.fallback, L, g, sp.csm, a.gidx[L.slot], first, sp.cam.cam_mask, PRUNE ? mp.pr.obs : nullptr);
     }
-    if (tid == 0) *sp.n_maps = s_base;
+    if (tid == 0) *mp.n_maps = s_scan.base;
 }
-
-// The three forms of the node passes' one predicate:
-//   kFormShadow (fyx_cull_shadow_casters*): every map carries the camera's mask, tested once per node;
-//   kFormObservers (fyx_cull_scene_observers): the observers as maps, no shadow pass, each observer's own mask;
-//   kFormSceneShadow (fyx_cull_scene_shadow_casters): the shadow pass, each map with its observer's own mask.
-enum ShadowForm { kFormShadow, kFormObservers, kFormSceneShadow };
 
 // the node's part of from_graph for a map, minus the frustum test: alive, renderable, reachable, globally visible and
 // enabled; the shadow forms add cast_shadows, and kFormShadow the render mask against the camera's.  The other forms test
 // each map's mask in shadow_in_map.
 template <int FORM>
-__device__ __forceinline__ bool shadow_candidate(const uint32_t nf, const uint32_t mask, const ShadowParams &sp)
+__device__ __forceinline__ bool shadow_candidate(const uint32_t nf, const uint32_t mask, const MapParams &mp)
 {
     if (FORM == kFormObservers) return (nf & kNeedBits) == kNeedBits;
     if (FORM == kFormSceneShadow) return (nf & kShadowNeed) == kShadowNeed;
-    return (nf & kShadowNeed) == kShadowNeed && (mask & sp.cam.cam_mask) != 0u;
+    return (nf & kShadowNeed) == kShadowNeed && (mask & mp.cam_mask) != 0u;
 }
 
 // The one predicate of the count and emit passes (and of a static batch's "rendered" in the pruner table): the node is in
@@ -1777,10 +1784,10 @@ __device__ __forceinline__ bool shadow_in_map(const FrustumDev *__restrict__ F, 
 }
 
 // the node's row of the pruner table: its own (it is a pruner) or its nearest pruner ancestor's children row
-__device__ __forceinline__ const uint32_t *pruner_row(const ShadowParams &sp, const uint32_t pc)
+__device__ __forceinline__ const uint32_t *pruner_row(const MapParams &mp, const uint32_t pc)
 {
     if (pc == FYX_NONE) return nullptr;
-    return sp.pr.rows + ((size_t)(pc & ~kPrSelf) * 2u + ((pc & kPrSelf) ? 0u : 1u)) * sp.pr.words;
+    return mp.pr.rows + ((size_t)(pc & ~kPrSelf) * 2u + ((pc & kPrSelf) ? 0u : 1u)) * mp.pr.words;
 }
 
 // The pruner table of a shadow cull, one launch per hierarchy level's pruners [p_lo, p_hi) (parents first), one thread per
@@ -1788,61 +1795,47 @@ __device__ __forceinline__ const uint32_t *pruner_row(const ShadowParams &sp, co
 // Break (scene/mesh/mod.rs:691-725):
 //   self_hidden[p]     = children_hidden[anc(p)] | (LOD object outside its range for the map's observer)
 //   children_hidden[p] = self_hidden[p] | (static batch rendered in the map)
-// The bodies of the node-pass kernels take the form; each kernel is one form of them.
 template <int FORM>
-__device__ __forceinline__ void shadow_pruners(const NodeArrays &a, const ShadowParams &sp, const uint32_t p_lo, const uint32_t p_hi)
+__global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, const MapParams mp, const uint32_t p_lo, const uint32_t p_hi)
 {
     pdl_wait(); // the map table and its observers
-    const uint32_t W = sp.pr.words;
+    const uint32_t W = mp.pr.words;
     const uint64_t t = (uint64_t)blockIdx.x * kBlock + threadIdx.x;
     if (t >= (uint64_t)(p_hi - p_lo) * W) return;
     const uint32_t p = p_lo + (uint32_t)(t / W), w = (uint32_t)(t % W);
-    const uint32_t slot = sp.pr.slot[p], anc = sp.pr.anc[p];
-    uint32_t self = anc != FYX_NONE ? sp.pr.rows[((size_t)anc * 2u + 1u) * W + w] : 0u, rendered = 0u;
+    const uint32_t slot = mp.pr.slot[p], anc = mp.pr.anc[p];
+    uint32_t self = anc != FYX_NONE ? mp.pr.rows[((size_t)anc * 2u + 1u) * W + w] : 0u, rendered = 0u;
     const uint32_t nf = a.flags[slot], mask = a.mask[slot];
-    const float2 r = sp.pr.range ? sp.pr.range[slot] : make_float2(NAN, NAN);
+    const float2 r = mp.pr.range ? mp.pr.range[slot] : make_float2(NAN, NAN);
     const bool lod = r.x == r.x, batch = (nf & FYX_NODE_STATIC_BATCH) != 0u;
     const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
     const float gx = a.G[0][slot].w, gy = a.G[1][slot].w, gz = a.G[2][slot].w; // global_position()
-    PackedConsts kc;
-    kc.one = make_float2(1.0f, 1.0f);
-    kc.negzero = make_float2(-0.0f, -0.0f);
-    const bool cand = shadow_candidate<FORM>(nf, mask, sp);
+    const PackedConsts kc = packed_consts();
+    const bool cand = shadow_candidate<FORM>(nf, mask, mp);
     const bool tame = cand && aabb_is_tame(wx, wy, wz);
     const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
-    const uint32_t n_maps = *sp.n_maps;
+    const uint32_t n_maps = *mp.n_maps;
     uint32_t unused = 0u;
     for (uint32_t b = 0; b < 32u; ++b) {
         const uint32_t m = w * 32u + b;
         if (m >= n_maps) break;
         if (lod) { // k_lod_level's arithmetic with the map's observer
-            const float *o = sp.pr.obs + (size_t)m * 5;
+            const float *o = mp.pr.obs + (size_t)m * 5;
             const float dx = FYX_ADD(o[0], -gx), dy = FYX_ADD(o[1], -gy), dz = FYX_ADD(o[2], -gz);
             const float dist = __fsqrt_rn(FYX_ADD(FYX_ADD(FYX_MUL(dx, dx), FYX_MUL(dy, dy)), FYX_MUL(dz, dz)));
             const float normalized = __fdiv_rn(FYX_ADD(dist, -o[3]), FYX_ADD(o[4], -o[3]));
             if (!((normalized >= r.x) && (normalized <= r.y))) self |= 1u << b;
         }
-        if (batch && shadow_in_map<false, FORM>(sp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused, mask)) rendered |= 1u << b;
+        if (batch && shadow_in_map<false, FORM>(mp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused, mask)) rendered |= 1u << b;
     }
-    sp.pr.rows[((size_t)p * 2u) * W + w] = self;
-    sp.pr.rows[((size_t)p * 2u + 1u) * W + w] = self | rendered;
-}
-
-template <bool OBS>
-__global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, const ShadowParams sp, const uint32_t p_lo, const uint32_t p_hi)
-{
-    shadow_pruners<OBS ? kFormObservers : kFormShadow>(a, sp, p_lo, p_hi);
-}
-
-__global__ void __launch_bounds__(kBlock) k_scene_shadow_pruners(const NodeArrays a, const ShadowParams sp, const uint32_t p_lo, const uint32_t p_hi)
-{
-    shadow_pruners<kFormSceneShadow>(a, sp, p_lo, p_hi);
+    mp.pr.rows[((size_t)p * 2u) * W + w] = self;
+    mp.pr.rows[((size_t)p * 2u + 1u) * W + w] = self | rendered;
 }
 
 // pass 2: every node read once (flags, mask, box: 32 B; with PRUNE its pruner id: 4 B more) and tested against every map;
 // one atomic per (warp, map) with an entry
 template <bool PRUNE, int FORM>
-__device__ __forceinline__ void shadow_count(const NodeArrays &a, const ShadowParams &sp)
+__global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, const MapParams mp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
     const bool valid = slot < a.cap;
@@ -1854,86 +1847,59 @@ __device__ __forceinline__ void shadow_count(const NodeArrays &a, const ShadowPa
         wx = ld_stream(a.wa[0] + slot);
         wy = ld_stream(a.wa[1] + slot);
         wz = ld_stream(a.wa[2] + slot);
-        if (PRUNE) pc = sp.pr.col[slot];
+        if (PRUNE) pc = mp.pr.col[slot];
     }
     pdl_trigger();
     pdl_wait(); // the map table
-    const bool cand = valid && shadow_candidate<FORM>(nf, mask, sp);
+    const bool cand = valid && shadow_candidate<FORM>(nf, mask, mp);
     uint32_t any = 0u;
     if (__any_sync(0xFFFFFFFFu, cand)) {
-        PackedConsts kc;
-        kc.one = make_float2(1.0f, 1.0f);
-        kc.negzero = make_float2(-0.0f, -0.0f);
+        const PackedConsts kc = packed_consts();
         const bool tame = cand && aabb_is_tame(wx, wy, wz);
         const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
-        const FrustumDev *__restrict__ F = sp.frusta;
-        const uint32_t n_maps = *sp.n_maps;
-        const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
+        const FrustumDev *__restrict__ F = mp.frusta;
+        const uint32_t n_maps = *mp.n_maps;
+        const uint32_t *hrow = PRUNE && cand ? pruner_row(mp, pc) : nullptr;
         uint32_t hword = 0u;
         for (uint32_t m = 0; m < n_maps; ++m) {
             const bool ok = shadow_in_map<PRUNE, FORM>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
             const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
-            if (b && lane == 0u) atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
+            if (b && lane == 0u) atomicAdd(mp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
             any |= b;
         }
     }
-    if (lane == 0u) sp.warp_any[slot >> 5] = any;
-}
-
-template <bool PRUNE, bool OBS>
-__global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, const ShadowParams sp)
-{
-    shadow_count<PRUNE, OBS ? kFormObservers : kFormShadow>(a, sp);
-}
-
-template <bool PRUNE>
-__global__ void __launch_bounds__(kBlock) k_scene_shadow_count(const NodeArrays a, const ShadowParams sp)
-{
-    shadow_count<PRUNE, kFormSceneShadow>(a, sp);
+    if (lane == 0u) mp.warp_any[slot >> 5] = any;
 }
 
 // the lists' places: maps[m].first / count, counts[m] becomes map m's write cursor, total = all entries
-__global__ void __launch_bounds__(1024) k_shadow_scan(const ShadowParams sp)
+__global__ void __launch_bounds__(1024) k_shadow_scan(const MapParams mp)
 {
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_base;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    __shared__ BlockScan<1024u> s_scan;
+    const uint32_t tid = threadIdx.x;
     pdl_wait();
-    if (tid == 0) s_base = 0u;
-    const uint32_t n = *sp.n_maps;
+    if (tid == 0) s_scan.base = 0u;
+    const uint32_t n = *mp.n_maps;
     for (uint32_t base = 0; base < n; base += 1024u) {
         const uint32_t m = base + tid;
-        const uint32_t c = m < n ? sp.counts[(size_t)m * kCountStride] : 0u;
-        uint32_t incl = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if (lane >= (uint32_t)o) incl += v;
-        }
-        if (lane == 31u) s_warp[warp] = incl;
-        __syncthreads();
-        uint32_t first = s_base + incl - c;
-        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
+        const uint32_t c = m < n ? mp.counts[(size_t)m * kCountStride] : 0u;
+        const uint32_t first = s_scan.place(c);
         if (m < n) {
-            sp.maps[m].first = first;
-            sp.maps[m].count = c;
-            sp.counts[(size_t)m * kCountStride] = first;
+            mp.maps[m].first = first;
+            mp.maps[m].count = c;
+            mp.counts[(size_t)m * kCountStride] = first;
         }
-        __syncthreads();
-        if (tid == 1023u) s_base = first + c;
-        __syncthreads();
     }
-    if (tid == 0) *sp.total = s_base;
+    if (tid == 0) *mp.total = s_scan.base;
 }
 
 // pass 3: the warps that had an entry test again and write their node indices (and, with instances enabled, their slots).
 // PRUNE: a warp whose entries would reach past its map's list (first + count) writes nothing and raises E_SHADOW_LIST.
 template <bool PRUNE, int FORM>
-__device__ __forceinline__ void shadow_emit(const NodeArrays &a, const ShadowParams &sp)
+__global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const MapParams mp)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x, lane = threadIdx.x & 31u;
     pdl_wait();
-    if (!sp.warp_any[slot >> 5]) return; // warp-uniform
+    if (!mp.warp_any[slot >> 5]) return; // warp-uniform
     const bool valid = slot < a.cap;
     uint32_t nf = 0u, mask = 0u, gi = 0u, pc = FYX_NONE;
     float2 wx = make_float2(0.f, 0.f), wy = wx, wz = wx;
@@ -1944,94 +1910,81 @@ __device__ __forceinline__ void shadow_emit(const NodeArrays &a, const ShadowPar
         wy = ld_stream(a.wa[1] + slot);
         wz = ld_stream(a.wa[2] + slot);
         gi = a.gidx[slot];
-        if (PRUNE) pc = sp.pr.col[slot];
+        if (PRUNE) pc = mp.pr.col[slot];
     }
-    const bool cand = valid && shadow_candidate<FORM>(nf, mask, sp);
-    PackedConsts kc;
-    kc.one = make_float2(1.0f, 1.0f);
-    kc.negzero = make_float2(-0.0f, -0.0f);
+    const bool cand = valid && shadow_candidate<FORM>(nf, mask, mp);
+    const PackedConsts kc = packed_consts();
     const bool tame = cand && aabb_is_tame(wx, wy, wz);
     const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
-    const FrustumDev *__restrict__ F = sp.frusta;
-    const uint32_t n_maps = *sp.n_maps;
+    const FrustumDev *__restrict__ F = mp.frusta;
+    const uint32_t n_maps = *mp.n_maps;
     const uint32_t lt = (1u << lane) - 1u;
-    const uint32_t *hrow = PRUNE && cand ? pruner_row(sp, pc) : nullptr;
+    const uint32_t *hrow = PRUNE && cand ? pruner_row(mp, pc) : nullptr;
     uint32_t hword = 0u;
     for (uint32_t m = 0; m < n_maps; ++m) {
         const bool ok = shadow_in_map<PRUNE, FORM>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
         const uint32_t b = __ballot_sync(0xFFFFFFFFu, ok);
         if (!b) continue;
         uint32_t at = 0u;
-        if (lane == 0u) at = atomicAdd(sp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
+        if (lane == 0u) at = atomicAdd(mp.counts + (size_t)m * kCountStride, (uint32_t)__popc(b));
         at = __shfl_sync(0xFFFFFFFFu, at, 0);
-        if (PRUNE && at + (uint32_t)__popc(b) > sp.maps[m].first + sp.maps[m].count) { // warp-uniform
-            if (lane == 0u) atomicOr(sp.pr.err, E_SHADOW_LIST);
+        if (PRUNE && at + (uint32_t)__popc(b) > mp.maps[m].first + mp.maps[m].count) { // warp-uniform
+            if (lane == 0u) atomicOr(mp.pr.err, E_SHADOW_LIST);
             continue;
         }
         if (ok) {
-            sp.entries[at + __popc(b & lt)] = gi;
-            if (sp.entry_slot) sp.entry_slot[at + __popc(b & lt)] = slot;
+            mp.entries[at + __popc(b & lt)] = gi;
+            if (mp.entry_slot) mp.entry_slot[at + __popc(b & lt)] = slot;
         }
     }
 }
 
-template <bool PRUNE, bool OBS>
-__global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, const ShadowParams sp)
+uint32_t launch_shadow_frusta(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ShadowParams &sp, bool pruned)
 {
-    shadow_emit<PRUNE, OBS ? kFormObservers : kFormShadow>(a, sp);
+    if (pruned) k_shadow_frusta<true><<<1, kBlock, 0, s>>>(a, mp, sp);
+    else k_shadow_frusta<false><<<1, kBlock, 0, s>>>(a, mp, sp);
+    return 1u;
 }
 
-template <bool PRUNE>
-__global__ void __launch_bounds__(kBlock) k_scene_shadow_emit(const NodeArrays a, const ShadowParams sp)
-{
-    shadow_emit<PRUNE, kFormSceneShadow>(a, sp);
-}
+// The instances of the node passes, by [pruned][form]: the one place that picks one
+using NodePass = void (*)(NodeArrays, MapParams);
+static const NodePass kCountPass[2][3] = {
+    {k_shadow_count<false, kFormShadow>, k_shadow_count<false, kFormObservers>, k_shadow_count<false, kFormSceneShadow>},
+    {k_shadow_count<true, kFormShadow>, k_shadow_count<true, kFormObservers>, k_shadow_count<true, kFormSceneShadow>}};
+static const NodePass kEmitPass[2][3] = {
+    {k_shadow_emit<false, kFormShadow>, k_shadow_emit<false, kFormObservers>, k_shadow_emit<false, kFormSceneShadow>},
+    {k_shadow_emit<true, kFormShadow>, k_shadow_emit<true, kFormObservers>, k_shadow_emit<true, kFormSceneShadow>}};
+static void (*const kPrunerTable[3])(NodeArrays, MapParams, uint32_t, uint32_t) = {k_shadow_pruners<kFormShadow>, k_shadow_pruners<kFormObservers>,
+                                                                                  k_shadow_pruners<kFormSceneShadow>};
 
-void launch_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp)
+uint32_t launch_map_count(cudaStream_t s, const NodeArrays &a, const MapParams &mp, ShadowForm form, const uint32_t *pr_level_off, uint32_t n_levels)
 {
-    k_shadow_frusta<false><<<1, kBlock, 0, s>>>(a, sp);
-    if (a.cap) launch_pdl(k_shadow_count<false, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
-    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
-}
-
-void launch_shadow_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene)
-{
-    if (!a.cap) return;
-    if (scene) launch_pdl(k_scene_shadow_emit<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
-    else launch_pdl(k_shadow_emit<false, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
-}
-
-// the pruner table, one launch of `kernel` (a form of k_shadow_pruners) per hierarchy level that holds pruners (parents first)
-static void launch_pruner_table(void (*kernel)(NodeArrays, ShadowParams, uint32_t, uint32_t), cudaStream_t s, const NodeArrays &a,
-                                const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels, uint64_t *launches)
-{
-    for (uint32_t l = 0; l < n_levels; ++l) {
+    const bool pruned = pr_level_off != nullptr;
+    uint32_t n = 0u;
+    for (uint32_t l = 0; pruned && l < n_levels; ++l) {
         const uint32_t lo = pr_level_off[l], hi = pr_level_off[l + 1];
         if (hi <= lo) continue;
-        launch_pdl(kernel, grid_for((uint64_t)(hi - lo) * sp.pr.words), kBlock, 0, s, a, sp, lo, hi);
-        ++*launches;
+        launch_pdl(kPrunerTable[form], grid_for((uint64_t)(hi - lo) * mp.pr.words), kBlock, 0, s, a, mp, lo, hi);
+        ++n;
     }
-}
-
-void launch_shadow_maps_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const uint32_t *pr_level_off, uint32_t n_levels,
-                               uint64_t *launches)
-{
-    k_shadow_frusta<true><<<1, kBlock, 0, s>>>(a, sp);
-    ++*launches;
-    launch_pruner_table(k_shadow_pruners<false>, s, a, sp, pr_level_off, n_levels, launches);
     if (a.cap) {
-        launch_pdl(k_shadow_count<true, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
-        ++*launches;
+        launch_pdl(kCountPass[pruned][form], grid_for(a.cap), kBlock, 0, s, a, mp);
+        ++n;
     }
-    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
-    ++*launches;
+    return n;
 }
 
-void launch_shadow_emit_pruned(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, bool scene)
+uint32_t launch_map_scan(cudaStream_t s, const MapParams &mp)
 {
-    if (!a.cap) return;
-    if (scene) launch_pdl(k_scene_shadow_emit<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
-    else launch_pdl(k_shadow_emit<true, false>, grid_for(a.cap), kBlock, 0, s, a, sp);
+    launch_pdl(k_shadow_scan, 1, 1024, 0, s, mp);
+    return 1u;
+}
+
+uint32_t launch_map_emit(cudaStream_t s, const NodeArrays &a, const MapParams &mp, ShadowForm form, bool pruned)
+{
+    if (!a.cap) return 0u;
+    launch_pdl(kEmitPass[pruned][form], grid_for(a.cap), kBlock, 0, s, a, mp);
+    return 1u;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2116,20 +2069,18 @@ __device__ __forceinline__ void observer_csm_camera(const NodeArrays &a, const S
 //      frustum and translation);
 //   2. a spot or point candidate that gets maps enters its key into the hash (open addressing, linear probing; a slot keeps
 //      the smallest candidate of its key);
-//   3. in candidate order, the same ordered block scan as k_shadow_frusta over (new maps, refs): a candidate that is the first
+//   3. in candidate order, one ordered block scan over (new maps, refs): a candidate that is the first
 //      of its key, or a directional light, builds its maps; every candidate writes its refs, to its own maps or its key's.
 // The work grows with the candidates (observers x lights in their lists; the benchmark scene has 26 x 17 = 442), twice
 // 256 at a time: it assumes at most some tens of thousands of candidates, as a one-CTA pass.
-__global__ void __launch_bounds__(kBlock) k_scene_shadow_maps(const NodeArrays a, const ShadowParams sp, const SceneShadowParams ss)
+__global__ void __launch_bounds__(kBlock) k_scene_shadow_maps(const NodeArrays a, const MapParams mp, const ShadowParams sp, const SceneShadowParams ss)
 {
-    __shared__ uint32_t s_warp[kBlock / 32];
-    __shared__ uint32_t s_maps, s_refs;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    __shared__ BlockScan<kBlock> s_scan;
+    __shared__ uint32_t s_maps, s_refs; // a round scans (new maps << 16 | refs); the two bases are carried apart, in full words
+    const uint32_t tid = threadIdx.x;
     pdl_trigger(); // the node pass loads its columns meanwhile
     if (tid == 0) s_maps = s_refs = 0u;
-    PackedConsts kc;
-    kc.one = make_float2(1.0f, 1.0f);
-    kc.negzero = make_float2(-0.0f, -0.0f);
+    const PackedConsts kc = packed_consts();
     for (uint32_t m = tid; m < ss.n_obs; m += kBlock) observer_csm_camera(a, sp, ss, m, ss.csm_cams[m]);
     for (uint32_t p = tid; p < ss.n_cand; p += kBlock) {
         SceneShadowCand &C = ss.cand[p];
@@ -2170,24 +2121,14 @@ __global__ void __launch_bounds__(kBlock) k_scene_shadow_maps(const NodeArrays a
             n_new = src == p ? n_refs : 0u;
         }
         // one scan of (new maps << 16 | refs): at most 6 x 256 of either per round
-        const uint32_t v = n_new << 16 | n_refs;
-        uint32_t incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if (lane >= (uint32_t)o) incl += t;
-        }
-        if (lane == 31u) s_warp[warp] = incl;
-        __syncthreads();
-        uint32_t excl = incl - v;
-        for (uint32_t w = 0; w < warp; ++w) excl += s_warp[w];
+        const uint32_t excl = s_scan.excl(n_new << 16 | n_refs);
         const uint32_t first_map = s_maps + (excl >> 16), first_ref = s_refs + (excl & 0xFFFFu);
         if (n_new) {
             const SceneShadowCand &C = ss.cand[p];
             const ShadowLightDev &L = sp.lights[C.light];
             ShadowLightGate g;
             shadow_light_gate(a, sp, L, ss.frusta[C.observer], ss.table[C.observer].translation, ss.csm_enabled != 0u, kc, g);
-            shadow_light_maps(sp, L, g, ss.csm_cams[C.observer], ss.light_entries[p], first_map, ss.table[C.observer].render_mask, sp.pr.obs);
+            shadow_light_maps(mp, sp.fallback, L, g, ss.csm_cams[C.observer], ss.light_entries[p], first_map, ss.table[C.observer].render_mask, mp.pr.obs);
             ss.cand[p].row = first_map;
         }
         __syncthreads(); // the rows of this round's first candidates
@@ -2200,35 +2141,25 @@ __global__ void __launch_bounds__(kBlock) k_scene_shadow_maps(const NodeArrays a
         __syncthreads();
     }
     if (tid == 0) {
-        *sp.n_maps = s_maps;
+        *mp.n_maps = s_maps;
         *ss.n_refs = s_refs;
     }
 }
 
-void launch_scene_shadow_maps(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const SceneShadowParams &ss, const uint32_t *pr_level_off,
-                              uint32_t n_levels, uint64_t *launches)
+uint32_t launch_scene_shadow_maps(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ShadowParams &sp, const SceneShadowParams &ss)
 {
-    k_scene_shadow_maps<<<1, kBlock, 0, s>>>(a, sp, ss);
-    ++*launches;
-    const bool pruned = pr_level_off != nullptr;
-    if (pruned) launch_pruner_table(k_scene_shadow_pruners, s, a, sp, pr_level_off, n_levels, launches);
-    if (a.cap) {
-        if (pruned) launch_pdl(k_scene_shadow_count<true>, grid_for(a.cap), kBlock, 0, s, a, sp);
-        else launch_pdl(k_scene_shadow_count<false>, grid_for(a.cap), kBlock, 0, s, a, sp);
-        ++*launches;
-    }
-    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
-    ++*launches;
+    k_scene_shadow_maps<<<1, kBlock, 0, s>>>(a, mp, sp, ss);
+    return 1u;
 }
 
 // ------------------------------------------------------------------------------------------------
 // N4 scene observers (fyx_cull_scene_observers): ObserversCollection::from_scene (renderer/observer.rs:88-153) with
 // Camera::calculate_matrices (scene/camera.rs:454-462), then one from_graph per observer (renderer/mod.rs:1034-1047) through
-// the shadow maps' node passes: the observers are the maps.
+// the many-map cull's node passes in kFormObservers: the observers are the maps.
 // ------------------------------------------------------------------------------------------------
 // one observer: its table row, its map row (what k_shadow_scan and the pack read), its frustum with the node's render mask,
 // its view matrix and its LOD observer (translation, z_near, z_far)
-__device__ __forceinline__ void observer_out(const ShadowParams &sp, const ObserverParams &op, const uint32_t m, const uint32_t node, const uint32_t kind, const uint32_t face,
+__device__ __forceinline__ void observer_out(const MapParams &mp, const ObserverParams &op, const uint32_t m, const uint32_t node, const uint32_t kind, const uint32_t face,
                                              const uint32_t mask, const float *t, const float z_near, const float z_far, const float *P,
                                              const float *V)
 {
@@ -2248,28 +2179,27 @@ __device__ __forceinline__ void observer_out(const ShadowParams &sp, const Obser
         o.view[k] = V[k];
         o.projection[k] = P[k];
         o.view_projection[k] = VP[k];
-        sp.views[(size_t)m * 16 + k] = V[k];
+        mp.views[(size_t)m * 16 + k] = V[k];
     }
-    fyx_shadow_map &mp = sp.maps[m];
-    mp.light = node;
-    mp.face = face;
-    mp.cascade = 0u;
-    mp.first = mp.count = 0u;
-    for (int k = 0; k < 16; ++k) mp.view_projection[k] = VP[k];
+    fyx_shadow_map &row = mp.maps[m];
+    row.light = node;
+    row.face = face;
+    row.cascade = 0u;
+    row.first = row.count = 0u;
+    for (int k = 0; k < 16; ++k) row.view_projection[k] = VP[k];
     // renderer/bundle.rs:893-896: from_view_projection_matrix(..).unwrap_or_default()
-    if (!frustum_from_view_projection(VP, sp.scratch[m])) sp.scratch[m] = sp.csm.fallback;
-    to_dev_frustum(sp.scratch[m], mask, 0u, sp.frusta[m]);
-    if (sp.pr.obs) map_observer(sp.pr.obs + (size_t)m * 5, t, z_near, z_far);
+    if (!frustum_from_view_projection(VP, mp.scratch[m])) mp.scratch[m] = op.fallback;
+    to_dev_frustum(mp.scratch[m], mask, 0u, mp.frusta[m]);
+    if (mp.pr.obs) map_observer(mp.pr.obs + (size_t)m * 5, t, z_near, z_far);
 }
 
-// One CTA: the records in order (due probes' six faces, then cameras), the same ordered block scan as k_shadow_frusta
-__global__ void __launch_bounds__(kBlock) k_observer_views(const NodeArrays a, const ShadowParams sp, const ObserverParams op)
+// One CTA: the records in order (due probes' six faces, then cameras), placed by the ordered block scan
+__global__ void __launch_bounds__(kBlock) k_observer_views(const NodeArrays a, const MapParams mp, const ObserverParams op)
 {
-    __shared__ uint32_t s_warp[kBlock / 32];
-    __shared__ uint32_t s_base;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    __shared__ BlockScan<kBlock> s_scan;
+    const uint32_t tid = threadIdx.x;
     pdl_trigger();
-    if (tid == 0) s_base = 0u;
+    if (tid == 0) s_scan.base = 0u;
     for (uint32_t base = 0; base < op.n_recs; base += kBlock) {
         const uint32_t i = base + tid;
         uint32_t n_obs = 0u;
@@ -2286,16 +2216,7 @@ __global__ void __launch_bounds__(kBlock) k_observer_views(const NodeArrays a, c
             // that fails leaves the probe due
             op.recs[i].emitted = R.kind == FYX_OBSERVER_PROBE_FACE && n_obs ? 1u : 0u;
         }
-        uint32_t incl = n_obs;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if (lane >= (uint32_t)o) incl += v;
-        }
-        if (lane == 31u) s_warp[warp] = incl;
-        __syncthreads();
-        uint32_t first = s_base + incl - n_obs;
-        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
+        const uint32_t first = s_scan.place(n_obs);
         if (n_obs) {
             const uint32_t slot = R.slot, node = a.gidx[slot], mask = a.mask[slot];
             const float4 r0 = a.G[0][slot], r1 = a.G[1][slot], r2 = a.G[2][slot];
@@ -2309,7 +2230,7 @@ __global__ void __launch_bounds__(kBlock) k_observer_views(const NodeArrays a, c
                 const bool own = R.v[0] != 0.0f || R.v[1] != 0.0f; // a render target's size (camera.rs:813-826)
                 camera_projection(R.mode, R.m22_or_vertical_size, R.z_near, R.z_far, own ? R.v[0] : op.frame_size[0],
                                   own ? R.v[1] : op.frame_size[1], P);
-                observer_out(sp, op, first, node, FYX_OBSERVER_CAMERA, 0u, mask, pos, R.z_near, R.z_far, P, V);
+                observer_out(mp, op, first, node, FYX_OBSERVER_CAMERA, 0u, mask, pos, R.z_near, R.z_far, P, V);
             } else {
                 // observer.rs:104-145: perspective fov 90°, aspect 1 (a cube face); translation = global_rendering_position
                 const float t[3] = {FYX_ADD(pos[0], R.v[0]), FYX_ADD(pos[1], R.v[1]), FYX_ADD(pos[2], R.v[2])};
@@ -2319,22 +2240,19 @@ __global__ void __launch_bounds__(kBlock) k_observer_views(const NodeArrays a, c
                     const float target[3] = {FYX_ADD(t[0], c_face_look[k][0]), FYX_ADD(t[1], c_face_look[k][1]), FYX_ADD(t[2], c_face_look[k][2])};
                     const float up[3] = {c_face_up[k][0], c_face_up[k][1], c_face_up[k][2]};
                     look_at_rh(t, target, up, V);
-                    observer_out(sp, op, first + k, node, FYX_OBSERVER_PROBE_FACE, k, mask, t, R.z_near, R.z_far, P, V);
+                    observer_out(mp, op, first + k, node, FYX_OBSERVER_PROBE_FACE, k, mask, t, R.z_near, R.z_far, P, V);
                 }
             }
         }
-        __syncthreads();
-        if (tid == kBlock - 1) s_base = first + n_obs;
-        __syncthreads();
     }
-    if (tid == 0) *sp.n_maps = s_base;
+    if (tid == 0) *mp.n_maps = s_scan.base;
 }
 
 // The light lists and environment maps of every observer in one pass over the flag column (k_cull_lights and
 // k_select_probes for any number of observers): EMIT = false counts each observer's lights and picks its environment map,
 // EMIT = true writes the lights at the cursors of k_observer_light_scan.
 template <bool EMIT>
-__global__ void __launch_bounds__(kBlock) k_observer_lights(const NodeArrays a, const ShadowParams sp, const ObserverParams op)
+__global__ void __launch_bounds__(kBlock) k_observer_lights(const NodeArrays a, const MapParams mp, const ObserverParams op)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x;
     pdl_wait();
@@ -2345,14 +2263,12 @@ __global__ void __launch_bounds__(kBlock) k_observer_lights(const NodeArrays a, 
     const bool light = (nf & need) == need, env = !EMIT && (nf & probe) == probe;
     if (!light && !env) return;
     const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
-    PackedConsts kc;
-    kc.one = make_float2(1.0f, 1.0f);
-    kc.negzero = make_float2(-0.0f, -0.0f);
+    const PackedConsts kc = packed_consts();
     const bool tame = aabb_is_tame(wx, wy, wz);
     const uint32_t gi = a.gidx[slot];
-    const uint32_t n = *sp.n_maps;
+    const uint32_t n = *mp.n_maps;
     for (uint32_t m = 0; m < n; ++m) {
-        if (light && frustum_intersects_aabb(sp.frusta[m], wx, wy, wz, kc, tame)) {
+        if (light && frustum_intersects_aabb(mp.frusta[m], wx, wy, wz, kc, tame)) {
             uint32_t *c = op.light_counts + (size_t)m * kCountStride;
             if (EMIT) op.light_raw[atomicAdd(c, 1u)] = gi;
             else atomicAdd(c, 1u);
@@ -2366,41 +2282,28 @@ __global__ void __launch_bounds__(kBlock) k_observer_lights(const NodeArrays a, 
 }
 
 // One CTA: the table's lists (from the map rows of k_shadow_scan), the light lists' places, the environment maps
-__global__ void __launch_bounds__(1024) k_observer_light_scan(const ShadowParams sp, const ObserverParams op)
+__global__ void __launch_bounds__(1024) k_observer_light_scan(const MapParams mp, const ObserverParams op)
 {
-    __shared__ uint32_t s_warp[32];
-    __shared__ uint32_t s_base;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    __shared__ BlockScan<1024u> s_scan;
+    const uint32_t tid = threadIdx.x;
     pdl_wait();
-    if (tid == 0) s_base = 0u;
-    const uint32_t n = *sp.n_maps;
+    if (tid == 0) s_scan.base = 0u;
+    const uint32_t n = *mp.n_maps;
     for (uint32_t base = 0; base < n; base += 1024u) {
         const uint32_t m = base + tid;
         const uint32_t c = m < n ? op.light_counts[(size_t)m * kCountStride] : 0u;
-        uint32_t incl = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-            if (lane >= (uint32_t)o) incl += v;
-        }
-        if (lane == 31u) s_warp[warp] = incl;
-        __syncthreads();
-        uint32_t first = s_base + incl - c;
-        for (uint32_t w = 0; w < warp; ++w) first += s_warp[w];
+        const uint32_t first = s_scan.place(c);
         if (m < n) {
             fyx_scene_observer &o = op.table[m];
-            o.first = sp.maps[m].first;
-            o.count = sp.maps[m].count;
+            o.first = mp.maps[m].first;
+            o.count = mp.maps[m].count;
             o.lights_first = first;
             o.lights_count = c;
             o.environment_map = op.best[m] ? op.best[m] - 1u : FYX_NONE;
             op.light_counts[(size_t)m * kCountStride] = first;
         }
-        __syncthreads();
-        if (tid == 1023u) s_base = first + c;
-        __syncthreads();
     }
-    if (tid == 0) *op.light_total = s_base;
+    if (tid == 0) *op.light_total = s_scan.base;
 }
 
 // One CTA per observer: its light list into ascending node index (pool order, as the reference's pair_iter).  Node
@@ -2428,38 +2331,38 @@ __global__ void __launch_bounds__(kBlock) k_observer_commit(ObserverRecDev *recs
     if (i < n && recs[i].emitted) recs[i].rendered = 1u;
 }
 
-void launch_observers_commit(cudaStream_t s, ObserverRecDev *recs, uint32_t n_recs)
+uint32_t launch_observers_commit(cudaStream_t s, ObserverRecDev *recs, uint32_t n_recs)
 {
-    if (n_recs) k_observer_commit<<<grid_for(n_recs), kBlock, 0, s>>>(recs, n_recs);
+    if (!n_recs) return 0u;
+    k_observer_commit<<<grid_for(n_recs), kBlock, 0, s>>>(recs, n_recs);
+    return 1u;
 }
 
-void launch_observers(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, const uint32_t *pr_level_off,
-                      uint32_t n_levels, uint64_t *launches)
+uint32_t launch_observer_views(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ObserverParams &op)
 {
-    k_observer_views<<<1, kBlock, 0, s>>>(a, sp, op);
-    ++*launches;
-    const bool pruned = pr_level_off != nullptr;
-    if (pruned) launch_pruner_table(k_shadow_pruners<true>, s, a, sp, pr_level_off, n_levels, launches);
-    if (a.cap) {
-        if (pruned) launch_pdl(k_shadow_count<true, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
-        else launch_pdl(k_shadow_count<false, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
-        launch_pdl(k_observer_lights<false>, grid_for(a.cap), kBlock, 0, s, a, sp, op);
-        *launches += 2;
-    }
-    launch_pdl(k_shadow_scan, 1, 1024, 0, s, sp);
-    launch_pdl(k_observer_light_scan, 1, 1024, 0, s, sp, op);
-    *launches += 2;
+    k_observer_views<<<1, kBlock, 0, s>>>(a, mp, op);
+    return 1u;
 }
 
-void launch_observers_emit(cudaStream_t s, const NodeArrays &a, const ShadowParams &sp, const ObserverParams &op, bool pruned, uint32_t n_obs,
-                           uint64_t *launches)
+uint32_t launch_observer_lights(cudaStream_t s, const NodeArrays &a, const MapParams &mp, const ObserverParams &op, bool emit)
 {
-    if (!a.cap || !n_obs) return;
-    if (pruned) launch_pdl(k_shadow_emit<true, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
-    else launch_pdl(k_shadow_emit<false, true>, grid_for(a.cap), kBlock, 0, s, a, sp);
-    launch_pdl(k_observer_lights<true>, grid_for(a.cap), kBlock, 0, s, a, sp, op);
+    if (!a.cap) return 0u;
+    if (emit) launch_pdl(k_observer_lights<true>, grid_for(a.cap), kBlock, 0, s, a, mp, op);
+    else launch_pdl(k_observer_lights<false>, grid_for(a.cap), kBlock, 0, s, a, mp, op);
+    return 1u;
+}
+
+uint32_t launch_observer_light_scan(cudaStream_t s, const MapParams &mp, const ObserverParams &op)
+{
+    launch_pdl(k_observer_light_scan, 1, 1024, 0, s, mp, op);
+    return 1u;
+}
+
+uint32_t launch_observer_light_sort(cudaStream_t s, const ObserverParams &op, uint32_t n_obs)
+{
+    if (!n_obs) return 0u;
     launch_pdl(k_observer_light_sort, n_obs, kBlock, 0, s, op);
-    *launches += 3;
+    return 1u;
 }
 
 // the pruners mark their own slots of the column

@@ -84,6 +84,13 @@ __host__ __device__ __forceinline__ float2 aabb_transform_row(const float4 row, 
 struct PackedConsts {
     float2 one, negzero;
 };
+__device__ __forceinline__ PackedConsts packed_consts(const float one = 1.0f, const float negzero = -0.0f)
+{
+    PackedConsts kc;
+    kc.one = make_float2(one, one);
+    kc.negzero = make_float2(negzero, negzero);
+    return kc;
+}
 __device__ __forceinline__ float2 mul2(const float2 a, const float2 b, const PackedConsts &)
 {
     return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
