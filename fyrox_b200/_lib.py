@@ -162,6 +162,20 @@ class fyx_instances(C.Structure):
     ]
 
 
+class fyx_dynamic_layout(C.Structure):
+    _fields_ = [("stride", C.c_uint32), ("position_offset", C.c_uint32), ("normal_offset", C.c_uint32), ("tangent_offset", C.c_uint32)]
+
+
+class fyx_dynamic_stream(C.Structure):
+    _fields_ = [("layout_id", C.c_uint32), ("stride", C.c_uint32), ("n_vertices", C.c_uint32), ("n_triangles", C.c_uint32),
+                ("vertices", C.c_void_p), ("triangles", C.c_void_p)]
+
+
+class fyx_dynamic_batches(C.Structure):
+    _fields_ = [("n_bundles", C.c_uint32), ("n_instances", C.c_uint32), ("n_streams", C.c_uint32), ("reserved", C.c_uint32),
+                ("bundles", C.c_void_p), ("instances", C.c_void_p), ("streams", C.POINTER(fyx_dynamic_stream))]
+
+
 LIGHT_UNKNOWN, LIGHT_SPOT, LIGHT_POINT, LIGHT_DIRECTIONAL = 0, 1, 2, 3
 
 
@@ -316,6 +330,15 @@ SYMBOLS = {
     "fyx_get_scene_observer_instances": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),
     "fyx_get_scene_observer_instances_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_instances)]),
     "fyx_get_scene_observer_instance_surfaces": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(u32p)]),
+    "fyx_add_dynamic_surface": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(fyx_dynamic_layout), C.c_uint32,
+                                            C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
+    "fyx_clear_dynamic_surfaces": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
+    "fyx_get_dynamic_batches": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
+    "fyx_get_dynamic_batches_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
+    "fyx_get_shadow_dynamic_batches": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
+    "fyx_get_shadow_dynamic_batches_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
+    "fyx_get_scene_observer_dynamic_batches": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
+    "fyx_get_scene_observer_dynamic_batches_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
     "fyx_pack_scene_observer_bone_matrices": (C.c_int32, [ctx_p]),
     "fyx_get_scene_observer_bone_matrix_blocks_device": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
     "fyx_get_scene_observer_bone_matrix_block": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),

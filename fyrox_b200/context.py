@@ -623,6 +623,63 @@ class Context:
             "bundles": arr(out.bundles, bdt, nb),
         }
 
+    # ---- dynamic batching (BatchingMode::Dynamic, scene/mesh/mod.rs:739-753, 804-833) ----
+    def add_dynamic_surface(self, node: int, ordinal: int, batch_key: int, layout_id: int, layout, vertices, triangles) -> int:
+        """Batch surface `ordinal` of `node` instead of pushing it: layout = (stride, position_offset, normal_offset,
+        tangent_offset) with FYX_NONE for an absent attribute, vertices = the VertexBuffer bytes, triangles = (n, 3) u32."""
+        ly = L.fyx_dynamic_layout(*[int(x) for x in layout])
+        v = np.ascontiguousarray(np.frombuffer(bytes(vertices), np.uint8) if not isinstance(vertices, np.ndarray) else vertices).view(np.uint8)
+        t = np.ascontiguousarray(triangles, dtype=np.uint32).reshape(-1, 3)
+        if v.size % ly.stride:
+            raise ValueError("vertex bytes are not a whole number of records")
+        out = C.c_uint32()
+        self._chk(self._lib.fyx_add_dynamic_surface(self._h, node, ordinal, batch_key, layout_id, C.byref(ly), v.size // ly.stride,
+                                                    v.ctypes.data_as(C.c_void_p) if v.size else None, len(t),
+                                                    t.ctypes.data_as(C.c_void_p) if t.size else None, C.byref(out)))
+        return out.value
+
+    def clear_dynamic_surfaces(self, nodes=None):
+        """Drop the dynamic registrations of `nodes` (None = all)."""
+        ix = _u32(nodes)
+        self._chk(self._lib.fyx_clear_dynamic_surfaces(self._h, 0 if ix is None else len(ix), _ptr(ix)))
+
+    DYNAMIC_BUNDLE = np.dtype([("batch_key", "<u4"), ("layout_id", "<u4"), ("first", "<u4"), ("count", "<u4"), ("sort_index", "<u8")])
+    DYNAMIC_INSTANCE = np.dtype([("node", "<u4"), ("triangle_offset", "<u4"), ("triangle_count", "<u4"), ("reserved", "<u4")])
+
+    def dynamic_batches(self, kind: str, index: int, device: bool = False) -> dict:
+        """The dynamic batches of the last pack of `kind` ("frustum", "shadow" or "observer") for segment `index`: bundles and
+        instances (structured arrays) and streams {layout_id: {"stride", "vertices" (u8 bytes), "triangles" ((n, 3) u32)}}.
+        device=True reads through the device getter (the same values, copied here)."""
+        fn = {"frustum": "fyx_get_dynamic_batches", "shadow": "fyx_get_shadow_dynamic_batches",
+              "observer": "fyx_get_scene_observer_dynamic_batches"}[kind] + ("_device" if device else "")
+        out = L.fyx_dynamic_batches()
+        self._chk(getattr(self._lib, fn)(self._h, index, C.byref(out)))
+        if device:
+            import torch
+
+            def arr(p, dtype, count):
+                if count == 0:
+                    return np.empty(0, dtype=dtype)
+                nb = count * np.dtype(dtype).itemsize
+
+                class Dev:
+                    __cuda_array_interface__ = {"shape": (nb,), "typestr": "|u1", "data": (p, False), "version": 3}
+
+                return torch.as_tensor(Dev(), device="cuda").cpu().numpy().view(dtype)
+        else:
+            def arr(p, dtype, count):
+                if count == 0:
+                    return np.empty(0, dtype=dtype)
+                buf = (C.c_char * (count * np.dtype(dtype).itemsize)).from_address(p)
+                return np.frombuffer(buf, dtype=dtype, count=count).copy()
+        streams = {}
+        for k in range(out.n_streams):
+            st = out.streams[k]
+            streams[st.layout_id] = {"stride": st.stride, "vertices": arr(st.vertices, np.uint8, st.n_vertices * st.stride),
+                                     "triangles": arr(st.triangles, np.uint32, st.n_triangles * 3).reshape(-1, 3)}
+        return {"bundles": arr(out.bundles, self.DYNAMIC_BUNDLE, out.n_bundles),
+                "instances": arr(out.instances, self.DYNAMIC_INSTANCE, out.n_instances), "streams": streams}
+
     def pack_bone_matrices(self, frustum: int):
         """Bone-matrix blocks (255 mat4, zero padded) of the skinned instances of the last pack_instances (bundle.rs:484-496)."""
         self._chk(self._lib.fyx_pack_bone_matrices(self._h, frustum))

@@ -11,6 +11,7 @@
 #include <memory>
 #include <new>
 #include <string>
+#include <unordered_set>
 #include <utility>
 #include <vector>
 
@@ -231,6 +232,14 @@ struct InstPack {
     uint32_t h_seg = FYX_NONE, h_surf_seg = FYX_NONE;
     bool valid = false, blocks_valid = false;
     uint32_t segments() const { return (uint32_t)inst_first.size() - 1; }
+    // the dynamic batches of every segment (fyx_dynamic_batches): bundles and instances at dyn_item0[seg], each segment's
+    // streams (one per layout it uses, ascending layout id) at dyn_stream0[seg] of dyn_streams with device pointers
+    DevBuf b_dyn_bundles, b_dyn_inst, b_dyn_vtx, b_dyn_tri;
+    std::vector<uint32_t> dyn_item0, dyn_counts, dyn_stream0; // [segments + 1], [segments * 2] bundles / instances, [segments + 1]
+    std::vector<fyx_dynamic_stream> dyn_streams;
+    PinnedBuf h_dyn[4];                     // bundles, instances, vertices, triangles of segment h_dyn_seg
+    std::vector<fyx_dynamic_stream> dyn_out_host, dyn_out_dev; // the streams handed out by the last host / device getter
+    uint32_t h_dyn_seg = FYX_NONE;
 };
 
 // N4: what a many-map cull leaves (fyx_drawprep.inl; MapParams in fyx_internal.h): the map table, the lists, their pinned
@@ -260,6 +269,15 @@ struct PackScratch {
     DevBuf hist, first_key, offset, tmp_sort, seg, tiles, totals;
     PinnedBuf h_totals;
     int32_t ensure(fyx_ctx *c, size_t bins, size_t entries, size_t segments);
+    // the dynamic pass (DynParams): the host's small arrays, the bitmap and counts, the per-item scratch, the hash tables
+    DevBuf dyn_small, dyn_bitmap, dyn_counts, dyn_items32, dyn_items64, dyn_hkey, dyn_hval;
+    PinnedBuf h_dyn_counts;
+};
+
+// Dynamic batching: one registered surface (fyx_add_dynamic_surface)
+struct DynReg {
+    uint32_t id, node, ordinal, batch_key, layout, n_verts, n_tris, tri_src;
+    uint64_t vtx_src;
 };
 
 } // namespace
@@ -432,6 +450,19 @@ struct fyx_ctx {
     DevBuf b_rank_slot;
     PackScratch pack;
     InstPack inst[FYX_MAX_FRUSTA];
+
+    // dynamic batching (fyx_drawprep.inl): the registrations and their pools; layouts and batch keys as first given; the
+    // device tables in push order (DynItemDev, dyn_flush), rebuilt when a registration, the topology or the DFS order changes
+    std::vector<DynReg> dyn_regs;
+    std::unordered_set<uint64_t> dyn_pairs;      // node << 32 | ordinal of every registration
+    uint32_t dyn_next_id = 0;
+    std::vector<fyx_dynamic_layout> dyn_layouts; // by layout id; stride FYX_NONE = no registration uses it
+    std::vector<uint32_t> dyn_key_layout;        // by batch key; FYX_NONE = no registration uses it
+    DevBuf b_dyn_vtx, b_dyn_tri;                 // pools: vertex bytes (each surface 16-byte aligned), triangles
+    uint64_t dyn_vtx_used = 0, dyn_tri_used = 0;
+    bool dyn_dirty = false;
+    uint32_t dyn_nodes = 0, dyn_items = 0, dyn_n_layouts = 0;
+    DevBuf b_dyn_of_slot, b_dyn_item_first, b_dyn_ordinal, b_dyn_items, b_dyn_layouts;
 
     // multi-GPU (fyx_comm.cu)
     void *comm = nullptr;
@@ -885,6 +916,23 @@ extern "C" void fyx_frustum_default(fyx_frustum *out)
 
 extern "C" void fyx_mat4_mul(const float a[16], const float b[16], float out[16]) { mat4_mul(a, b, out); }
 
+// Drops the dynamic registrations `gone` selects; the pairs, batch keys and layouts in use are those of the rest
+template <class Pred> void dyn_drop(fyx_ctx *c, Pred gone)
+{
+    c->dyn_regs.erase(std::remove_if(c->dyn_regs.begin(), c->dyn_regs.end(), gone), c->dyn_regs.end());
+    c->dyn_pairs.clear();
+    std::vector<uint8_t> key_used(c->dyn_key_layout.size(), 0), layout_used(c->dyn_layouts.size(), 0);
+    for (const DynReg &r : c->dyn_regs) {
+        c->dyn_pairs.insert((uint64_t)r.node << 32 | r.ordinal);
+        key_used[r.batch_key] = layout_used[r.layout] = 1;
+    }
+    for (size_t k = 0; k < key_used.size(); ++k)
+        if (!key_used[k]) c->dyn_key_layout[k] = FYX_NONE;
+    for (size_t l = 0; l < layout_used.size(); ++l)
+        if (!layout_used[l]) c->dyn_layouts[l].stride = FYX_NONE;
+    c->dyn_dirty = true;
+}
+
 // --------------------------------------------------------------------------------------------
 // scene description
 // --------------------------------------------------------------------------------------------
@@ -1148,6 +1196,8 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     for (size_t i = 0; i < c->probe_src.size(); ++i)
         if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->probe_src[i].present = 0u;
     c->obs_table_dirty = true;
+    // dynamic registrations too
+    dyn_drop(c, [&](const DynReg &r) { return r.node >= capacity || c->slot_of_node[r.node] == FYX_NONE; });
     c->ms_dirty = c->have_ms;  // the per-slot surface table too (the CSR itself is by node)
     if (c->ms_of_node.size() < capacity) c->ms_of_node.resize(capacity, make_uint2(0u, 0u));
     c->anim_csr_dirty = true; // animated nodes are addressed by slot
@@ -1164,6 +1214,7 @@ extern "C" int32_t fyx_set_dfs_order(fyx_ctx *c, uint32_t capacity, const uint32
     else c->dfs_rank.clear();
     c->rank_on_device = false;
     c->tables_dirty = true;
+    c->dyn_dirty = true;
     return FYX_OK;
 }
 

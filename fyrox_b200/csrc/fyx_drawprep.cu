@@ -39,6 +39,17 @@ __device__ __forceinline__ uint2 surfaces_of(const InstParams &ip, const uint32_
 }
 __device__ __forceinline__ uint32_t warp_max_u32(const uint32_t v) { return __reduce_max_sync(0xFFFFFFFFu, v); }
 
+// the node's dense dynamic index (FYX_NONE = no surface of it is batched)
+__device__ __forceinline__ uint32_t dyn_node(const InstParams &ip, const uint32_t slot) { return ip.dyn_of_slot ? ip.dyn_of_slot[slot] : FYX_NONE; }
+// surface k of dynamic node d is batched, not pushed (scene/mesh/mod.rs:739-753)
+__device__ __forceinline__ bool dyn_surface(const InstParams &ip, const uint32_t d, const uint32_t k)
+{
+    if (d == FYX_NONE) return false;
+    for (uint32_t j = ip.dyn_item_first[d]; j < ip.dyn_item_first[d + 1]; ++j)
+        if (ip.dyn_ordinal[j] == k) return true;
+    return false;
+}
+
 // the segment (shadow map of the group) that owns list position i: the last map whose first entry is <= the entry (maps with
 // an empty list share their first with the next map and lose to it)
 __device__ __forceinline__ uint32_t segment_of(const InstParams &ip, const uint32_t i)
@@ -60,7 +71,7 @@ template <bool kSeg> __device__ __forceinline__ void inst_keys(const NodeArrays 
 {
     const uint32_t i = blockIdx.x * kBlock + threadIdx.x;
     const bool valid = i < ip.n;
-    uint32_t slot = 0u, nsurf = 0u, seg = FYX_NONE, bin0 = 0u;
+    uint32_t slot = 0u, nsurf = 0u, ninst = 0u, seg = FYX_NONE, bin0 = 0u, dn = FYX_NONE;
     uint2 sr = make_uint2(0u, 0u);
     unsigned long long key = ~0ull;
     if (valid) {
@@ -77,17 +88,20 @@ template <bool kSeg> __device__ __forceinline__ void inst_keys(const NodeArrays 
         const uint32_t rank = ip.rank_of_slot ? ip.rank_of_slot[slot] : ip.vis_node[i];
         key = ((unsigned long long)rank << 32) | i;
         sr = surfaces_of(ip, slot);
-        nsurf = sr.y ? sr.y : 1u;
+        nsurf = ninst = sr.y ? sr.y : 1u;
+        dn = dyn_node(ip, slot);
+        if (dn != FYX_NONE)
+            for (uint32_t k = 0; k < nsurf; ++k) ninst -= dyn_surface(ip, dn, k) ? 1u : 0u;
     }
     const int lane = threadIdx.x & 31;
     if constexpr (kSeg) { // instances per map (a map's entries are contiguous: one or two atomics per warp)
         const uint32_t peers = __match_any_sync(0xFFFFFFFFu, seg);
-        const uint32_t sum = __reduce_add_sync(peers, nsurf);
+        const uint32_t sum = __reduce_add_sync(peers, ninst);
         if (valid && lane == __ffs(peers) - 1) atomicAdd(ip.seg_inst + seg, sum);
     }
     const uint32_t rounds = warp_max_u32(nsurf);
     for (uint32_t k = 0; k < rounds; ++k) {
-        const bool act = k < nsurf;
+        const bool act = k < nsurf && !dyn_surface(ip, dn, k);
         uint32_t b = 0xFFFFFFFFu;
         if (act) b = bin0 + (sr.y ? ip.ms_bundle[sr.x + k] : (ip.bundle_of_slot ? ip.bundle_of_slot[slot] : 0u));
         // warp-aggregated histogram: one atomic per distinct bin in the warp
@@ -303,12 +317,13 @@ template <bool kSeg> __device__ __forceinline__ void inst_scatter(const NodeArra
     const uint32_t i = blockIdx.x * kBlock + threadIdx.x;
     const int lane = threadIdx.x & 31;
     const bool valid = i < ip.n;
-    uint32_t slot = 0u, nsurf = 0u, node_flags = 0u, bin0 = 0u, map = 0u;
+    uint32_t slot = 0u, nsurf = 0u, node_flags = 0u, bin0 = 0u, map = 0u, dn = FYX_NONE;
     uint2 sr = make_uint2(0u, 0u);
     if (valid) {
         slot = ip.vis_slot[i];
         sr = surfaces_of(ip, slot);
         nsurf = sr.y ? sr.y : 1u;
+        dn = dyn_node(ip, slot);
         node_flags = a.flags[slot];
         if constexpr (kSeg) {
             const uint32_t seg = segment_of(ip, i);
@@ -318,7 +333,7 @@ template <bool kSeg> __device__ __forceinline__ void inst_scatter(const NodeArra
     }
     const uint32_t rounds = warp_max_u32(nsurf);
     for (uint32_t k = 0; k < rounds; ++k) {
-        const bool act = k < nsurf;
+        const bool act = k < nsurf && !dyn_surface(ip, dn, k);
         uint32_t b = 0xFFFFFFFFu, pos = 0u, skin = FYX_NONE;
         if (act) {
             b = bin0 + (sr.y ? ip.ms_bundle[sr.x + k] : (ip.bundle_of_slot ? ip.bundle_of_slot[slot] : 0u));
@@ -381,6 +396,318 @@ template <bool kSeg> __device__ __forceinline__ void inst_scatter(const NodeArra
 
 __global__ void __launch_bounds__(kBlock) k_inst_scatter(const NodeArrays a, const InstParams ip) { inst_scatter<false>(a, ip); }
 __global__ void __launch_bounds__(kBlock) k_shadow_inst_scatter(const NodeArrays a, const InstParams ip) { inst_scatter<true>(a, ip); }
+
+// ---- Dynamic batching: one pack's dynamic pass (DynParams) ----
+// the segment of list entry i: the last whose first entry is <= i (an empty segment shares its first with the next and loses)
+__device__ __forceinline__ uint32_t dyn_segment(const DynParams &dp, const uint32_t i)
+{
+    uint32_t lo = 0u, hi = dp.n_seg - 1u;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (dp.seg_first[mid] <= i) lo = mid;
+        else hi = mid - 1u;
+    }
+    return lo;
+}
+
+// mark: the segment's dynamic nodes as bits (dense index = push order), its items, vertices and triangles per layout; the
+// counts are summed over the warp's lanes that hit the same (segment, layout) before one atomic per counter
+__global__ void __launch_bounds__(kBlock) k_dyn_mark(const DynParams dp)
+{
+    const uint32_t i = blockIdx.x * kBlock + threadIdx.x;
+    uint32_t d = FYX_NONE, seg = 0u, j0 = 0u, nj = 0u;
+    if (i < dp.n) d = dp.dyn_of_slot[dp.vis_slot[i]];
+    if (d != FYX_NONE) {
+        seg = dyn_segment(dp, i);
+        atomicOr(dp.bitmap + (size_t)seg * dp.words + (d >> 5), 1u << (d & 31u));
+        j0 = dp.item_first[d];
+        nj = dp.item_first[d + 1] - j0;
+    }
+    const uint32_t rounds = warp_max_u32(nj);
+    const int lane = threadIdx.x & 31;
+    for (uint32_t k = 0; k < rounds; ++k) {
+        uint32_t key = FYX_NONE, nv = 0u, nt = 0u;
+        if (k < nj) {
+            const DynItemDev it = dp.items[j0 + k];
+            key = seg * dp.n_layouts + it.layout;
+            nv = it.n_verts;
+            nt = it.n_tris;
+        }
+        const uint32_t peers = __match_any_sync(0xFFFFFFFFu, key);
+        const uint32_t cnt = __popc(peers), sv = __reduce_add_sync(peers, nv), st = __reduce_add_sync(peers, nt);
+        if (key != FYX_NONE && lane == __ffs(peers) - 1) {
+            uint32_t *c = dp.counts + (size_t)key * 3u;
+            atomicAdd(c, cnt);
+            atomicAdd(c + 1, sv);
+            atomicAdd(c + 2, st);
+        }
+    }
+}
+
+constexpr unsigned long long kDynEmpty = ~0ull; // never a sort index (those stop at u64::MAX - 1) nor a bundle key (batch key < 2^24)
+__device__ __forceinline__ uint32_t dyn_hash(unsigned long long k, const uint32_t mask)
+{
+    k ^= k >> 33;
+    k *= 0xff51afd7ed558ccdull;
+    k ^= k >> 33;
+    k *= 0xc4ceb9fe1a85ec53ull;
+    k ^= k >> 33;
+    return (uint32_t)k & mask;
+}
+// the smallest value inserted with key k wins
+__device__ __forceinline__ void dyn_insert(unsigned long long *keys, uint32_t *vals, const uint32_t mask, const unsigned long long k, const uint32_t v)
+{
+    for (uint32_t h = dyn_hash(k, mask);; h = (h + 1u) & mask) {
+        const unsigned long long prev = atomicCAS(keys + h, kDynEmpty, k);
+        if (prev == kDynEmpty || prev == k) {
+            atomicMin(vals + h, v);
+            return;
+        }
+    }
+}
+__device__ __forceinline__ uint32_t dyn_lookup(const unsigned long long *keys, const uint32_t *vals, const uint32_t mask, const unsigned long long k)
+{
+    for (uint32_t h = dyn_hash(k, mask);; h = (h + 1u) & mask)
+        if (__ldcg(keys + h) == k) return __ldcg(vals + h);
+}
+
+// One CTA per segment, in the reference's push order (items at seg_item0[seg] + p, p = push position):
+//   1. the items of the marked nodes, node after node (bitmap order = DFS rank order);
+//   2. each item's first vertex and triangle in its layout's stream (a scan per layout the segment uses);
+//   3. the bundle key (batch key, sort index): equal sort indices are named by their first item (hash 1), equal keys by their
+//      first item (hash 2) — the bundle's first push;
+//   4. runs (an item starts an instance unless the previous item went to the same bundle: last_bundle_id) and bundles, both
+//      numbered in push order;
+//   5. instances per bundle, their scan, and each run's place in its bundle (push order within the bundle).
+__global__ void __launch_bounds__(kBinThreads) k_dyn_order(const NodeArrays a, const DynParams dp)
+{
+    __shared__ uint32_t s_b[kBinThreads];
+    const uint32_t seg = blockIdx.x, t = threadIdx.x;
+    const uint32_t i0 = dp.seg_item0[seg], ni = dp.seg_item0[seg + 1] - i0;
+    if (ni == 0u) {
+        if (t == 0) dp.o_seg[seg * 2] = dp.o_seg[seg * 2 + 1] = 0u;
+        return;
+    }
+    const uint32_t hmask = dp.seg_hmask[seg];
+    unsigned long long *hk1 = dp.hkey + dp.seg_hash0[seg], *hk2 = hk1 + hmask + 1u;
+    uint32_t *hv1 = dp.hval + dp.seg_hash0[seg], *hv2 = hv1 + hmask + 1u;
+    // Every thread keeps the running carries in registers: the scan's totals are the same in every thread, so no thread
+    // writes a shared carry that another may still be reading.
+    uint2 total, carry = make_uint2(0u, 0u);
+    // 1. items in push order
+    for (uint32_t w0 = 0; w0 < dp.words; w0 += kBinThreads) {
+        const uint32_t w = w0 + t;
+        const uint32_t bits = w < dp.words ? dp.bitmap[(size_t)seg * dp.words + w] : 0u;
+        uint32_t cnt = 0u;
+        for (uint32_t b = bits; b; b &= b - 1u) {
+            const uint32_t d = w * 32u + (__ffs(b) - 1);
+            cnt += dp.item_first[d + 1] - dp.item_first[d];
+        }
+        uint32_t pos = carry.x + cta_exclusive_scan(make_uint2(cnt, 0u), total).x;
+        for (uint32_t b = bits; b; b &= b - 1u) {
+            const uint32_t d = w * 32u + (__ffs(b) - 1);
+            for (uint32_t j = dp.item_first[d]; j < dp.item_first[d + 1]; ++j) dp.ord_item[i0 + pos++] = j;
+        }
+        carry.x += total.x;
+    }
+    __syncthreads(); // the items
+    // 2. vertex and triangle offsets in each layout's stream
+    for (uint32_t l = 0; l < dp.n_layouts; ++l) {
+        if (dp.counts[((size_t)seg * dp.n_layouts + l) * 3u] == 0u) continue;
+        carry = make_uint2(0u, 0u);
+        for (uint32_t p0 = 0; p0 < ni; p0 += kBinThreads) {
+            const uint32_t p = p0 + t;
+            uint2 v = make_uint2(0u, 0u);
+            if (p < ni) {
+                const DynItemDev it = dp.items[dp.ord_item[i0 + p]];
+                if (it.layout == l) v = make_uint2(it.n_verts, it.n_tris);
+            }
+            const uint2 ex = cta_exclusive_scan(v, total);
+            if (p < ni && dp.items[dp.ord_item[i0 + p]].layout == l) {
+                dp.voff[i0 + p] = carry.x + ex.x;
+                dp.toff[i0 + p] = carry.y + ex.y;
+            }
+            carry = make_uint2(carry.x + total.x, carry.y + total.y);
+        }
+    }
+    __syncthreads(); // the offsets
+    // 3. the bundle keys
+    const float *view = dp.views + (size_t)seg * 16u;
+    for (uint32_t p = t; p < ni; p += kBinThreads) {
+        const uint32_t slot = dp.items[dp.ord_item[i0 + p]].slot;
+        const uint64_t si = sorting_index(view, a.G[0][slot].w, a.G[1][slot].w, a.G[2][slot].w);
+        dp.sidx[i0 + p] = si;
+        dyn_insert(hk1, hv1, hmask, si, p);
+    }
+    __syncthreads();
+    for (uint32_t p = t; p < ni; p += kBinThreads) {
+        const uint64_t k2 = ((uint64_t)dp.items[dp.ord_item[i0 + p]].batch_key << 32) | dyn_lookup(hk1, hv1, hmask, dp.sidx[i0 + p]);
+        dp.key2[i0 + p] = k2;
+        dyn_insert(hk2, hv2, hmask, k2, p);
+    }
+    __syncthreads();
+    // 4. runs and bundles in push order
+    carry = make_uint2(0u, 0u);
+    for (uint32_t p0 = 0; p0 < ni; p0 += kBinThreads) {
+        const uint32_t p = p0 + t;
+        uint32_t bfirst = FYX_NONE, run_start = 0u, bstart = 0u;
+        uint64_t k2 = 0;
+        if (p < ni) {
+            k2 = __ldcg(dp.key2 + i0 + p);
+            bfirst = dyn_lookup(hk2, hv2, hmask, k2);
+            run_start = (p == 0u || __ldcg(dp.key2 + i0 + p - 1u) != k2) ? 1u : 0u;
+            bstart = bfirst == p ? 1u : 0u;
+        }
+        const uint2 ex = cta_exclusive_scan(make_uint2(run_start, bstart), total);
+        const uint32_t r = carry.x + ex.x + run_start - 1u; // the item's run
+        if (p < ni) {
+            dp.run_of[i0 + p] = r;
+            if (bstart) {
+                const uint32_t b = carry.y + ex.y;
+                dp.bord[i0 + p] = b;
+                const DynItemDev it = dp.items[dp.ord_item[i0 + p]];
+                fyx_dynamic_bundle rec;
+                rec.batch_key = it.batch_key;
+                rec.layout_id = it.layout;
+                rec.first = rec.count = 0u;
+                rec.sort_index = dp.sidx[i0 + p];
+                dp.o_bundles[i0 + b] = rec;
+            }
+        }
+        __syncthreads(); // the bundle numbers of this chunk's first pushes
+        if (p < ni && run_start) {
+            const uint32_t b = __ldcg(dp.bord + i0 + bfirst);
+            dp.run_item[i0 + r] = p;
+            dp.run_bundle[i0 + r] = b;
+            atomicAdd(dp.bcur + i0 + b, 1u);
+        }
+        carry = make_uint2(carry.x + total.x, carry.y + total.y);
+        __syncthreads(); // this chunk's atomics before the counts are read
+    }
+    const uint32_t n_runs = carry.x, n_bundles = carry.y;
+    // each run's last triangle: the run's items are consecutive pushes of one layout
+    for (uint32_t p = t; p < ni; p += kBinThreads) {
+        const uint32_t r = dp.run_of[i0 + p];
+        if (p + 1u == ni || __ldcg(dp.run_of + i0 + p + 1u) != r) dp.run_tend[i0 + r] = dp.toff[i0 + p] + dp.items[dp.ord_item[i0 + p]].n_tris;
+    }
+    // 5. the bundles' instances: counts -> first instance (bcur becomes the cursor)
+    __syncthreads();
+    carry = make_uint2(0u, 0u);
+    for (uint32_t b0 = 0; b0 < n_bundles; b0 += kBinThreads) {
+        const uint32_t b = b0 + t;
+        const uint32_t c = b < n_bundles ? __ldcg(dp.bcur + i0 + b) : 0u;
+        const uint32_t first = carry.x + cta_exclusive_scan(make_uint2(c, 0u), total).x;
+        if (b < n_bundles) {
+            dp.bcur[i0 + b] = first;
+            dp.o_bundles[i0 + b].first = first;
+            dp.o_bundles[i0 + b].count = c;
+        }
+        carry.x += total.x;
+    }
+    __syncthreads(); // every bundle's first instance
+    // each run's instance: its bundle's cursor before this chunk, plus the earlier runs of the same bundle in the chunk
+    for (uint32_t r0 = 0; r0 < n_runs; r0 += kBinThreads) {
+        const uint32_t r = r0 + t;
+        const uint32_t b = r < n_runs ? __ldcg(dp.run_bundle + i0 + r) : FYX_NONE;
+        s_b[t] = b;
+        __syncthreads();
+        if (r < n_runs) {
+            uint32_t rank = 0u;
+            for (uint32_t j = 0; j < t; ++j) rank += s_b[j] == b ? 1u : 0u;
+            const uint32_t p = __ldcg(dp.run_item + i0 + r);
+            const uint32_t tf = __ldcg(dp.toff + i0 + p);
+            fyx_dynamic_instance inst;
+            inst.node = dp.items[__ldcg(dp.ord_item + i0 + p)].node;
+            inst.triangle_offset = tf;
+            inst.triangle_count = __ldcg(dp.run_tend + i0 + r) - tf;
+            inst.reserved = 0u;
+            dp.o_inst[i0 + __ldcg(dp.bcur + i0 + b) + rank] = inst;
+        }
+        __syncthreads();
+        if (r < n_runs) atomicAdd(dp.bcur + i0 + b, 1u);
+        __syncthreads();
+    }
+    if (t == 0) {
+        dp.o_seg[seg * 2] = n_bundles;
+        dp.o_seg[seg * 2 + 1] = n_runs;
+    }
+}
+
+// a float at any byte alignment
+__device__ __forceinline__ float dyn_ld(const unsigned char *p)
+{
+    return __uint_as_float((uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24));
+}
+__device__ __forceinline__ void dyn_st(unsigned char *p, const float f)
+{
+    const uint32_t u = __float_as_uint(f);
+    p[0] = (unsigned char)u;
+    p[1] = (unsigned char)(u >> 8);
+    p[2] = (unsigned char)(u >> 16);
+    p[3] = (unsigned char)(u >> 24);
+}
+// Matrix4::transform_point / transform_vector (nalgebra) of an affine world matrix, rows r0..r2, bottom row (0, 0, 0, 1):
+// t = M3x3 * v (+ translation), n = row3 . v (+ 1); t / n unless n == 0 (scene/mesh/mod.rs:109-126)
+__device__ __forceinline__ void dyn_transform(const float4 &r0, const float4 &r1, const float4 &r2, const float *v, const bool point, float *o)
+{
+    const float4 r[3] = {r0, r1, r2};
+    float n = FYX_ADD(FYX_ADD(FYX_MUL(0.0f, v[0]), FYX_MUL(0.0f, v[1])), FYX_MUL(0.0f, v[2]));
+    if (point) n = FYX_ADD(n, 1.0f);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        float x = FYX_ADD(FYX_ADD(FYX_MUL(r[i].x, v[0]), FYX_MUL(r[i].y, v[1])), FYX_MUL(r[i].z, v[2]));
+        if (point) x = FYX_ADD(x, r[i].w);
+        o[i] = (n != 0.0f) ? __fdiv_rn(x, n) : x;
+    }
+}
+
+// geometry, one warp per item: the vertex records copied (u32-wide when the stride allows), then the three attributes
+// transformed by the node's world matrix; the triangles shifted by the item's first vertex in its stream
+__global__ void __launch_bounds__(kBlock) k_dyn_geometry(const NodeArrays a, const DynParams dp, const uint32_t n_items)
+{
+    const uint32_t q = (blockIdx.x * kBlock + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    if (q >= n_items) return;
+    uint32_t lo = 0u, hi = dp.n_seg - 1u; // the item's segment
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1u) >> 1;
+        if (dp.seg_item0[mid] <= q) lo = mid;
+        else hi = mid - 1u;
+    }
+    const DynItemDev it = dp.items[dp.ord_item[q]];
+    const DynLayoutDev ly = dp.layouts[it.layout];
+    const size_t sl = (size_t)lo * dp.n_layouts + it.layout;
+    const uint32_t v0 = dp.voff[q];
+    const unsigned char *src = dp.vtx + it.vtx_src;
+    unsigned char *dst = dp.o_vtx + dp.stream_vtx[sl] + (size_t)v0 * ly.stride;
+    const uint32_t bytes = it.n_verts * ly.stride;
+    if ((ly.stride & 3u) == 0u) {
+        for (uint32_t e = lane; e < bytes / 4u; e += 32u) reinterpret_cast<uint32_t *>(dst)[e] = reinterpret_cast<const uint32_t *>(src)[e];
+    } else {
+        for (uint32_t e = lane; e < bytes; e += 32u) dst[e] = src[e];
+    }
+    const uint32_t *ts = dp.tri + it.tri_src;
+    uint32_t *td = dp.o_tri + ((size_t)dp.stream_tri[sl] + dp.toff[q]) * 3u;
+    for (uint32_t e = lane; e < it.n_tris * 3u; e += 32u) td[e] = ts[e] + v0;
+    __syncwarp();
+    const float4 r0 = a.G[0][it.slot], r1 = a.G[1][it.slot], r2 = a.G[2][it.slot];
+    for (uint32_t v = lane; v < it.n_verts; v += 32u) {
+        const unsigned char *s = src + (size_t)v * ly.stride;
+        unsigned char *d = dst + (size_t)v * ly.stride;
+        float x[3], o[3];
+        const uint32_t off[3] = {ly.pos, ly.nrm, ly.tan};
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            if (off[k] == FYX_NONE) continue;
+            x[0] = dyn_ld(s + off[k]);
+            x[1] = dyn_ld(s + off[k] + 4);
+            x[2] = dyn_ld(s + off[k] + 8);
+            dyn_transform(r0, r1, r2, x, k == 0, o);
+            dyn_st(d + off[k], o[0]);
+            dyn_st(d + off[k] + 4, o[1]);
+            dyn_st(d + off[k] + 8, o[2]);
+        }
+    }
+}
 
 } // namespace
 
@@ -469,6 +796,18 @@ void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &
     const unsigned grid = (ip.n + kBlock - 1) / kBlock;
     if (segmented) k_shadow_inst_scatter<<<grid, kBlock, 0, s>>>(a, ip);
     else k_inst_scatter<<<grid, kBlock, 0, s>>>(a, ip);
+}
+
+void launch_dyn_mark(cudaStream_t s, const DynParams &dp)
+{
+    if (dp.n && dp.n_seg) k_dyn_mark<<<(dp.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(dp);
+}
+
+void launch_dyn_batches(cudaStream_t s, const NodeArrays &a, const DynParams &dp, uint32_t n_items)
+{
+    if (!n_items) return;
+    k_dyn_order<<<dp.n_seg, kBinThreads, 0, s>>>(a, dp);
+    k_dyn_geometry<<<(unsigned)(((uint64_t)n_items * 32u + kBlock - 1) / kBlock), kBlock, 0, s>>>(a, dp, n_items);
 }
 
 } // namespace fyx

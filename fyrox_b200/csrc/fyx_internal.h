@@ -191,7 +191,62 @@ struct InstParams {
     uint32_t *seg_first;            // [n_seg] first instance of the segment (all groups)
     uint32_t *seg_bfirst;           // [n_seg] first bundle of the segment (all groups)
     uint2 *tile_sum;                // [tiles] (instances, bundles) per tile of kScanTile bins, then their exclusive prefix
+    // ---- Dynamic batching (fyx_add_dynamic_surface): surfaces batched by the pack's dynamic pass are not instances.
+    // dyn_of_slot nullptr = none registered; else the node's dense dynamic index (FYX_NONE = none), whose registered
+    // surface ordinals are dyn_ordinal[dyn_item_first[d] .. dyn_item_first[d + 1])
+    const uint32_t *dyn_of_slot, *dyn_item_first, *dyn_ordinal;
 };
+
+// Dynamic batching (scene/mesh/mod.rs:739-753, 804-833; renderer/bundle.rs:1177-1243).  The registered surfaces, in the
+// reference's push order: dynamic nodes ordered by DFS rank (else node index), each node's surfaces by ordinal.
+struct DynItemDev {
+    uint32_t node, slot, batch_key, layout;
+    uint32_t n_verts, n_tris;
+    uint32_t tri_src;   // first u32 of its triangles in the registration pool
+    uint32_t reserved;
+    uint64_t vtx_src;   // first byte of its vertices in the registration pool (16-byte aligned)
+};
+struct DynLayoutDev {
+    uint32_t stride, pos, nrm, tan; // attribute offsets, FYX_NONE = not transformed
+};
+// One pack's dynamic pass over its segments: mark (the segments' dynamic nodes and counts), then, once the host has placed
+// every segment's items, hash tables and (segment, layout) streams, order + bundles (one CTA per segment) and geometry.
+struct DynParams {
+    // registrations
+    const uint32_t *dyn_of_slot, *item_first; // [slots], [D + 1]
+    const DynItemDev *items;
+    const DynLayoutDev *layouts;
+    uint32_t n_layouts, words; // words: bitmap u32 per segment (ceil(D / 32))
+    const unsigned char *vtx;
+    const uint32_t *tri;
+    // the pack's list, cut into segments
+    uint32_t n, n_seg;
+    const uint32_t *vis_slot;
+    const uint32_t *seg_first; // [n_seg + 1] first list entry of each segment, then the list's end
+    const float *views;        // [n_seg * 16] each segment's view matrix
+    uint32_t *bitmap;          // [n_seg * words]
+    uint32_t *counts;          // [n_seg * n_layouts * 3]: items, vertices, triangles
+    // placed by the host from counts
+    const uint32_t *seg_item0;   // [n_seg + 1] first item (all segments' items one after the other)
+    const uint32_t *seg_hash0;   // [n_seg] first entry of the segment's two hash tables
+    const uint32_t *seg_hmask;   // [n_seg] entries per table - 1 (a power of two)
+    const uint64_t *stream_vtx;  // [n_seg * n_layouts] first output byte of each (segment, layout) vertex stream
+    const uint32_t *stream_tri;  // [n_seg * n_layouts] first output triangle of each (segment, layout) stream
+    // per item (in push order, at seg_item0 + position), cleared by the host where noted
+    uint32_t *ord_item, *voff, *toff, *bord, *run_of, *run_item, *run_bundle, *run_tend;
+    uint32_t *bcur;              // per bundle: instances, then the first instance / cursor (cleared to 0)
+    uint64_t *sidx, *key2;
+    unsigned long long *hkey;    // cleared to ~0
+    uint32_t *hval;              // cleared to ~0
+    // outputs
+    fyx_dynamic_bundle *o_bundles;   // at seg_item0[seg]
+    fyx_dynamic_instance *o_inst;    // at seg_item0[seg]
+    uint32_t *o_seg;                 // [n_seg * 2] bundles, instances
+    unsigned char *o_vtx;
+    uint32_t *o_tri;
+};
+void launch_dyn_mark(cudaStream_t s, const DynParams &dp);
+void launch_dyn_batches(cudaStream_t s, const NodeArrays &a, const DynParams &dp, uint32_t n_items);
 // keys + scan (o_totals), then the scatter.  One segment: the one-CTA scan; segmented (the shadow maps of one group): the
 // device-wide scan of the bins
 constexpr uint32_t kScanTile = 4096; // bins per CTA of the device-wide scan

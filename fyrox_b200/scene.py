@@ -190,15 +190,42 @@ class BatchingMode:
     NONE, STATIC, DYNAMIC = "None", "Static", "Dynamic"
 
 
+# AnimatedVertex (scene/mesh/vertex.rs:140-210): position, tex_coord, normal, tangent, bone weights, bone indices
+ANIMATED_VERTEX_ATTRIBUTES = [("position", 12), ("tex_coord0", 8), ("normal", 12), ("tangent", 16), ("bone_weight", 16), ("bone_indices", 4)]
+
+
+def dynamic_layout(attributes) -> tuple:
+    """The fyx_dynamic_layout (stride, position, normal, tangent offsets) of a VertexBuffer layout given as [(usage, size in
+    bytes)] in order.  transform_vertex reaches an attribute through cast_attribute (scene/mesh/buffer.rs:1338-1357), which
+    checks only its size: position and normal are transformed when they are 12 bytes, the tangent when it is 16, whatever the
+    declared component type; otherwise the offset is FYX_NONE."""
+    off, got = 0, {"position": L.FYX_NONE, "normal": L.FYX_NONE, "tangent": L.FYX_NONE}
+    for usage, size in attributes:
+        if usage in got and size == (16 if usage == "tangent" else 12):
+            got[usage] = off
+        off += size
+    return (off, got["position"], got["normal"], got["tangent"])
+
+
 @dataclass
 class Surface:
     """Surface (scene/mesh/surface.rs:1249-1271): bone handles + the VertexBuffer bytes (+ SurfaceData::blend_shapes_container)."""
 
     bones: List[Handle] = field(default_factory=list)
-    vertex_buffer: Optional[np.ndarray] = None  # uint8, AnimatedVertex records
+    vertex_buffer: Optional[np.ndarray] = None  # uint8 records of `layout` (AnimatedVertex unless given)
     surface_id: Optional[int] = None            # fyx surface id once uploaded
     blend_shapes_container: Optional[BlendShapesContainer] = None
+    triangles: Optional[np.ndarray] = None      # (n, 3) u32: SurfaceData::geometry_buffer
+    layout: Optional[list] = None               # [(usage, size in bytes)]: VertexBuffer::layout_descriptor; None = AnimatedVertex
+    material: int = 0                           # the host's key of Surface::material
     _shapes_uploaded: bool = False
+
+    def attributes(self) -> list:
+        return self.layout if self.layout is not None else ANIMATED_VERTEX_ATTRIBUTES
+
+    def vertex_count(self) -> int:
+        stride = dynamic_layout(self.attributes())[0]
+        return 0 if self.vertex_buffer is None else np.asarray(self.vertex_buffer).view(np.uint8).size // stride
 
 
 class Node:
@@ -220,6 +247,7 @@ class Node:
             [np.finfo(f32).max] * 3 + [-np.finfo(f32).max] * 3, f32)
         self.surfaces: List[Surface] = []
         self.batching_mode = BatchingMode.NONE  # Mesh::batching_mode (scene/mesh/mod.rs:372)
+        self.render_path = 0                    # Mesh::render_path: 0 Deferred, 1 Forward
         self._graph: Optional["Graph"] = None
         self._handle = Handle.NONE
 
@@ -233,6 +261,13 @@ class Node:
     def blend_shapes_mut(self) -> List[BlendShape]:
         self._notify("blend_shapes")
         return self.blend_shapes()
+
+    def batched_surfaces(self) -> List[int]:
+        """Ordinals of the surfaces Mesh::collect_render_data batches instead of pushing (scene/mesh/mod.rs:739-753): a Dynamic
+        mesh without blend shapes (on any surface), a surface without bones and with fewer than 256 vertices."""
+        if self.kind != "mesh" or self.batching_mode != BatchingMode.DYNAMIC or self.blend_shapes():
+            return []
+        return [k for k, s in enumerate(self.surfaces) if not s.bones and s.vertex_count() < 256]
 
     def set_batching_mode(self, mode: str):
         """Mesh::set_batching_mode (scene/mesh/mod.rs:612-617); Static => RdcControlFlow::Break when the mesh is rendered."""
@@ -399,6 +434,10 @@ class Graph:
         self._dirty: Dict[str, set] = {"transform": set(), "flags": set(), "mask": set(), "aabb": set(), "blend_shapes": set()}
         self._cache: Dict[str, np.ndarray] = {}
         self._surfaces_uploaded = 0
+        # dynamic batching: dense ids of (material, render path) and of layouts, and what each node has registered
+        self._batch_keys: Dict[tuple, int] = {}
+        self._layout_ids: Dict[tuple, int] = {}
+        self._dynamic: Dict[int, tuple] = {}
         self.root = self.add_node(Node("pivot", "__ROOT__"))  # Graph::new, graph/mod.rs:408-424
 
     # ---- pool ----
@@ -531,6 +570,42 @@ class Graph:
                 s.surface_id = self.ctx.add_skinned_surface(i, bones, ib, s.vertex_buffer, ANIMATED_VERTEX_LAYOUT)
                 self._surfaces_uploaded += 1
         self._upload_blend_shapes()
+        self._register_dynamic()
+
+    def _register_dynamic(self):
+        """Registers exactly the surfaces the reference batches (Node.batched_surfaces): a node whose batched surfaces changed
+        is cleared and registered again; a mesh of several surfaces hands them over (fyx_set_node_surfaces) so the ordinals
+        it registers exist."""
+        want = {}
+        for i, n in enumerate(self._records):
+            if n is None:
+                continue
+            ks = n.batched_surfaces()
+            if ks or i in self._dynamic:
+                want[i] = tuple((k, id(n.surfaces[k]), id(n.surfaces[k].vertex_buffer), id(n.surfaces[k].triangles), n.surfaces[k].material,
+                                 n.render_path) for k in ks)
+        for i in [i for i in self._dynamic if i >= len(self._records) or self._records[i] is None]:
+            del self._dynamic[i]  # the topology change dropped its registrations
+        changed = [i for i, sig in want.items() if self._dynamic.get(i, ()) != sig]
+        if not changed:
+            return
+        self.ctx.clear_dynamic_surfaces(np.array(changed, np.uint32))
+        for i in changed:
+            n, sig = self._records[i], want[i]
+            if sig and len(n.surfaces) > 1:
+                self.ctx.set_node_surfaces([i], [[(0, s.surface_id) for s in n.surfaces]])
+            for k, *_ in sig:
+                s = n.surfaces[k]
+                attrs = tuple(s.attributes())
+                lid = self._layout_ids.setdefault(attrs, len(self._layout_ids))
+                key = self._batch_keys.setdefault((s.material, n.render_path), len(self._batch_keys))
+                tris = s.triangles if s.triangles is not None else np.empty((0, 3), np.uint32)
+                vb = s.vertex_buffer if s.vertex_buffer is not None else np.empty(0, np.uint8)
+                self.ctx.add_dynamic_surface(i, k, key, lid, dynamic_layout(attrs), np.asarray(vb).view(np.uint8), tris)
+            if sig:
+                self._dynamic[i] = sig
+            else:
+                self._dynamic.pop(i, None)
 
     def _upload_blend_shapes(self):
         """SurfaceData::blend_shapes_container -> fyx_set_blend_shapes once, Mesh::blend_shapes weights whenever they were touched."""

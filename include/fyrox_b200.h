@@ -745,6 +745,80 @@ int32_t fyx_get_scene_observer_bone_matrix_blocks_device(fyx_ctx *ctx, uint32_t 
 int32_t fyx_get_scene_observer_bone_matrix_block(fyx_ctx *ctx, uint32_t observer, uint32_t instance, float *out_255x16,
                                                  uint32_t *out_has_block);
 
+/* ---- Dynamic batching (BatchingMode::Dynamic) ----------------------------------------------------------------------
+ * Mesh::collect_render_data batches a surface instead of pushing it when the mesh is BatchingMode::Dynamic, has no blend
+ * shapes, the surface has no bones and it has fewer than 256 vertices (scene/mesh/mod.rs:739-753).  In every pass (camera,
+ * each shadow map, each observer) it then copies the surface's vertices with transform_vertex (scene/mesh/mod.rs:109-126:
+ * position by world.transform_point, normal and tangent xyz by world.transform_vector, tangent w kept) and appends them, with
+ * the surface's triangles shifted by the vertex count so far, to one shared surface per vertex layout (DynamicSurfaceCache,
+ * renderer/cache/mod.rs:225-281) in the bundle keyed by (material, sort index, render path); consecutive push_triangles into
+ * the same bundle extend the last instance instead of adding one (renderer/bundle.rs:1177-1243; scene/mesh/mod.rs:804-833).
+ *
+ * A registered surface is uploaded once and stays in device memory.  The instance packs (fyx_pack_instances,
+ * fyx_pack_shadow_instances, fyx_pack_scene_observer_instances) then no longer pack it as an instance (the other instances keep
+ * their surface ordinals) and build each segment's dynamic batches instead, as one from_graph would. */
+typedef struct fyx_dynamic_layout { /* the VertexBuffer layout, as transform_vertex sees it */
+    uint32_t stride;
+    /* cast_attribute (scene/mesh/buffer.rs:1338-1357) checks only an attribute's size in bytes, never its declared type: give
+     * an offset whenever the attribute's size is 12 bytes (position, normal) or 16 bytes (tangent), else FYX_NONE */
+    uint32_t position_offset; /* 12 bytes: transform_point */
+    uint32_t normal_offset;   /* 12 bytes: transform_vector */
+    uint32_t tangent_offset;  /* 16 bytes: xyz transform_vector, w kept */
+} fyx_dynamic_layout;
+/* Register surface `surface_ordinal` (the Mesh::surfaces index) of `node` as batched.  batch_key = the host's dense id
+ * (< 2^24) for the (material, render path) pair; layout_id = the host's dense id (< 2^16) for the layout's hash, which selects
+ * the shared surface.  verts = n_verts records of layout->stride bytes; triangles = 3 u32 per triangle.  FYX_ERR_INVALID_ARGUMENT
+ * for n_verts >= 256 (the reference pushes such a surface), a surface that fyx_set_node_surfaces names as skinned, an ordinal
+ * the node does not have, a (node, ordinal) already registered, a layout_id given before with another layout, and a
+ * batch_key given before with another layout_id (the reference's push_vertex_raw would panic, scene/mesh/buffer.rs:506-517).
+ * Registrations stay with their node index across fyx_set_topology; a node it removes drops them.  A surface that a later
+ * fyx_set_node_surfaces removes or names skinned is pushed again (its registration is kept but not used).  The call copies the
+ * data before it returns.  out_id may be NULL. */
+int32_t fyx_add_dynamic_surface(fyx_ctx *ctx, uint32_t node, uint32_t surface_ordinal, uint32_t batch_key, uint32_t layout_id,
+                                const fyx_dynamic_layout *layout, uint32_t n_verts, const void *verts, uint32_t n_triangles,
+                                const uint32_t *triangles, uint32_t *out_id);
+/* Drop the registrations of the listed nodes (nodes NULL = of every node).  A batch key or layout id that no registration uses
+ * any more may come back with another layout id or layout.  The pools' space is reused once dropped surfaces are the larger part. */
+int32_t fyx_clear_dynamic_surfaces(fyx_ctx *ctx, uint32_t count, const uint32_t *nodes);
+
+typedef struct fyx_dynamic_bundle {
+    uint32_t batch_key, layout_id;
+    uint32_t first, count; /* the bundle's instances, counted from the segment's first */
+    uint64_t sort_index;   /* that of the node pushed first into the bundle */
+} fyx_dynamic_bundle;
+typedef struct fyx_dynamic_instance {
+    uint32_t node;            /* the first node of the run of pushes the instance covers */
+    uint32_t triangle_offset; /* ElementRange::Specific in its layout's triangle stream */
+    uint32_t triangle_count;
+    uint32_t reserved;
+} fyx_dynamic_instance;
+typedef struct fyx_dynamic_stream { /* one layout's shared surface of the segment */
+    uint32_t layout_id, stride, n_vertices, n_triangles;
+    const void *vertices;       /* [n_vertices * stride] bytes */
+    const uint32_t *triangles;  /* [n_triangles * 3] */
+} fyx_dynamic_stream;
+/* One segment's (frustum, map or observer) dynamic batches.  Bundles in the order of their first push; streams in ascending
+ * layout_id, one per layout the segment uses.  Offsets and indices count from the segment's first vertex and first triangle of
+ * that layout: that is the reference's shared surface when the pass is the first of the frame to use the layout; otherwise
+ * the reference's numbers are these plus the earlier passes' vertex and triangle counts of the layout. */
+typedef struct fyx_dynamic_batches {
+    uint32_t n_bundles, n_instances, n_streams, reserved;
+    const fyx_dynamic_bundle *bundles;
+    const fyx_dynamic_instance *instances;
+    const fyx_dynamic_stream *streams; /* host memory (its vertices / triangles point where the getter says) */
+} fyx_dynamic_batches;
+/* The dynamic batches of the last fyx_pack_instances of `frustum`, fyx_pack_shadow_instances (map) or
+ * fyx_pack_scene_observer_instances (observer): pinned host copies valid until the next host getter call on the same pack or
+ * the next pack, or (_device) pointers into device memory.  The streams array of a host getter's result stays valid until the
+ * next host getter call on that pack, that of a device getter's until the next device getter call.  Refusals are the instance
+ * getters'. */
+int32_t fyx_get_dynamic_batches(fyx_ctx *ctx, uint32_t frustum, fyx_dynamic_batches *out);
+int32_t fyx_get_dynamic_batches_device(fyx_ctx *ctx, uint32_t frustum, fyx_dynamic_batches *out);
+int32_t fyx_get_shadow_dynamic_batches(fyx_ctx *ctx, uint32_t map, fyx_dynamic_batches *out);
+int32_t fyx_get_shadow_dynamic_batches_device(fyx_ctx *ctx, uint32_t map, fyx_dynamic_batches *out);
+int32_t fyx_get_scene_observer_dynamic_batches(fyx_ctx *ctx, uint32_t observer, fyx_dynamic_batches *out);
+int32_t fyx_get_scene_observer_dynamic_batches_device(fyx_ctx *ctx, uint32_t observer, fyx_dynamic_batches *out);
+
 /* ---- multi-GPU: one context per GPU, one process per GPU ------------------------------------- */
 /* The node array is sharded (sub-trees + replicated ancestors, SURVEY §8e); each context culls its
  * shard; the per-frustum visible lists are all-gathered with NCCL over NVLink so every rank holds
