@@ -46,6 +46,7 @@ NODE_DEFAULT = NODE_VISIBILITY | NODE_ENABLED | NODE_FRUSTUM_CULLING | NODE_CAST
 UPDATE_INCREMENTAL = 0
 UPDATE_ALL = 1
 PASS_SHADOW = 1
+SPRITE_3D, SPRITE_RECTANGLE = 1, 2  # fyx_sprite::kind
 FRAME_ASYNC = 1
 FRAME_ALLGATHER = 2
 FRAME_READBACK_OWN = 4
@@ -333,6 +334,8 @@ SYMBOLS = {
     "fyx_add_dynamic_surface": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(fyx_dynamic_layout), C.c_uint32,
                                             C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32)]),
     "fyx_clear_dynamic_surfaces": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
+    "fyx_set_sprites": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "fyx_clear_sprites": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
     "fyx_get_dynamic_batches": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
     "fyx_get_dynamic_batches_device": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),
     "fyx_get_shadow_dynamic_batches": (C.c_int32, [ctx_p, C.c_uint32, C.POINTER(fyx_dynamic_batches)]),

@@ -643,6 +643,24 @@ class Context:
         ix = _u32(nodes)
         self._chk(self._lib.fyx_clear_dynamic_surfaces(self._h, 0 if ix is None else len(ix), _ptr(ix)))
 
+    # fyx_sprite (48 bytes): a Sprite's or dim2::Rectangle's record (scene/sprite.rs:322-405, scene/dim2/rectangle.rs:323-410)
+    SPRITE = np.dtype([("kind", "<u4"), ("batch_key", "<u4"), ("layout_id", "<u4"), ("flip", "<u4"), ("uv_rect", "<f4", 4),
+                       ("size", "<f4"), ("rotation", "<f4"), ("color", "u1", 4), ("reserved", "<u4")])
+
+    def set_sprites(self, nodes, records):
+        """Make `nodes` quad nodes with `records` (SPRITE, one per node), or update their records: kind SPRITE_3D or
+        SPRITE_RECTANGLE, flip bit 0 flip_x and bit 1 flip_y.  The packs then batch each as push_triangles does."""
+        rec = np.ascontiguousarray(records, dtype=self.SPRITE).reshape(-1)
+        ix = _u32(nodes)
+        if ix is None or len(ix) != len(rec):
+            raise ValueError("one record per node")
+        self._chk(self._lib.fyx_set_sprites(self._h, len(rec), _ptr(ix), rec.ctypes.data_as(C.c_void_p)))
+
+    def clear_sprites(self, nodes=None):
+        """Make `nodes` (None = every node) ordinary nodes again."""
+        ix = _u32(nodes)
+        self._chk(self._lib.fyx_clear_sprites(self._h, 0 if ix is None else len(ix), _ptr(ix)))
+
     DYNAMIC_BUNDLE = np.dtype([("batch_key", "<u4"), ("layout_id", "<u4"), ("first", "<u4"), ("count", "<u4"), ("sort_index", "<u8")])
     DYNAMIC_INSTANCE = np.dtype([("node", "<u4"), ("triangle_offset", "<u4"), ("triangle_count", "<u4"), ("reserved", "<u4")])
 

@@ -11,6 +11,7 @@
 #include <memory>
 #include <new>
 #include <string>
+#include <unordered_map>
 #include <unordered_set>
 #include <utility>
 #include <vector>
@@ -274,10 +275,11 @@ struct PackScratch {
     PinnedBuf h_dyn_counts;
 };
 
-// Dynamic batching: one registered surface (fyx_add_dynamic_surface)
+// Dynamic batching: one registered surface (fyx_add_dynamic_surface), or, in dyn_flush, a quad node (ordinal FYX_NONE)
 struct DynReg {
     uint32_t id, node, ordinal, batch_key, layout, n_verts, n_tris, tri_src;
     uint64_t vtx_src;
+    uint32_t kind = kDynMesh;
 };
 
 } // namespace
@@ -311,7 +313,7 @@ struct fyx_ctx {
     // rarely changed rest of its Transform
     SlotColumn trs{fyx_trs{{0, 0, 0}, {0, 0, 0, 1}, {1, 1, 1}}};
     SlotColumn statics{fyx_transform_statics{{0, 0, 0, 1}, {1, 0, 0, 0, 1, 0, 0, 0, 1}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}}};
-    std::array<SlotColumn *, 7> slot_columns() { return {&L[0], &L[1], &L[2], &trs, &statics, &bundle, &lod_range}; }
+    std::array<SlotColumn *, 8> slot_columns() { return {&L[0], &L[1], &L[2], &trs, &statics, &bundle, &lod_range, &quads}; }
 
     // error word written by kernels
     DevBuf d_err;
@@ -463,6 +465,13 @@ struct fyx_ctx {
     bool dyn_dirty = false;
     uint32_t dyn_nodes = 0, dyn_items = 0, dyn_n_layouts = 0;
     DevBuf b_dyn_of_slot, b_dyn_item_first, b_dyn_ordinal, b_dyn_items, b_dyn_layouts;
+    uint32_t dyn_quad_items = 0; // of dyn_items
+    // quad nodes (fyx_set_sprites): kind, batch key and layout id by node index (kind 0 = not a quad node); the full records
+    // by slot, which the quad kernel reads
+    std::vector<uint3> quad_of_node;
+    std::vector<uint32_t> quad_seen; // by node index: the fyx_set_sprites call that last listed it (duplicate check)
+    uint32_t quad_call = 0;
+    SlotColumn quads{fyx_sprite{}};
 
     // multi-GPU (fyx_comm.cu)
     void *comm = nullptr;
@@ -916,7 +925,8 @@ extern "C" void fyx_frustum_default(fyx_frustum *out)
 
 extern "C" void fyx_mat4_mul(const float a[16], const float b[16], float out[16]) { mat4_mul(a, b, out); }
 
-// Drops the dynamic registrations `gone` selects; the pairs, batch keys and layouts in use are those of the rest
+// Drops the dynamic registrations `gone` selects; the pairs, batch keys and layouts in use are those of the rest and of the
+// quad nodes
 template <class Pred> void dyn_drop(fyx_ctx *c, Pred gone)
 {
     c->dyn_regs.erase(std::remove_if(c->dyn_regs.begin(), c->dyn_regs.end(), gone), c->dyn_regs.end());
@@ -926,6 +936,8 @@ template <class Pred> void dyn_drop(fyx_ctx *c, Pred gone)
         c->dyn_pairs.insert((uint64_t)r.node << 32 | r.ordinal);
         key_used[r.batch_key] = layout_used[r.layout] = 1;
     }
+    for (const uint3 &q : c->quad_of_node)
+        if (q.x) key_used[q.y] = layout_used[q.z] = 1;
     for (size_t k = 0; k < key_used.size(); ++k)
         if (!key_used[k]) c->dyn_key_layout[k] = FYX_NONE;
     for (size_t l = 0; l < layout_used.size(); ++l)
@@ -1196,7 +1208,10 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     for (size_t i = 0; i < c->probe_src.size(); ++i)
         if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->probe_src[i].present = 0u;
     c->obs_table_dirty = true;
-    // dynamic registrations too
+    // dynamic registrations and quad nodes too
+    if (c->quad_of_node.size() > capacity) c->quad_of_node.resize(capacity);
+    for (size_t i = 0; i < c->quad_of_node.size(); ++i)
+        if (c->slot_of_node[i] == FYX_NONE) c->quad_of_node[i].x = 0u;
     dyn_drop(c, [&](const DynReg &r) { return r.node >= capacity || c->slot_of_node[r.node] == FYX_NONE; });
     c->ms_dirty = c->have_ms;  // the per-slot surface table too (the CSR itself is by node)
     if (c->ms_of_node.size() < capacity) c->ms_of_node.resize(capacity, make_uint2(0u, 0u));

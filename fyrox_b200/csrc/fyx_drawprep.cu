@@ -46,7 +46,7 @@ __device__ __forceinline__ bool dyn_surface(const InstParams &ip, const uint32_t
 {
     if (d == FYX_NONE) return false;
     for (uint32_t j = ip.dyn_item_first[d]; j < ip.dyn_item_first[d + 1]; ++j)
-        if (ip.dyn_ordinal[j] == k) return true;
+        if (ip.dyn_ordinal[j] == k || ip.dyn_ordinal[j] == FYX_NONE) return true;
     return false;
 }
 
@@ -411,12 +411,20 @@ __device__ __forceinline__ uint32_t dyn_segment(const DynParams &dp, const uint3
 }
 
 // mark: the segment's dynamic nodes as bits (dense index = push order), its items, vertices and triangles per layout; the
-// counts are summed over the warp's lanes that hit the same (segment, layout) before one atomic per counter
-__global__ void __launch_bounds__(kBlock) k_dyn_mark(const DynParams dp)
+// counts are summed over the warp's lanes that hit the same (segment, layout) before one atomic per counter.  A quad node
+// pushes nothing in a shadow pass, and a sprite nothing without cast_shadows (sprite.rs:327-329, rectangle.rs:328-330).
+__global__ void __launch_bounds__(kBlock) k_dyn_mark(const NodeArrays a, const DynParams dp)
 {
     const uint32_t i = blockIdx.x * kBlock + threadIdx.x;
     uint32_t d = FYX_NONE, seg = 0u, j0 = 0u, nj = 0u;
-    if (i < dp.n) d = dp.dyn_of_slot[dp.vis_slot[i]];
+    if (i < dp.n) {
+        const uint32_t slot = dp.vis_slot[i];
+        d = dp.dyn_of_slot[slot];
+        if (d != FYX_NONE) {
+            const uint32_t kind = dp.items[dp.item_first[d]].kind;
+            if (kind != kDynMesh && (dp.shadow || (kind == FYX_SPRITE_3D && !(a.flags[slot] & FYX_NODE_CAST_SHADOWS)))) d = FYX_NONE;
+        }
+    }
     if (d != FYX_NONE) {
         seg = dyn_segment(dp, i);
         atomicOr(dp.bitmap + (size_t)seg * dp.words + (d >> 5), 1u << (d & 31u));
@@ -661,21 +669,29 @@ __device__ __forceinline__ void dyn_transform(const float4 &r0, const float4 &r1
     }
 }
 
-// geometry, one warp per item: the vertex records copied (u32-wide when the stride allows), then the three attributes
-// transformed by the node's world matrix; the triangles shifted by the item's first vertex in its stream
-__global__ void __launch_bounds__(kBlock) k_dyn_geometry(const NodeArrays a, const DynParams dp, const uint32_t n_items)
+// the segment of placed item q: the last whose first item is <= q
+__device__ __forceinline__ uint32_t dyn_item_segment(const DynParams &dp, const uint32_t q)
 {
-    const uint32_t q = (blockIdx.x * kBlock + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
-    if (q >= n_items) return;
-    uint32_t lo = 0u, hi = dp.n_seg - 1u; // the item's segment
+    uint32_t lo = 0u, hi = dp.n_seg - 1u;
     while (lo < hi) {
         const uint32_t mid = (lo + hi + 1u) >> 1;
         if (dp.seg_item0[mid] <= q) lo = mid;
         else hi = mid - 1u;
     }
+    return lo;
+}
+
+// geometry, one warp per registered surface: the vertex records copied (u32-wide when the stride allows), then the three
+// attributes transformed by the node's world matrix; the triangles shifted by the item's first vertex in its stream.  Quad
+// items are k_dyn_quads'.
+__global__ void __launch_bounds__(kBlock) k_dyn_geometry(const NodeArrays a, const DynParams dp, const uint32_t n_items)
+{
+    const uint32_t q = (blockIdx.x * kBlock + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    if (q >= n_items) return;
     const DynItemDev it = dp.items[dp.ord_item[q]];
+    if (it.kind != kDynMesh) return;
     const DynLayoutDev ly = dp.layouts[it.layout];
-    const size_t sl = (size_t)lo * dp.n_layouts + it.layout;
+    const size_t sl = (size_t)dyn_item_segment(dp, q) * dp.n_layouts + it.layout;
     const uint32_t v0 = dp.voff[q];
     const unsigned char *src = dp.vtx + it.vtx_src;
     unsigned char *dst = dp.o_vtx + dp.stream_vtx[sl] + (size_t)v0 * ly.stride;
@@ -707,6 +723,86 @@ __global__ void __launch_bounds__(kBlock) k_dyn_geometry(const NodeArrays a, con
             dyn_st(d + off[k] + 8, o[2]);
         }
     }
+}
+
+// One vertex of a quad as words: SpriteVertex (10 words) or RectangleVertex (6 words), corner (sx, sy) = (+-0.5, +-0.5)
+template <bool kSprite>
+__device__ __forceinline__ void quad_vertex(const fyx_sprite &r, const float4 &r0, const float4 &r1, const float4 &r2, const float sx,
+                                            const float sy, const float u, const float v, uint32_t *w)
+{
+    float p[3];
+    if constexpr (kSprite) {
+        p[0] = r0.w; // global_position(): the translation column, unchanged
+        p[1] = r1.w;
+        p[2] = r2.w;
+    } else {
+        const float c[3] = {sx, sy, 0.0f};
+        dyn_transform(r0, r1, r2, c, true, p);
+    }
+    w[0] = __float_as_uint(p[0]);
+    w[1] = __float_as_uint(p[1]);
+    w[2] = __float_as_uint(p[2]);
+    w[3] = __float_as_uint(u);
+    w[4] = __float_as_uint(v);
+    uint32_t k = 5;
+    if constexpr (kSprite) {
+        w[5] = __float_as_uint(r.size);
+        w[6] = __float_as_uint(r.rotation);
+        w[7] = __float_as_uint(sx);
+        w[8] = __float_as_uint(sy);
+        k = 9;
+    }
+    w[k] = (uint32_t)r.color[0] | ((uint32_t)r.color[1] << 8) | ((uint32_t)r.color[2] << 16) | ((uint32_t)r.color[3] << 24);
+}
+
+// The four vertices and two triangles of quad item q (scene/sprite.rs:331-379, scene/dim2/rectangle.rs:332-384).  The stream
+// base is 16-byte aligned and both strides are multiples of 8: the vertices go out as 16-byte stores when the item's first
+// vertex is even, else as 8-byte stores.
+template <bool kSprite>
+__device__ __forceinline__ void quad_write(const NodeArrays &a, const DynParams &dp, const DynItemDev &it, const uint32_t q)
+{
+    constexpr uint32_t kWords = kSprite ? 10u : 6u; // per vertex
+    const fyx_sprite r = dp.quads[it.slot];
+    const float4 r0 = a.G[0][it.slot], r1 = a.G[1][it.slot], r2 = a.G[2][it.slot];
+    const float lx = r.uv_rect[0], rx = FYX_ADD(r.uv_rect[0], r.uv_rect[2]);
+    const float ty = r.uv_rect[1], by = FYX_ADD(r.uv_rect[1], r.uv_rect[3]);
+    const bool fx = r.flip & 1u, fy = r.flip & 2u;
+    // corner k's tex_coord x is flip_x ? a : b with (a, b) = (lx, rx) for corners 0 and 3 of a sprite, 1 and 2 of a rectangle
+    const float ua = fx ? lx : rx, ub = fx ? rx : lx;
+    const float u[4] = {kSprite ? ua : ub, kSprite ? ub : ua, kSprite ? ub : ua, kSprite ? ua : ub};
+    const float vt = fy ? by : ty, vb = fy ? ty : by;
+    uint32_t w[4 * kWords];
+    quad_vertex<kSprite>(r, r0, r1, r2, 0.5f, 0.5f, u[0], vt, w);
+    quad_vertex<kSprite>(r, r0, r1, r2, -0.5f, 0.5f, u[1], vt, w + kWords);
+    quad_vertex<kSprite>(r, r0, r1, r2, -0.5f, -0.5f, u[2], vb, w + 2 * kWords);
+    quad_vertex<kSprite>(r, r0, r1, r2, 0.5f, -0.5f, u[3], vb, w + 3 * kWords);
+    const size_t sl = (size_t)dyn_item_segment(dp, q) * dp.n_layouts + it.layout;
+    const uint32_t v0 = dp.voff[q];
+    unsigned char *dst = dp.o_vtx + dp.stream_vtx[sl] + (size_t)v0 * (kWords * 4u);
+    if ((v0 & 1u) == 0u) {
+#pragma unroll
+        for (uint32_t k = 0; k < kWords; ++k) reinterpret_cast<uint4 *>(dst)[k] = make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]);
+    } else {
+#pragma unroll
+        for (uint32_t k = 0; k < 2 * kWords; ++k) reinterpret_cast<uint2 *>(dst)[k] = make_uint2(w[2 * k], w[2 * k + 1]);
+    }
+    uint32_t *td = dp.o_tri + ((size_t)dp.stream_tri[sl] + dp.toff[q]) * 3u;
+    td[0] = v0;
+    td[1] = v0 + 1u;
+    td[2] = v0 + 2u;
+    td[3] = v0;
+    td[4] = v0 + 2u;
+    td[5] = v0 + 3u;
+}
+
+// quads, one thread per item; registered surfaces are k_dyn_geometry's
+__global__ void __launch_bounds__(kBlock) k_dyn_quads(const NodeArrays a, const DynParams dp, const uint32_t n_items)
+{
+    const uint32_t q = blockIdx.x * kBlock + threadIdx.x;
+    if (q >= n_items) return;
+    const DynItemDev it = dp.items[dp.ord_item[q]];
+    if (it.kind == FYX_SPRITE_3D) quad_write<true>(a, dp, it, q);
+    else if (it.kind == FYX_SPRITE_RECTANGLE) quad_write<false>(a, dp, it, q);
 }
 
 } // namespace
@@ -798,16 +894,18 @@ void launch_inst_scatter(cudaStream_t s, const NodeArrays &a, const InstParams &
     else k_inst_scatter<<<grid, kBlock, 0, s>>>(a, ip);
 }
 
-void launch_dyn_mark(cudaStream_t s, const DynParams &dp)
+void launch_dyn_mark(cudaStream_t s, const NodeArrays &a, const DynParams &dp)
 {
-    if (dp.n && dp.n_seg) k_dyn_mark<<<(dp.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(dp);
+    if (dp.n && dp.n_seg) k_dyn_mark<<<(dp.n + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, dp);
 }
 
-void launch_dyn_batches(cudaStream_t s, const NodeArrays &a, const DynParams &dp, uint32_t n_items)
+int launch_dyn_batches(cudaStream_t s, const NodeArrays &a, const DynParams &dp, uint32_t n_items, bool meshes, bool quads)
 {
-    if (!n_items) return;
+    if (!n_items) return 0;
     k_dyn_order<<<dp.n_seg, kBinThreads, 0, s>>>(a, dp);
-    k_dyn_geometry<<<(unsigned)(((uint64_t)n_items * 32u + kBlock - 1) / kBlock), kBlock, 0, s>>>(a, dp, n_items);
+    if (meshes) k_dyn_geometry<<<(unsigned)(((uint64_t)n_items * 32u + kBlock - 1) / kBlock), kBlock, 0, s>>>(a, dp, n_items);
+    if (quads) k_dyn_quads<<<(n_items + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, dp, n_items);
+    return 1 + (meshes ? 1 : 0) + (quads ? 1 : 0);
 }
 
 } // namespace fyx

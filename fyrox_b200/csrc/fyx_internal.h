@@ -193,17 +193,19 @@ struct InstParams {
     uint2 *tile_sum;                // [tiles] (instances, bundles) per tile of kScanTile bins, then their exclusive prefix
     // ---- Dynamic batching (fyx_add_dynamic_surface): surfaces batched by the pack's dynamic pass are not instances.
     // dyn_of_slot nullptr = none registered; else the node's dense dynamic index (FYX_NONE = none), whose registered
-    // surface ordinals are dyn_ordinal[dyn_item_first[d] .. dyn_item_first[d + 1])
+    // surface ordinals are dyn_ordinal[dyn_item_first[d] .. dyn_item_first[d + 1]); ordinal FYX_NONE = every surface (a quad node)
     const uint32_t *dyn_of_slot, *dyn_item_first, *dyn_ordinal;
 };
 
-// Dynamic batching (scene/mesh/mod.rs:739-753, 804-833; renderer/bundle.rs:1177-1243).  The registered surfaces, in the
-// reference's push order: dynamic nodes ordered by DFS rank (else node index), each node's surfaces by ordinal.
+// Dynamic batching (scene/mesh/mod.rs:739-753, 804-833; renderer/bundle.rs:1177-1243).  The registered surfaces and the quad
+// nodes (fyx_set_sprites: one item of 4 vertices and 2 triangles each), in the reference's push order: dynamic nodes ordered by
+// DFS rank (else node index), each node's surfaces by ordinal.
+constexpr uint32_t kDynMesh = 0u; // DynItemDev::kind of a registered surface; else FYX_SPRITE_3D / FYX_SPRITE_RECTANGLE
 struct DynItemDev {
     uint32_t node, slot, batch_key, layout;
     uint32_t n_verts, n_tris;
     uint32_t tri_src;   // first u32 of its triangles in the registration pool
-    uint32_t reserved;
+    uint32_t kind;
     uint64_t vtx_src;   // first byte of its vertices in the registration pool (16-byte aligned)
 };
 struct DynLayoutDev {
@@ -219,6 +221,9 @@ struct DynParams {
     uint32_t n_layouts, words; // words: bitmap u32 per segment (ceil(D / 32))
     const unsigned char *vtx;
     const uint32_t *tri;
+    const fyx_sprite *quads;   // [slots] the quad nodes' records (fyx_set_sprites)
+    uint32_t shadow;           // the pack's segments are shadow passes; one flag serves them all because every caller of
+                               // pack_segments packs passes of one kind (see there)
     // the pack's list, cut into segments
     uint32_t n, n_seg;
     const uint32_t *vis_slot;
@@ -245,8 +250,9 @@ struct DynParams {
     unsigned char *o_vtx;
     uint32_t *o_tri;
 };
-void launch_dyn_mark(cudaStream_t s, const DynParams &dp);
-void launch_dyn_batches(cudaStream_t s, const NodeArrays &a, const DynParams &dp, uint32_t n_items);
+void launch_dyn_mark(cudaStream_t s, const NodeArrays &a, const DynParams &dp);
+// order, then geometry when `meshes` (the tables hold registered surfaces) and the quad kernel when `quads`; returns the launches
+int launch_dyn_batches(cudaStream_t s, const NodeArrays &a, const DynParams &dp, uint32_t n_items, bool meshes, bool quads);
 // keys + scan (o_totals), then the scatter.  One segment: the one-CTA scan; segmented (the shadow maps of one group): the
 // device-wide scan of the bins
 constexpr uint32_t kScanTile = 4096; // bins per CTA of the device-wide scan

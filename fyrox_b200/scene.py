@@ -207,6 +207,12 @@ def dynamic_layout(attributes) -> tuple:
     return (off, got["position"], got["normal"], got["tangent"])
 
 
+# SpriteVertex (scene/sprite.rs) and RectangleVertex (scene/dim2/rectangle.rs): the layouts their push_triangles names
+SPRITE_VERTEX_ATTRIBUTES = [("position", 12), ("tex_coord0", 8), ("params", 16), ("color", 4)]
+RECTANGLE_VERTEX_ATTRIBUTES = [("position", 12), ("tex_coord0", 8), ("color", 4)]
+QUAD_KINDS = {"sprite": L.SPRITE_3D, "rectangle": L.SPRITE_RECTANGLE}
+
+
 @dataclass
 class Surface:
     """Surface (scene/mesh/surface.rs:1249-1271): bone handles + the VertexBuffer bytes (+ SurfaceData::blend_shapes_container)."""
@@ -248,6 +254,14 @@ class Node:
         self.surfaces: List[Surface] = []
         self.batching_mode = BatchingMode.NONE  # Mesh::batching_mode (scene/mesh/mod.rs:372)
         self.render_path = 0                    # Mesh::render_path: 0 Deferred, 1 Forward
+        # Sprite (scene/sprite.rs) and dim2::Rectangle (scene/dim2/rectangle.rs) fields; size and rotation are the sprite's
+        self.uv_rect = np.array([0, 0, 1, 1], f32)  # position.x, position.y, size.x, size.y
+        self.color = (255, 255, 255, 255)
+        self.size = f32(0.2)
+        self.rotation = f32(0.0)
+        self.flip_x = False
+        self.flip_y = False
+        self.material = 0  # the host's key of the material
         self._graph: Optional["Graph"] = None
         self._handle = Handle.NONE
 
@@ -273,6 +287,33 @@ class Node:
         """Mesh::set_batching_mode (scene/mesh/mod.rs:612-617); Static => RdcControlFlow::Break when the mesh is rendered."""
         self.batching_mode = mode
         self._notify("flags")
+
+    # Sprite / Rectangle setters (scene/sprite.rs, scene/dim2/rectangle.rs)
+    def _set_quad(self, name, v):
+        setattr(self, name, v)
+        self._notify("sprite")
+        return self
+
+    def set_uv_rect(self, r):
+        return self._set_quad("uv_rect", np.asarray(r, f32).reshape(4))
+
+    def set_color(self, c):
+        return self._set_quad("color", tuple(int(x) for x in c))
+
+    def set_size(self, v):
+        return self._set_quad("size", f32(v))
+
+    def set_rotation(self, v):
+        return self._set_quad("rotation", f32(v))
+
+    def set_flip_x(self, v):
+        return self._set_quad("flip_x", bool(v))
+
+    def set_flip_y(self, v):
+        return self._set_quad("flip_y", bool(v))
+
+    def set_material(self, m: int):
+        return self._set_quad("material", int(m))
 
     # tracked properties
     def local_transform(self) -> Transform:
@@ -344,7 +385,7 @@ class Node:
         f |= L.NODE_ENABLED if self._enabled else 0
         f |= L.NODE_FRUSTUM_CULLING if self.frustum_culling else 0
         f |= L.NODE_CAST_SHADOWS if self.cast_shadows else 0
-        f |= L.NODE_RENDERABLE if self.kind == "mesh" else 0
+        f |= L.NODE_RENDERABLE if self.kind in ("mesh", "sprite", "rectangle") else 0
         f |= L.NODE_STATIC_BATCH if (self.kind == "mesh" and self.batching_mode == BatchingMode.STATIC) else 0
         return f
 
@@ -421,6 +462,26 @@ def MeshBuilder(base: BaseBuilder = None) -> BaseBuilder:
     return b
 
 
+def _quad_builder(kind: str, base: BaseBuilder = None) -> BaseBuilder:
+    b = base or BaseBuilder()
+    b._n.kind = kind
+    for name, conv in (("uv_rect", lambda r: np.asarray(r, f32).reshape(4)), ("color", lambda c: tuple(int(x) for x in c)),
+                       ("size", f32), ("rotation", f32), ("flip_x", bool), ("flip_y", bool), ("material", int)):
+        setattr(b, "with_" + name, (lambda nm, cv: lambda v: (setattr(b._n, nm, cv(v)), b)[1])(name, conv))
+    return b
+
+
+def SpriteBuilder(base: BaseBuilder = None) -> BaseBuilder:
+    """SpriteBuilder (scene/sprite.rs:408-520): a renderable node with the default unit box (Base::local_bounding_box, which
+    the frustum test uses whatever the size)."""
+    return _quad_builder("sprite", base)
+
+
+def RectangleBuilder(base: BaseBuilder = None) -> BaseBuilder:
+    """RectangleBuilder (scene/dim2/rectangle.rs:413-500): a renderable node with the unit box."""
+    return _quad_builder("rectangle", base)
+
+
 class Graph:
     """Graph (scene/graph/mod.rs:130-175): a pool of nodes; hierarchical data lives on the GPU."""
 
@@ -431,13 +492,15 @@ class Graph:
         self._free: List[int] = []
         self.root = Handle.NONE
         self._topology_dirty = True
-        self._dirty: Dict[str, set] = {"transform": set(), "flags": set(), "mask": set(), "aabb": set(), "blend_shapes": set()}
+        self._dirty: Dict[str, set] = {"transform": set(), "flags": set(), "mask": set(), "aabb": set(), "blend_shapes": set(), "sprite": set()}
         self._cache: Dict[str, np.ndarray] = {}
         self._surfaces_uploaded = 0
         # dynamic batching: dense ids of (material, render path) and of layouts, and what each node has registered
         self._batch_keys: Dict[tuple, int] = {}
         self._layout_ids: Dict[tuple, int] = {}
         self._dynamic: Dict[int, tuple] = {}
+        self._quads: Dict[int, int] = {}  # quad nodes set in the context: index -> id(node)
+        self._surfaced: set = set()  # indices given their surfaces through set_node_surfaces (by _register_dynamic)
         self.root = self.add_node(Node("pivot", "__ROOT__"))  # Graph::new, graph/mod.rs:408-424
 
     # ---- pool ----
@@ -532,6 +595,8 @@ class Graph:
             alive = np.nonzero(flags & L.NODE_ALIVE)[0].astype(np.uint32)
             if alive.size:
                 self.ctx.set_local_matrices(local[alive], alive)
+            # quad nodes first: a pool index that stopped being one may now register dynamic surfaces
+            self._sync_quads()
             # surfaces refer to node indices: (re)upload all of them after a topology change
             self._upload_surfaces(reset=True)
             self._topology_dirty = False
@@ -551,6 +616,7 @@ class Graph:
             a = live(self._dirty["aabb"])
             if a:
                 self.ctx.set_local_aabbs(np.stack([self._records[i].local_bounding_box for i in a]), np.array(a, np.uint32))
+            self._sync_quads()
             for s in self._dirty.values():
                 s.clear()
             self._upload_surfaces(reset=False)
@@ -594,6 +660,7 @@ class Graph:
             n, sig = self._records[i], want[i]
             if sig and len(n.surfaces) > 1:
                 self.ctx.set_node_surfaces([i], [[(0, s.surface_id) for s in n.surfaces]])
+                self._surfaced.add(i)
             for k, *_ in sig:
                 s = n.surfaces[k]
                 attrs = tuple(s.attributes())
@@ -606,6 +673,41 @@ class Graph:
                 self._dynamic[i] = sig
             else:
                 self._dynamic.pop(i, None)
+
+    def _sync_quads(self):
+        """Sprite and Rectangle nodes: the records of new quad nodes and of those whose fields changed ("sprite"); a pool index
+        that no longer holds the quad node it was set for is cleared."""
+        gone = [i for i, ident in self._quads.items()
+                if i >= len(self._records) or self._records[i] is None or id(self._records[i]) != ident or self._records[i].kind not in QUAD_KINDS]
+        if gone:
+            self.ctx.clear_sprites(np.array(gone, np.uint32))
+            for i in gone:
+                del self._quads[i]
+        dirty = self._dirty["sprite"]
+        push = [i for i, n in enumerate(self._records) if n is not None and n.kind in QUAD_KINDS and (i in dirty or i not in self._quads)]
+        if not push:
+            return
+        # a pool index reused by a quad node still carries what the removed mesh gave the context (fyx_set_topology keeps it,
+        # the index being alive): its registrations and its surface list go first
+        reused = [i for i in push if i in self._dynamic]
+        if reused:
+            self.ctx.clear_dynamic_surfaces(np.array(reused, np.uint32))
+            for i in reused:
+                del self._dynamic[i]
+        surfaced = [i for i in push if i in self._surfaced]
+        if surfaced:
+            self.ctx.set_node_surfaces(surfaced, [[] for _ in surfaced])
+            self._surfaced.difference_update(surfaced)
+        rec = np.zeros(len(push), Context.SPRITE)
+        for k, i in enumerate(push):
+            n = self._records[i]
+            attrs = tuple(SPRITE_VERTEX_ATTRIBUTES if n.kind == "sprite" else RECTANGLE_VERTEX_ATTRIBUTES)
+            rec[k] = (QUAD_KINDS[n.kind], self._batch_keys.setdefault((n.material, 1), len(self._batch_keys)),
+                      self._layout_ids.setdefault(attrs, len(self._layout_ids)), (1 if n.flip_x else 0) | (2 if n.flip_y else 0),
+                      n.uv_rect, n.size, n.rotation, n.color, 0)
+        self.ctx.set_sprites(np.array(push, np.uint32), rec)
+        for i in push:
+            self._quads[i] = id(self._records[i])
 
     def _upload_blend_shapes(self):
         """SurfaceData::blend_shapes_container -> fyx_set_blend_shapes once, Mesh::blend_shapes weights whenever they were touched."""

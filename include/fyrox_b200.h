@@ -819,6 +819,52 @@ int32_t fyx_get_shadow_dynamic_batches_device(fyx_ctx *ctx, uint32_t map, fyx_dy
 int32_t fyx_get_scene_observer_dynamic_batches(fyx_ctx *ctx, uint32_t observer, fyx_dynamic_batches *out);
 int32_t fyx_get_scene_observer_dynamic_batches_device(fyx_ctx *ctx, uint32_t observer, fyx_dynamic_batches *out);
 
+/* ---- Sprites and 2D rectangles: the other push_triangles callers ------------------------------------------------------
+ * Sprite::collect_render_data (scene/sprite.rs:322-405) and dim2::Rectangle::collect_render_data (scene/dim2/rectangle.rs:
+ * 323-410) push one quad per node, after should_be_rendered, through the same push_triangles as Dynamic meshes: four vertices,
+ * triangles [0,1,2] [0,2,3], render path Forward, sort index calculate_sorting_index(global_position).  A quad node is one more
+ * item of its pass's dynamic batches: it shares bundle_map and last_bundle_id with the Dynamic surfaces of the pass, and its
+ * layout's stream with any Dynamic surface given the same layout_id.  The getters above return the quads; a quad node is
+ * never an ordinary instance (fyx_instances) of any pack, and surfaces fyx_set_node_surfaces later gives it are not packed.
+ *   Gates: a sprite pushes nothing in a shadow pass, nor, in any pass, when its FYX_NODE_CAST_SHADOWS is off (sprite.rs:
+ *   327-329); a rectangle pushes nothing in a shadow pass (rectangle.rs:328-330).  Shadow passes (renderer/mod.rs:128-131):
+ *   every map of fyx_pack_shadow_instances, and a fyx_pack_instances frustum culled with FYX_PASS_SHADOW; never an observer.
+ *   Culling: both are tested with AABB::unit() transformed by the global transform (sprite.rs:314-316 through base.rs:741-750;
+ *   rectangle.rs:310-317), never with the sprite's size: the host keeps each quad node's unit box.
+ *   Vertices (lx = uv_rect[0], rx = uv_rect[0] + uv_rect[2], ty = uv_rect[1], by = uv_rect[1] + uv_rect[3], f32 adds), in the
+ *   corner order (+,+) (-,+) (-,-) (+,-):
+ *     SpriteVertex, 40 bytes: position f32x3 = the global position (the translation column, unchanged) in every vertex,
+ *       tex_coord f32x2, params f32x4 = (size, rotation, +-0.5, +-0.5), color u8x4.  tex_coord x: flip_x ? lx : rx,
+ *       flip_x ? rx : lx, flip_x ? rx : lx, flip_x ? lx : rx.
+ *     RectangleVertex, 24 bytes: position f32x3 = global_transform.transform_point((+-0.5, +-0.5, 0)), tex_coord f32x2, color
+ *       u8x4.  tex_coord x is the sprite's mirrored: flip_x ? rx : lx, flip_x ? lx : rx, flip_x ? lx : rx, flip_x ? rx : lx.
+ *     tex_coord y of both: flip_y ? by : ty for vertices 0 and 1, flip_y ? ty : by for vertices 2 and 3.
+ *   The layout of a kind, in fyx_dynamic_layout terms: {40, 0, FYX_NONE, FYX_NONE} for sprites, {24, 0, FYX_NONE, FYX_NONE}
+ *   for rectangles.  Layout ids and batch keys are shared with fyx_add_dynamic_surface: an id or key is free again only when
+ *   neither a registration nor a quad node uses it. */
+#define FYX_SPRITE_3D        1u /* scene::sprite::Sprite */
+#define FYX_SPRITE_RECTANGLE 2u /* scene::dim2::rectangle::Rectangle */
+typedef struct fyx_sprite {
+    uint32_t kind;        /* FYX_SPRITE_3D | FYX_SPRITE_RECTANGLE */
+    uint32_t batch_key;   /* < 2^24, the host's id for (material, Forward) */
+    uint32_t layout_id;   /* < 2^16, the host's id for the kind's vertex layout */
+    uint32_t flip;        /* bit 0 flip_x, bit 1 flip_y */
+    float uv_rect[4];     /* position.x, position.y, size.x, size.y */
+    float size, rotation; /* sprite only */
+    uint8_t color[4];     /* r, g, b, a */
+    uint32_t reserved;
+} fyx_sprite;             /* 48 bytes */
+/* Make nodes idx[0..count) (idx NULL = nodes 0..count-1) quad nodes with records[k], or update their records.  A change of
+ * uv_rect, color, size, rotation or flip only rewrites the records; a new quad node, or a change of kind, batch_key or
+ * layout_id, rebuilds the push-order tables at the next pack.  FYX_ERR_INVALID_ARGUMENT, with nothing changed, for: an
+ * unknown kind; a node out of range, not alive or listed twice; a node with fyx_add_dynamic_surface registrations, with
+ * surfaces from fyx_set_node_surfaces or with a skinned surface; a batch_key >= 2^24 or layout_id >= 2^16; a layout_id in use
+ * with another layout; a batch_key in use with another layout_id.  Records stay with their node index across
+ * fyx_set_topology; a node it removes drops its record.  fyx_add_dynamic_surface refuses a quad node. */
+int32_t fyx_set_sprites(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const fyx_sprite *records);
+/* Make the listed nodes (nodes NULL = every node) ordinary nodes again. */
+int32_t fyx_clear_sprites(fyx_ctx *ctx, uint32_t count, const uint32_t *nodes);
+
 /* ---- multi-GPU: one context per GPU, one process per GPU ------------------------------------- */
 /* The node array is sharded (sub-trees + replicated ancestors, SURVEY §8e); each context culls its
  * shard; the per-frustum visible lists are all-gathered with NCCL over NVLink so every rank holds
