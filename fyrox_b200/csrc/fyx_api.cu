@@ -10,6 +10,7 @@
 #include <cstring>
 #include <memory>
 #include <new>
+#include <set>
 #include <string>
 #include <unordered_map>
 #include <unordered_set>
@@ -275,11 +276,52 @@ struct PackScratch {
     PinnedBuf h_dyn_counts;
 };
 
-// Dynamic batching: one registered surface (fyx_add_dynamic_surface), or, in dyn_flush, a quad node (ordinal FYX_NONE)
+// Dynamic batching: one registered surface (fyx_add_dynamic_surface)
 struct DynReg {
     uint32_t id, node, ordinal, batch_key, layout, n_verts, n_tris, tri_src;
     uint64_t vtx_src;
-    uint32_t kind = kDynMesh;
+};
+
+// Dynamic batching (fyx_drawprep.inl): what push_triangles batches, the registered surfaces of Dynamic meshes and the quad
+// nodes (fyx_set_sprites), with the layout ids and batch keys they share, the pools, and the device tables in push order
+// (DynItemDev).  The tables are rebuilt by the first pack after invalidate(), which every input of the flush calls: the
+// registrations, the quad nodes, the topology, the DFS order and the node surfaces.
+struct DynBatches {
+    enum Use { kNeither, kRegistrations, kQuad }; // what a node holds
+    // this call's claims of layout ids (with their layouts) and batch keys (with their layout ids), not yet committed
+    struct Claims {
+        std::unordered_map<uint32_t, fyx_dynamic_layout> layout;
+        std::unordered_map<uint32_t, uint32_t> key;
+    };
+    std::vector<DynReg> regs;
+    std::set<uint64_t> pairs; // node << 32 | ordinal of every registration
+    uint32_t next_id = 0;
+    // quad nodes: kind, batch key and layout id by node index (kind 0 = not a quad node); the full records by slot, which the
+    // quad kernel reads
+    std::vector<uint3> quad_of_node;
+    std::vector<uint32_t> quad_seen; // by node index: the fyx_set_sprites call that last listed it (duplicate check)
+    uint32_t quad_call = 0;
+    SlotColumn quads{fyx_sprite{}};
+    std::vector<fyx_dynamic_layout> layouts; // by layout id; stride FYX_NONE = nothing uses it
+    std::vector<uint32_t> key_layout;        // by batch key; FYX_NONE = nothing uses it
+    DevBuf b_vtx, b_tri;                     // pools: vertex bytes (each surface 16-byte aligned), triangles
+    uint64_t vtx_used = 0, tri_used = 0;
+    bool stale = false;
+    uint32_t n_nodes = 0, n_items = 0, n_quads = 0, n_layouts = 0; // of the device tables
+    DevBuf b_of_slot, b_item_first, b_ordinal, b_items, b_layouts;
+
+    void invalidate() { stale = true; }
+    Use use_of(uint32_t node) const;
+    // a claim of `layout_id` for `ly` and of `batch_key` for `layout_id`: refused when the committed tables or `staged` give
+    // either to another, else added to `staged`
+    int32_t check_claim(fyx_ctx *c, uint32_t layout_id, const fyx_dynamic_layout &ly, uint32_t batch_key, Claims &staged) const;
+    void commit(const Claims &staged);
+    void release(); // after registrations or quad nodes went: their pairs, and the layout ids and batch keys nothing uses, go
+    void topology_changed(const fyx_ctx *c); // a node that is not alive any more drops its registrations and quad
+    int32_t compact(fyx_ctx *c);
+    int32_t flush(fyx_ctx *c);
+    int32_t pack(fyx_ctx *c, InstPack &o, const uint32_t *vis_slot, const float *views, const float *view, const std::vector<uint32_t> &first,
+                 bool shadow);
 };
 
 } // namespace
@@ -313,7 +355,7 @@ struct fyx_ctx {
     // rarely changed rest of its Transform
     SlotColumn trs{fyx_trs{{0, 0, 0}, {0, 0, 0, 1}, {1, 1, 1}}};
     SlotColumn statics{fyx_transform_statics{{0, 0, 0, 1}, {1, 0, 0, 0, 1, 0, 0, 0, 1}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}}};
-    std::array<SlotColumn *, 8> slot_columns() { return {&L[0], &L[1], &L[2], &trs, &statics, &bundle, &lod_range, &quads}; }
+    std::array<SlotColumn *, 8> slot_columns() { return {&L[0], &L[1], &L[2], &trs, &statics, &bundle, &lod_range, &dyn.quads}; }
 
     // error word written by kernels
     DevBuf d_err;
@@ -453,25 +495,7 @@ struct fyx_ctx {
     PackScratch pack;
     InstPack inst[FYX_MAX_FRUSTA];
 
-    // dynamic batching (fyx_drawprep.inl): the registrations and their pools; layouts and batch keys as first given; the
-    // device tables in push order (DynItemDev, dyn_flush), rebuilt when a registration, the topology or the DFS order changes
-    std::vector<DynReg> dyn_regs;
-    std::unordered_set<uint64_t> dyn_pairs;      // node << 32 | ordinal of every registration
-    uint32_t dyn_next_id = 0;
-    std::vector<fyx_dynamic_layout> dyn_layouts; // by layout id; stride FYX_NONE = no registration uses it
-    std::vector<uint32_t> dyn_key_layout;        // by batch key; FYX_NONE = no registration uses it
-    DevBuf b_dyn_vtx, b_dyn_tri;                 // pools: vertex bytes (each surface 16-byte aligned), triangles
-    uint64_t dyn_vtx_used = 0, dyn_tri_used = 0;
-    bool dyn_dirty = false;
-    uint32_t dyn_nodes = 0, dyn_items = 0, dyn_n_layouts = 0;
-    DevBuf b_dyn_of_slot, b_dyn_item_first, b_dyn_ordinal, b_dyn_items, b_dyn_layouts;
-    uint32_t dyn_quad_items = 0; // of dyn_items
-    // quad nodes (fyx_set_sprites): kind, batch key and layout id by node index (kind 0 = not a quad node); the full records
-    // by slot, which the quad kernel reads
-    std::vector<uint3> quad_of_node;
-    std::vector<uint32_t> quad_seen; // by node index: the fyx_set_sprites call that last listed it (duplicate check)
-    uint32_t quad_call = 0;
-    SlotColumn quads{fyx_sprite{}};
+    DynBatches dyn; // Dynamic meshes and quad nodes
 
     // multi-GPU (fyx_comm.cu)
     void *comm = nullptr;
@@ -925,26 +949,6 @@ extern "C" void fyx_frustum_default(fyx_frustum *out)
 
 extern "C" void fyx_mat4_mul(const float a[16], const float b[16], float out[16]) { mat4_mul(a, b, out); }
 
-// Drops the dynamic registrations `gone` selects; the pairs, batch keys and layouts in use are those of the rest and of the
-// quad nodes
-template <class Pred> void dyn_drop(fyx_ctx *c, Pred gone)
-{
-    c->dyn_regs.erase(std::remove_if(c->dyn_regs.begin(), c->dyn_regs.end(), gone), c->dyn_regs.end());
-    c->dyn_pairs.clear();
-    std::vector<uint8_t> key_used(c->dyn_key_layout.size(), 0), layout_used(c->dyn_layouts.size(), 0);
-    for (const DynReg &r : c->dyn_regs) {
-        c->dyn_pairs.insert((uint64_t)r.node << 32 | r.ordinal);
-        key_used[r.batch_key] = layout_used[r.layout] = 1;
-    }
-    for (const uint3 &q : c->quad_of_node)
-        if (q.x) key_used[q.y] = layout_used[q.z] = 1;
-    for (size_t k = 0; k < key_used.size(); ++k)
-        if (!key_used[k]) c->dyn_key_layout[k] = FYX_NONE;
-    for (size_t l = 0; l < layout_used.size(); ++l)
-        if (!layout_used[l]) c->dyn_layouts[l].stride = FYX_NONE;
-    c->dyn_dirty = true;
-}
-
 // --------------------------------------------------------------------------------------------
 // scene description
 // --------------------------------------------------------------------------------------------
@@ -1208,11 +1212,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     for (size_t i = 0; i < c->probe_src.size(); ++i)
         if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->probe_src[i].present = 0u;
     c->obs_table_dirty = true;
-    // dynamic registrations and quad nodes too
-    if (c->quad_of_node.size() > capacity) c->quad_of_node.resize(capacity);
-    for (size_t i = 0; i < c->quad_of_node.size(); ++i)
-        if (c->slot_of_node[i] == FYX_NONE) c->quad_of_node[i].x = 0u;
-    dyn_drop(c, [&](const DynReg &r) { return r.node >= capacity || c->slot_of_node[r.node] == FYX_NONE; });
+    c->dyn.topology_changed(c); // dynamic registrations and quad nodes too
     c->ms_dirty = c->have_ms;  // the per-slot surface table too (the CSR itself is by node)
     if (c->ms_of_node.size() < capacity) c->ms_of_node.resize(capacity, make_uint2(0u, 0u));
     c->anim_csr_dirty = true; // animated nodes are addressed by slot
@@ -1229,7 +1229,7 @@ extern "C" int32_t fyx_set_dfs_order(fyx_ctx *c, uint32_t capacity, const uint32
     else c->dfs_rank.clear();
     c->rank_on_device = false;
     c->tables_dirty = true;
-    c->dyn_dirty = true;
+    c->dyn.invalidate();
     return FYX_OK;
 }
 

@@ -101,6 +101,33 @@ def test_two_layouts_give_independent_streams():
     assert out["instances"][["node", "triangle_offset"]].tolist() == [(1, 0), (3, 1), (2, 0)]
 
 
+def test_a_random_pass_batches_or_pushes_every_surface_once():
+    """Nodes of one or two surfaces, some batched under three keys, four sort indices, moved worlds: the stream is the batched
+    surfaces' transformed vertices in push order with their triangles shifted, the rest are pushed, the bundles follow the first
+    pushes and their instances cover every triangle."""
+    rng = np.random.default_rng(3)
+    dyn = {}
+    for n in range(1, 40):
+        for k in range(int(rng.integers(1, 3))):
+            if rng.random() < 0.6:
+                v = rng.standard_normal((int(rng.integers(3, 12)), 12)).astype(f32)
+                dyn[(n, k)] = dbo.DynSurface(int(rng.integers(0, 3)), 0, LAYOUT, v.tobytes(), rng.integers(0, len(v), (4, 3)).astype(np.uint32))
+    n_surf = {n: 1 + max([k for (m, k) in dyn if m == n], default=0) for n in range(1, 40)}
+    sort = lambda n: n % 4  # noqa: E731
+    world = lambda n: np.array([1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, n * 0.5, -1.0, 2.0, 1], f32)  # noqa: E731
+    out, pushed = run(list(range(1, 40)), dyn, n_surf=lambda n: n_surf[n], sort=sort, world=world)
+    order = [(n, k) for n in range(1, 40) for k in range(n_surf[n])]
+    batched = [p for p in order if p in dyn]
+    assert pushed == [p for p in order if p not in dyn]
+    st = out["streams"][0]
+    assert st["vertices"].tobytes() == b"".join(dbo.transform_vertices(dyn[p].vertices, LAYOUT, world(p[0])) for p in batched)
+    first = np.cumsum([0] + [len(dyn[p].vertices) // LAYOUT[0] for p in batched])
+    assert st["triangles"].tolist() == np.concatenate([dyn[p].triangles + np.uint32(f) for p, f in zip(batched, first)]).tolist()
+    keys = list(dict.fromkeys((dyn[p].batch_key, sort(p[0])) for p in batched))
+    assert out["bundles"][["batch_key", "sort_index"]].tolist() == keys
+    assert out["instances"]["triangle_count"].sum() == sum(len(dyn[p].triangles) for p in batched)
+
+
 def test_the_mirrors_layout_rule_looks_only_at_sizes():
     # a 12-byte "position" of any declared type is transformed; a 16-byte normal, a 12-byte tangent or an 8-byte position is not
     assert scene.dynamic_layout([("position", 12), ("normal", 12), ("tangent", 16), ("uv", 8)]) == (48, 0, 12, 24)

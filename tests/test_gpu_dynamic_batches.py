@@ -1,7 +1,8 @@
 """Dynamic batching on the device: each pack's dynamic batches (bundles, instances, transformed vertex streams, shifted
 triangles) against tests/dynamic_batch_oracle.py run over the same pass in DFS order, for a camera frustum (with and without
 fyx_set_dfs_order) and every shadow map; registered surfaces leave the ordinary instances; register-then-clear changes nothing;
-registrations follow their nodes across fyx_set_topology; the device getters equal the host getters."""
+registrations follow their nodes across fyx_set_topology; a registered surface that fyx_set_node_surfaces later removes or
+names skinned is pushed again; the device getters equal the host getters."""
 import numpy as np
 import pytest
 
@@ -16,6 +17,7 @@ pytestmark = pytest.mark.gpu
 
 f32 = np.float32
 NONE = dbo.NONE
+EYE = np.eye(4, dtype=f32).reshape(16)
 LAYOUTS = {0: (48, 0, 12, 24), 1: (15, 3, NONE, NONE)}  # the second has an odd stride: records are not 4-byte aligned
 
 
@@ -56,11 +58,12 @@ def register(ctx, rng, sc, n_meshes=300, n_keys=6, add=True, keep_one=False, exc
     return dyn, n_surf
 
 
-def expect(og, order, dyn, n_surf, view, sort_of=None):
-    """The oracle's pass over `order` (the pass's nodes in push order)."""
-    vp = np.eye(4, dtype=f32).reshape(16)
-    return dbo.dynamic_pass([int(n) for n in order], lambda n: n_surf.get(n, 1), dyn, sort_of or (lambda n: og.instance(n, view, vp)[0]),
-                            lambda n: np.asarray(og.global_transform(n), f32))
+def expect(og, order, dyn, n_surf, view, sort_of=None, quads=None, shadow=False, flags=None):
+    """The oracle's pass over `order` (the pass's nodes in push order); the quad nodes' gates take the pass kind and the nodes'
+    flags."""
+    return dbo.dynamic_pass([int(n) for n in order], lambda n: n_surf.get(n, 1), dyn, sort_of or (lambda n: og.instance(n, view, EYE)[0]),
+                            lambda n: np.asarray(og.global_transform(n), f32), quads, shadow,
+                            lambda n: bool(flags[n] & fb.NODE_CAST_SHADOWS))
 
 
 def push_order(nodes, rank=None):
@@ -92,11 +95,12 @@ def build(ctx, seed, n=3000, lights=12):
     return rng, sc, og, dyn, n_surf
 
 
-def check_frustum(ctx, og, dyn, n_surf, rank=None, view=None):
+def check_frustum(ctx, og, dyn, n_surf, rank=None, view=None, cull=True):
     """The camera frustum's pass; the nodes and their order come from the oracle's own DFS (og.from_graph, pre-order): as it
-    is with fyx_set_dfs_order, by node index without."""
+    is with fyx_set_dfs_order, by node index without.  cull=False packs the last cull's list again."""
     fo, ff = camera_frustum(zfar=150.0)
-    ctx.cull([ff])
+    if cull:
+        ctx.cull([ff])
     if view is None:
         view = np.eye(4, dtype=f32)
         view[:3, 3] = (0.5, -0.25, 2.0)
@@ -203,6 +207,24 @@ def test_registrations_follow_their_nodes_across_topology(ctx):
     ctx.set_local_matrices(sc.local[back], back)
     ctx.update_transforms(fb.UPDATE_ALL)
     check_frustum(ctx, og, kept, n_surf)
+
+
+def test_node_surfaces_changed_after_a_pack(ctx):
+    """Surface 1 registered on two-surface meshes, one pack, then fyx_set_node_surfaces cuts some of the meshes to one surface
+    and names surface 1 of the others skinned: the next pack of the same list (a skinned mesh's box is its bones', which the
+    oracle's graph does not have) batches neither and pushes the skinned ones, as the oracle does."""
+    rng, sc, og, dyn, n_surf = build(ctx, 100)
+    meshes = [m for m, k in n_surf.items() if k == 2 and (m, 1) in dyn]
+    cut, skin = meshes[0::2], meshes[1::2]
+    check_frustum(ctx, og, dyn, n_surf)
+    ctx.set_node_surfaces(cut, [[(int(rng.integers(0, 5)), None)] for _ in cut])
+    sids = [ctx.add_skinned_surface(m, np.array([1], np.uint32), EYE.reshape(1, 16), None, n_verts=0) for m in skin]
+    ctx.set_node_surfaces(skin, [[(int(rng.integers(0, 5)), None), (int(rng.integers(0, 5)), sid)] for sid in sids])
+    n_surf.update({m: 1 for m in cut})
+    kept = {p: s for p, s in dyn.items() if p[1] != 1 or p[0] not in set(meshes)}
+    check_frustum(ctx, og, kept, n_surf, cull=False)
+    vis = set(ctx.get_visible(0).tolist())
+    assert len(vis & set(cut)) > 3 and len(vis & set(skin)) > 3  # the pass meets both kinds of change
 
 
 def test_refusals(ctx):

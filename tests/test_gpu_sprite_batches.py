@@ -1,5 +1,5 @@
 """Sprites and 2D rectangles on the device (fyx_set_sprites): each pack's dynamic batches, quads and Dynamic meshes together,
-against tests/sprite_batch_oracle.py run over the same pass in DFS order, byte for byte; the gates by pass kind; quad nodes are
+against tests/dynamic_batch_oracle.py run over the same pass in DFS order, byte for byte; the gates by pass kind; quad nodes are
 never ordinary instances; records follow their nodes; set-then-clear launches and returns what a context that never set
 quads does; the refusals leave the state as it was; the scene mirror end to end."""
 import ctypes as C
@@ -12,7 +12,7 @@ import sprite_batch_oracle as sbo
 import fyrox_b200 as fb
 from fyrox_b200.context import Context
 from helpers import camera_frustum, preorder_rank
-from test_gpu_dynamic_batches import assert_same, canonical, push_order, register
+from test_gpu_dynamic_batches import EYE, assert_same, canonical, expect, push_order, register
 from test_gpu_instance_pack import launches
 from test_gpu_shadow_casters import ShadowScene, in_view
 from test_gpu_shadow_instances import shadow_cull
@@ -21,7 +21,6 @@ pytestmark = pytest.mark.gpu
 
 f32 = np.float32
 NONE = dbo.NONE
-EYE = np.eye(4, dtype=f32).reshape(16)
 SPRITE_L, RECT_L = 2, 3  # layout ids; register() uses 0 and 1 with batch keys 0..5
 SPRITE_LAYOUT = (40, 0, NONE, NONE)
 RECT_LAYOUT = (24, 0, NONE, NONE)
@@ -76,12 +75,6 @@ def build(ctx, seed, n=3000, lights=12, p_cast=0.8, p=0.5):
     return rng, sc, og, dyn, n_surf, quads
 
 
-def expect(og, sc, order, dyn, n_surf, quads, view, shadow, sort_of=None):
-    return sbo.mixed_pass([int(n) for n in order], lambda n: n_surf.get(n, 1), dyn, quads,
-                          sort_of or (lambda n: og.instance(n, view, EYE)[0]), lambda n: np.asarray(og.global_transform(n), f32),
-                          shadow, lambda n: bool(sc.flags[n] & fb.NODE_CAST_SHADOWS))
-
-
 def no_quad_instances(inst, quads):
     assert not set(inst["node"].tolist()) & set(quads)
 
@@ -96,7 +89,7 @@ def check_frustum(ctx, og, sc, dyn, n_surf, quads, rank=None, view=None, shadow=
     inst = ctx.pack_instances(0, view, EYE)
     dfs = [int(n) for n in og.from_graph(fo, shadow_pass=shadow)]
     assert sorted(dfs) == sorted(ctx.get_visible(0).tolist())  # the quad nodes are in the visible list
-    want, pushed = expect(og, sc, dfs if rank is not None else sorted(dfs), dyn, n_surf, quads, view, shadow)
+    want, pushed = expect(og, dfs if rank is not None else sorted(dfs), dyn, n_surf, view, quads=quads, shadow=shadow, flags=sc.flags)
     got = ctx.dynamic_batches("frustum", 0)
     assert_same(got, want, "frustum")
     assert_same(ctx.dynamic_batches("frustum", 0, device=True), want, "frustum device")
@@ -133,7 +126,7 @@ def test_every_shadow_map_carries_no_quads(ctx):
     for k, (m, w) in enumerate(zip(maps, want_maps)):
         nodes = w[4]
         seen += len(set(nodes.tolist()) & set(quads))
-        want, pushed = expect(og, sc, push_order(nodes), dyn, n_surf, quads, w[5], True)
+        want, pushed = expect(og, push_order(nodes), dyn, n_surf, w[5], quads=quads, shadow=True, flags=sc.flags)
         assert_same(ctx.dynamic_batches("shadow", k), want, ("map", k))
         assert_same(ctx.dynamic_batches("shadow", k, device=True), want, ("map device", k))
         inst = ctx.get_shadow_instances(k)
@@ -168,7 +161,8 @@ def test_scene_observers_with_masks_lod_and_static_batches(ctx):
     ctx.pack_scene_observer_instances()
     total = 0
     for o, (r, w) in enumerate(zip(table, want_obs)):
-        want, pushed = expect(og, s.sc, push_order(w["visible"]), dyn, n_surf, quads, np.asarray(w["view"], f32).reshape(16), False)
+        want, pushed = expect(og, push_order(w["visible"]), dyn, n_surf, np.asarray(w["view"], f32).reshape(16), quads=quads,
+                              flags=s.sc.flags)
         assert_same(ctx.dynamic_batches("observer", o), want, ("observer", o))
         assert_same(ctx.dynamic_batches("observer", o, device=True), want, ("observer device", o))
         inst = ctx.get_scene_observer_instances(o)
@@ -194,7 +188,7 @@ def test_observers_shadow_maps_carry_no_quads(ctx):
         sort_of = dict(zip(inst["node"].tolist(), inst["sort_index"].tolist()))
         nodes = entries[m["first"]: m["first"] + m["count"]]
         seen += len(set(nodes.tolist()) & set(quads))
-        want, pushed = expect(og, s.sc, push_order(nodes), dyn, n_surf, quads, None, True, sort_of=lambda n: sort_of[n])
+        want, pushed = expect(og, push_order(nodes), dyn, n_surf, None, lambda n: sort_of[n], quads, shadow=True, flags=s.sc.flags)
         assert_same(ctx.dynamic_batches("shadow", k), want, ("map", k))
         assert sorted(zip(inst["node"].tolist(), inst["surface"].tolist())) == sorted(pushed), k
     assert seen > 0
@@ -434,8 +428,8 @@ def test_scene_mirror_end_to_end(ctx):
             attrs = tuple(scene.SPRITE_VERTEX_ATTRIBUTES if n.kind == "sprite" else scene.RECTANGLE_VERTEX_ATTRIBUTES)
             qs[i] = sbo.Quad(scene.QUAD_KINDS[n.kind], g._batch_keys[(n.material, 1)], g._layout_ids[attrs], tuple(n.uv_rect.tolist()),
                              n.color, float(n.size), float(n.rotation), n.flip_x, n.flip_y)
-        return sbo.mixed_pass(sorted(qs), lambda i: 1, {}, qs, lambda i: 0, lambda i: np.asarray(by_index[i].global_transform(), f32),
-                              False, lambda i: by_index[i].cast_shadows)[0]
+        return dbo.dynamic_pass(sorted(qs), lambda i: 1, {}, lambda i: 0, lambda i: np.asarray(by_index[i].global_transform(), f32), qs,
+                                False, lambda i: by_index[i].cast_shadows)[0]
 
     sprite_l = g._layout_ids[tuple(scene.SPRITE_VERTEX_ATTRIBUTES)]
     d = pack()

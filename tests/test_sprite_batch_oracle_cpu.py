@@ -1,5 +1,5 @@
-"""The mixed push_triangles oracle (tests/sprite_batch_oracle.py) on hand-built passes with known answers, the record layout,
-and the scene mirror's quad nodes, none of which needs a GPU."""
+"""The quad nodes of the push_triangles oracle (tests/dynamic_batch_oracle.py, tests/sprite_batch_oracle.py) on hand-built
+passes with known answers, the record layout, and the scene mirror's quad nodes, none of which needs a GPU."""
 import ctypes as C
 
 import numpy as np
@@ -27,8 +27,8 @@ def moved(x, y, z):
 
 def run(nodes, dyn=None, quads=None, shadow=False, cast=lambda n: True, world=ident, sort=None, n_surf=None):
     dyn = dyn or {}
-    return sbo.mixed_pass(nodes, n_surf or (lambda n: 1 + max([k for (m, k) in dyn if m == n], default=-1)), dyn, quads or {},
-                          sort or (lambda n: 100), world, shadow, cast)
+    return dbo.dynamic_pass(nodes, n_surf or (lambda n: 1 + max([k for (m, k) in dyn if m == n], default=-1)), dyn,
+                            sort or (lambda n: 100), world, quads, shadow, cast)
 
 
 def test_record_is_48_bytes():
@@ -40,26 +40,6 @@ def test_record_is_48_bytes():
     assert C.sizeof(Rec) == 48 and Context.SPRITE.itemsize == 48
     for name, _ in Rec._fields_:
         assert getattr(Rec, name).offset == Context.SPRITE.fields[name][1], name
-
-
-def test_equals_dynamic_pass_without_quads():
-    rng = np.random.default_rng(3)
-    dyn = {}
-    for n in range(1, 40):
-        for k in range(int(rng.integers(1, 3))):
-            if rng.random() < 0.6:
-                v = rng.standard_normal((int(rng.integers(3, 12)), 12)).astype(f32)
-                dyn[(n, k)] = dbo.DynSurface(int(rng.integers(0, 3)), 0, (48, 0, 12, 24), v.tobytes(),
-                                             rng.integers(0, len(v), (4, 3)).astype(np.uint32))
-    n_surf = {n: 1 + max([k for (m, k) in dyn if m == n], default=0) for n in range(1, 40)}
-    sort = lambda n: n % 4  # noqa: E731
-    world = lambda n: moved(n * 0.5, -1.0, 2.0)  # noqa: E731
-    a, pa = dbo.dynamic_pass(list(range(1, 40)), lambda n: n_surf[n], dyn, sort, world)
-    b, pb = run(list(range(1, 40)), dyn, n_surf=lambda n: n_surf[n], sort=sort, world=world)
-    assert pa == pb and a["bundles"].tobytes() == b["bundles"].tobytes() and a["instances"].tobytes() == b["instances"].tobytes()
-    for l, st in a["streams"].items():
-        assert st["vertices"].tobytes() == b["streams"][l]["vertices"].tobytes()
-        assert st["triangles"].tolist() == b["streams"][l]["triangles"].tolist()
 
 
 UV = (0.25, 0.5, 0.125, 0.25)  # lx 0.25, rx 0.375, ty 0.5, by 0.75
