@@ -298,8 +298,8 @@ static void tick(orc_animation *a, float dt)
 /* One BoundValue reaching a node: BoundValueCollection::apply (scene/animation/mod.rs:147-179) through
  * Transform::set_position / set_scale / set_rotation (scene/transform.rs:202-262: stored only if the transform is
  * already dirty or the value differs), each via local_transform_mut() = TransformChanged.
- * dirty[n] = Transform::dirty of node n (cleared by the matrix() of the last Graph::update), touched[n] = a
- * TransformChanged message was sent. */
+ * dirty[n] = Transform::dirty of node n (cleared by the matrix() of the last Graph::update; see frame_dirty_or_new),
+ * touched[n] = a TransformChanged message was sent. */
 static void apply_value(uint32_t binding, int is_quat, int is_vec3, const float v[4], uint32_t n, const orc_graph *g,
                         orc_transform *transforms, uint32_t n_nodes, uint8_t *dirty, uint8_t *touched)
 {
@@ -355,13 +355,24 @@ static void refresh_touched(orc_graph *g, orc_transform *transforms, uint32_t n_
         if (touched[k]) orc_node_set_local_transform(g, k, &transforms[k]);
 }
 
+/* Transform::dirty of every node for one frame.  Graph::update clears it (process_node_messages calls matrix() on
+ * every transform that changed) and then updates the nodes in pool order (graph/mod.rs:1459-1504): the animation
+ * players and the blend machines all apply their poses in that one loop and nothing calls matrix() between them, so
+ * a transform a player set stays dirty for a machine that sets it later in the same frame.  `frame_dirty` is that
+ * per-node flag, owned by the caller across the passes of one frame; NULL = a frame with this pass alone. */
+static uint8_t *frame_dirty_or_new(uint8_t *frame_dirty, uint32_t n_nodes)
+{
+    return frame_dirty ? frame_dirty : (uint8_t *)calloc(n_nodes ? n_nodes : 1, 1);
+}
+
 /* AnimationContainer::update_animations — scene/animation/mod.rs:83-88: every enabled animation, in pool order,
  * ticks and applies its pose.  `transforms` = the nodes' Transform objects (indexed by node); the local matrices
  * of the touched nodes are then refreshed (what Transform::matrix() does lazily inside Graph::update) and a
  * TransformChanged message is queued for each. */
-void orc_update_animations(orc_animation **anims, uint32_t n, float dt, orc_graph *g, orc_transform *transforms, uint32_t n_nodes)
+void orc_update_animations_in_frame(orc_animation **anims, uint32_t n, float dt, orc_graph *g, orc_transform *transforms,
+                                    uint32_t n_nodes, uint8_t *frame_dirty)
 {
-    uint8_t *dirty = (uint8_t *)calloc(n_nodes ? n_nodes : 1, 1);
+    uint8_t *dirty = frame_dirty_or_new(frame_dirty, n_nodes);
     uint8_t *touched = (uint8_t *)calloc(n_nodes ? n_nodes : 1, 1);
     for (uint32_t i = 0; i < n; ++i)
         if (anims[i] && anims[i]->enabled) {
@@ -369,8 +380,13 @@ void orc_update_animations(orc_animation **anims, uint32_t n, float dt, orc_grap
             apply_pose(anims[i], g, transforms, n_nodes, dirty, touched);
         }
     refresh_touched(g, transforms, n_nodes, touched);
-    free(dirty);
+    if (dirty != frame_dirty) free(dirty);
     free(touched);
+}
+
+void orc_update_animations(orc_animation **anims, uint32_t n, float dt, orc_graph *g, orc_transform *transforms, uint32_t n_nodes)
+{
+    orc_update_animations_in_frame(anims, n, dt, g, transforms, n_nodes, NULL);
 }
 
 /* ---- blend machine, the smallest useful subset (fyrox-animation/src/machine) ----
@@ -398,8 +414,8 @@ static void node_pose_push(node_pose *p, const pose_value *v)
     p->vals[p->n++] = *v;
 }
 
-void orc_blend_group_update(orc_animation **anims, const float *weights, uint32_t n, float dt, orc_graph *g,
-                            orc_transform *transforms, uint32_t n_nodes)
+void orc_blend_group_update_in_frame(orc_animation **anims, const float *weights, uint32_t n, float dt, orc_graph *g,
+                                     orc_transform *transforms, uint32_t n_nodes, uint8_t *frame_dirty)
 {
     for (uint32_t i = 0; i < n; ++i) /* animations_cache is a set: an animation ticks once */
         if (anims[i] && anims[i]->enabled) {
@@ -449,7 +465,7 @@ void orc_blend_group_update(orc_animation **anims, const float *weights, uint32_
             sp->n = 0;
         }
     }
-    uint8_t *dirty = (uint8_t *)calloc(n_nodes ? n_nodes : 1, 1);
+    uint8_t *dirty = frame_dirty_or_new(frame_dirty, n_nodes);
     uint8_t *touched = (uint8_t *)calloc(n_nodes ? n_nodes : 1, 1);
     for (uint32_t nd = 0; nd < n_nodes; ++nd)
         for (uint32_t k = 0; k < out[nd].n; ++k) {
@@ -463,6 +479,12 @@ void orc_blend_group_update(orc_animation **anims, const float *weights, uint32_
     }
     free(out);
     free(src);
-    free(dirty);
+    if (dirty != frame_dirty) free(dirty);
     free(touched);
+}
+
+void orc_blend_group_update(orc_animation **anims, const float *weights, uint32_t n, float dt, orc_graph *g,
+                            orc_transform *transforms, uint32_t n_nodes)
+{
+    orc_blend_group_update_in_frame(anims, weights, n, dt, g, transforms, n_nodes, NULL);
 }

@@ -234,6 +234,13 @@ void  orc_update_animations(orc_animation **anims, uint32_t n, float dt, orc_gra
                             uint32_t n_nodes);                                    /* scene/animation/mod.rs:83-88,107-179 */
 void  orc_blend_group_update(orc_animation **anims, const float *weights, uint32_t n, float dt, orc_graph *g,
                              orc_transform *transforms, uint32_t n_nodes);       /* machine/mod.rs:344-382, node/blend.rs:136-166, pose.rs:41-101 */
+/* The same passes inside one frame: frame_dirty = Transform::dirty per node, shared by every pass of the frame (the
+ * player and the machines) and cleared by the caller when the graph updates; NULL = a frame with this pass alone,
+ * which is what the two calls above are. */
+void  orc_update_animations_in_frame(orc_animation **anims, uint32_t n, float dt, orc_graph *g, orc_transform *transforms,
+                                     uint32_t n_nodes, uint8_t *frame_dirty);
+void  orc_blend_group_update_in_frame(orc_animation **anims, const float *weights, uint32_t n, float dt, orc_graph *g,
+                                      orc_transform *transforms, uint32_t n_nodes, uint8_t *frame_dirty);
 int   orc_node_is_alive(const orc_graph *g, uint32_t n);
 
 /* ---- "soa-omp-NT": the same arithmetic on flat arrays with OpenMP (fyrox_oracle_mt.c) — a best-effort multi-core CPU

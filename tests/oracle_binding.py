@@ -164,8 +164,10 @@ def lib() -> C.CDLL:
         "orc_animation_time_position": (C.c_float, [vp]),
         "orc_animation_is_enabled": (C.c_int, [vp]),
         "orc_update_animations": (None, [vp, C.c_uint32, C.c_float, vp, vp, C.c_uint32]),
+        "orc_update_animations_in_frame": (None, [vp, C.c_uint32, C.c_float, vp, vp, C.c_uint32, vp]),
         "orc_node_is_alive": (C.c_int, [vp, C.c_uint32]),
         "orc_blend_group_update": (None, [vp, f32p, C.c_uint32, C.c_float, vp, vp, C.c_uint32]),
+        "orc_blend_group_update_in_frame": (None, [vp, f32p, C.c_uint32, C.c_float, vp, vp, C.c_uint32, vp]),
         "orc_mt_new": (vp, [C.c_uint32, C.c_uint32, vp, vp, vp, vp, vp]),
         "orc_mt_free": (None, [vp]),
         "orc_mt_set_threads": (None, [vp, C.c_int]),
@@ -276,6 +278,14 @@ class Graph:
     def __init__(self, handle=None):
         self.L = lib()
         self.h = handle if handle is not None else self.L.orc_graph_new()
+        self._frame_dirty = np.zeros(0, np.uint8)
+
+    def frame_dirty(self, n_nodes):
+        """Transform::dirty of every node in this frame: set by the animation passes, cleared by update() /
+        update_hierarchical_data() (matrix() of every changed transform)."""
+        if self._frame_dirty.size < n_nodes:
+            self._frame_dirty = np.zeros(n_nodes, np.uint8)
+        return self._frame_dirty.ctypes.data_as(C.c_void_p)
 
     @staticmethod
     def build(parent, flags=None, render_mask=None, local_m16=None, local_aabb=None):
@@ -348,9 +358,11 @@ class Graph:
 
     def update(self):
         self.L.orc_graph_update(self.h)
+        self._frame_dirty[:] = 0
 
     def update_hierarchical_data(self):
         self.L.orc_graph_update_hierarchical_data(self.h)
+        self._frame_dirty[:] = 0
 
     def global_transform(self, n):
         out = np.empty(16, dtype=np.float32)
@@ -481,16 +493,17 @@ class Animation:
 
 
 def update_animations(anims, dt, graph: "Graph", transforms):
-    """AnimationContainer::update_animations over a list of Animation; `transforms` is a ctypes array of Transform per node."""
+    """AnimationContainer::update_animations over a list of Animation; `transforms` is a ctypes array of Transform per node.
+    The transforms stay dirty for the later passes of the frame until graph.update()."""
     arr = (C.c_void_p * max(len(anims), 1))(*[a.h for a in anims])
-    lib().orc_update_animations(arr, len(anims), float(dt), graph.h, transforms, len(transforms))
+    lib().orc_update_animations_in_frame(arr, len(anims), float(dt), graph.h, transforms, len(transforms), graph.frame_dirty(len(transforms)))
 
 
 def blend_group_update(anims, weights, dt, graph: "Graph", transforms):
     """One Machine (one layer, one state, BlendAnimations over PlayAnimation sources) evaluated and applied."""
     arr = (C.c_void_p * max(len(anims), 1))(*[a.h for a in anims])
     w = np.ascontiguousarray(weights, dtype=np.float32)
-    lib().orc_blend_group_update(arr, fp(w), len(anims), float(dt), graph.h, transforms, len(transforms))
+    lib().orc_blend_group_update_in_frame(arr, fp(w), len(anims), float(dt), graph.h, transforms, len(transforms), graph.frame_dirty(len(transforms)))
 
 
 # ---- "soa-omp-NT" multi-core baseline (fyrox_oracle_mt.c) ---------------------------------------------------
