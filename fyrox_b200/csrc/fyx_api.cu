@@ -434,9 +434,7 @@ struct fyx_ctx {
 
     // N4 LOD filter (fyx_drawprep.inl)
     SlotColumn lod_range{make_float2(NAN, NAN)}; // (begin, end); begin NaN = not a LOD object
-    DevBuf b_lodp;              // per slot: hidden-frusta bits
-    DevBuf b_prune;             // per slot: frusta in which the node's children are pruned (rendered static batches, hidden ancestors)
-    bool maybe_static_batch = false; // some node carries FYX_NODE_STATIC_BATCH: the cull runs level by level
+    bool maybe_static_batch = false; // some node carries FYX_NODE_STATIC_BATCH: the cull runs un-fused, through the pruner table
     std::vector<fyx_observer> observers;
 
     // N4 light lists (fyx_drawprep.inl)
@@ -454,7 +452,7 @@ struct fyx_ctx {
     uint32_t n_light_table = 0;
     DevBuf b_light_table;
     MapCull shadow_cull; // the last shadow cull: of one camera, or of the scene's observers
-    // per-map LOD filter and static-batch pruning (fyx_cull_shadow_casters_pruned).  pr_node: by node index, kPrLod | kPrBatch
+    // LOD filter and static-batch pruning of the camera culls and the many-map culls.  pr_node: by node index, kPrLod | kPrBatch
     // for a node with a LOD range / FYX_NODE_STATIC_BATCH (kept beside the device columns, so that a change is seen without
     // reading them back).  The pruner column is rebuilt by the first pruned cull after such a change (pr_dirty).
     std::vector<uint8_t> pr_node;
@@ -884,6 +882,7 @@ static void fyx_comm_destroy_internal(fyx_ctx *c); // fyx_comm.inl
 // DFS-pruning features (LOD filter, static batches): the cull cannot be fused into the level kernels (fyx_drawprep.inl)
 static bool unfused_cull(const fyx_ctx *c, uint32_t nf);
 static int32_t cull_unfused(fyx_ctx *c, uint32_t nf);
+static int32_t cull_prune_prepare(fyx_ctx *c, uint32_t nf);
 static int32_t animate_enqueue(fyx_ctx *c, float dt);  // fyx_anim.inl
 static int32_t allgather_enqueue(fyx_ctx *c, VisSlot &V, cudaStream_t s);
 static int32_t allgather_finish(fyx_ctx *c, VisSlot &V, cudaStream_t s);
@@ -1740,7 +1739,7 @@ extern "C" int32_t fyx_update_transforms(fyx_ctx *c, uint32_t update_flags)
 extern "C" int32_t fyx_cull(fyx_ctx *c, uint32_t nf, const fyx_frustum *fr, const uint32_t *cam_mask, const uint32_t *pass_flags)
 {
     int32_t rc;
-    if ((rc = enter(c))) return rc;
+    if ((rc = enter(c)) || (rc = cull_prune_prepare(c, nf))) return rc;
     return run_timed(c, EV_CULL, c->timings.cull_ms, [&] {
         if ((rc = prepare_cull(c, nf, fr, cam_mask, pass_flags)) || !nf) return rc;
         return cull_unfused(c, nf);
@@ -1751,7 +1750,7 @@ extern "C" int32_t fyx_update_and_cull(fyx_ctx *c, uint32_t update_flags, uint32
                                        const uint32_t *cam_mask, const uint32_t *pass_flags)
 {
     int32_t rc;
-    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    if ((rc = enter(c)) || (rc = commit_surfaces(c)) || (rc = cull_prune_prepare(c, nf))) return rc;
     return run_timed(c, EV_UPDATE, c->timings.update_ms, [&] {
         return (rc = prepare_cull(c, nf, fr, cam_mask, pass_flags)) ? rc : update_cull_enqueue(c, update_flags, nf);
     });
@@ -1877,7 +1876,7 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
     if (!c || !fr) return FYX_ERR_INVALID_ARGUMENT;
     if (fr->struct_size < offsetof(fyx_frame_desc, do_animate)) return fail(c, FYX_ERR_INVALID_ARGUMENT, "fyx_frame_desc.struct_size too small");
     int32_t rc;
-    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    if ((rc = enter(c)) || (rc = commit_surfaces(c)) || (rc = cull_prune_prepare(c, fr->n_frusta))) return rc;
     cudaStream_t s = c->stream;
     CU(cudaEventRecord(c->ev[EV_START], s));
     // 0. animation players tick before Graph::update (N2): curves are device-resident, nothing to upload

@@ -807,36 +807,6 @@ __global__ void __launch_bounds__(kBlock) k_dyn_quads(const NodeArrays a, const 
 
 } // namespace
 
-// N4 LOD filter, one hierarchy level: bit f of lodp[slot] = "hidden for observer f by the node's own LOD range or by an
-// ancestor's" (renderer/bundle.rs:898-916: normalised distance outside [begin, end]; :995: the DFS does not descend).
-__global__ void __launch_bounds__(kBlock) k_lod_level(const NodeArrays a, const uint32_t lo, const uint32_t hi, const float2 *range,
-                                                      uint32_t *lodp, const LodParams lp)
-{
-    const uint32_t slot = lo + blockIdx.x * kBlock + threadIdx.x;
-    if (slot >= hi) return;
-    const uint32_t p = a.parent[slot];
-    uint32_t hidden = (p != FYX_NONE) ? lodp[p] : 0u;
-    const float2 r = range[slot];
-    if (r.x == r.x) { // the node is an object of a LOD level
-        const float gx = a.G[0][slot].w, gy = a.G[1][slot].w, gz = a.G[2][slot].w; // global_position()
-        for (int f = 0; f < lp.nf; ++f) {
-            // metric_distance: |observer - position|, nalgebra's left-to-right dot, then sqrt
-            const float dx = FYX_ADD(lp.ox[f], -gx), dy = FYX_ADD(lp.oy[f], -gy), dz = FYX_ADD(lp.oz[f], -gz);
-            const float dist = __fsqrt_rn(FYX_ADD(FYX_ADD(FYX_MUL(dx, dx), FYX_MUL(dy, dy)), FYX_MUL(dz, dz)));
-            const float normalized = __fdiv_rn(FYX_ADD(dist, -lp.zn[f]), lp.zr[f]);
-            const bool visible = (normalized >= r.x) && (normalized <= r.y);
-            if (!visible) hidden |= 1u << f;
-        }
-    }
-    lodp[slot] = hidden;
-}
-
-void launch_lod_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, const float2 *range, uint32_t *lodp, const LodParams &lp)
-{
-    if (hi <= lo) return;
-    k_lod_level<<<(hi - lo + kBlock - 1) / kBlock, kBlock, 0, s>>>(a, lo, hi, range, lodp, lp);
-}
-
 // N3, bone matrices of the packed instances — RenderDataBundle::write_uniforms (renderer/bundle.rs:484-496): a skinned instance
 // gets a block of MAX_BONE_MATRICES (255) mat4: its bone_matrices, then all-zero matrices; an unskinned one gets none.
 // pass 1: which instance gets which block (order of the blocks is unspecified); inst_skin = the fyx surface id that skins the instance

@@ -276,16 +276,12 @@ void launch_update_subforest(cudaStream_t s, const NodeArrays &a, const Subfores
 // ---- launchers (fyx_kernels.cu) ----
 void launch_update_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, bool update_all,
                          const CullParams *cull /* nullptr = no fused cull */);
-void launch_cull(cudaStream_t s, const NodeArrays &a, const CullParams &cp, const uint32_t *lodp = nullptr /* per slot: frusta hidden by the LOD filter */);
-// one hierarchy level [lo, hi) with DFS pruning by rendered static batches (prune: per slot, frusta hidden for the children)
-void launch_cull_range(cudaStream_t s, const NodeArrays &a, const CullParams &cp, const uint32_t *lodp, uint32_t lo, uint32_t hi, uint32_t *prune);
-// N4 LOD filter (fyx_drawprep.cu): per observer translation, z_near and z_far - z_near
-struct LodParams {
-    int nf;
-    float ox[FYX_MAX_FRUSTA], oy[FYX_MAX_FRUSTA], oz[FYX_MAX_FRUSTA], zn[FYX_MAX_FRUSTA], zr[FYX_MAX_FRUSTA];
+// the observers of fyx_set_observers, one per frustum, by value
+struct Observers {
+    uint32_t n;
+    fyx_observer o[FYX_MAX_FRUSTA];
 };
-void launch_lod_level(cudaStream_t s, const NodeArrays &a, uint32_t lo, uint32_t hi, const float2 *range, uint32_t *lodp, const LodParams &lp);
-void launch_select_probes(cudaStream_t s, const NodeArrays &a, const LodParams &obs, uint32_t *best /* [nf], cleared to 0 by the caller: node index + 1 */);
+void launch_select_probes(cudaStream_t s, const NodeArrays &a, const Observers &obs, uint32_t *best /* [n], cleared to 0 by the caller: node index + 1 */);
 void launch_cull_lights(cudaStream_t s, const NodeArrays &a, const CullParams &cp, uint32_t *const *d_out_ptrs, uint32_t *counts);
 
 // N4 shadow casters (fyx_cull_shadow_casters): one record per light node, in pool order
@@ -419,6 +415,11 @@ uint32_t launch_observer_views(cudaStream_t s, const NodeArrays &a, const MapPar
 // after the table kernel: the pruner table when pr_level_off is given (one launch per entry of pr_level_off that holds
 // pruners, parents first), then the count pass; then the scan; then, once the host has sized the lists, the emit pass
 uint32_t launch_map_count(cudaStream_t s, const NodeArrays &a, const MapParams &mp, ShadowForm form, const uint32_t *pr_level_off, uint32_t n_levels);
+// The stand-alone camera cull over all slots: first, with pr_level_off, the camera's pruner table (pr.words = 1; pr.range
+// nullptr = no LOD filter), one launch per entry of pr_level_off that holds pruners, parents first; then k_cull, which masks
+// each node with its row (pr.col nullptr = no pruning)
+uint32_t launch_cull(cudaStream_t s, const NodeArrays &a, const CullParams &cp, const MapParams::Prune &pr, const Observers &obs,
+                     const uint32_t *pr_level_off, uint32_t n_levels);
 uint32_t launch_map_scan(cudaStream_t s, const MapParams &mp);
 uint32_t launch_map_emit(cudaStream_t s, const NodeArrays &a, const MapParams &mp, ShadowForm form, bool pruned);
 // fyx_cull_scene_observers' own passes: the light counts and environment maps (emit = false) or the light lists (emit = true);

@@ -388,15 +388,67 @@ __global__ void __launch_bounds__(kBlock) k_update_subforest(const NodeArrays a,
 // Stand-alone cull over all slots (static scene / extra passes: every shadow pass re-runs the cull
 // with its own frustum, renderer/shadow/*.rs).  32 B read per node + 4 B per visible entry.
 // ------------------------------------------------------------------------------------------------
-// prune != nullptr: one launch per hierarchy level [lo, hi) — a node is hidden for the frusta in which an ancestor pruned the
-// DFS: a statically batched mesh that is rendered (RdcControlFlow::Break, scene/mesh/mod.rs:725; renderer/bundle.rs:996-1001)
-// or, through lodp, a LOD object out of range.  prune[slot] = frusta hidden for the node's children.
-template <int NFT>
-__global__ void __launch_bounds__(kBlock) k_cull(const NodeArrays a, const CullParams cp, const uint32_t *lodp, const uint32_t lo, const uint32_t hi,
-                                                 uint32_t *prune)
+// the node's row of a pruner table: its own (it is a pruner) or its nearest pruner ancestor's children row
+__device__ __forceinline__ const uint32_t *pruner_row(const uint32_t *rows, const uint32_t words, const uint32_t pc)
 {
-    const uint32_t slot = lo + blockIdx.x * kBlock + threadIdx.x;
-    const bool valid = slot < hi;
+    if (pc == FYX_NONE) return nullptr;
+    return rows + ((size_t)(pc & ~kPrSelf) * 2u + ((pc & kPrSelf) ? 0u : 1u)) * words;
+}
+
+// One step of a pruner table, for pruner p at `slot` and the maps [32 w, 32 w + 32) of n_maps — the pruned DFS of
+// renderer/bundle.rs:898-916, 988-1004 with each map's observer, and Mesh::collect_render_data's Break
+// (scene/mesh/mod.rs:691-725):
+//   self_hidden[p]     = children_hidden[anc(p)] | (LOD object outside its range for the map's observer)
+//   children_hidden[p] = self_hidden[p] | (static batch drawn in the map)
+// Every pruner table computes its rows here; the caller gives map m's LOD observer, observer(m) (a fyx_observer: the
+// translation, z_near and z_far of ObserverPosition), and drawn(m): the node is in map m's list.
+template <class Observer, class Drawn>
+__device__ __forceinline__ void pruner_step(const NodeArrays &a, const MapParams::Prune &pr, const uint32_t p, const uint32_t slot,
+                                            const uint32_t w, const uint32_t n_maps, Observer observer, Drawn drawn)
+{
+    const uint32_t W = pr.words, anc = pr.anc[p];
+    uint32_t self = anc != FYX_NONE ? pr.rows[((size_t)anc * 2u + 1u) * W + w] : 0u, rendered = 0u;
+    const float2 r = pr.range ? pr.range[slot] : make_float2(NAN, NAN);
+    const bool lod = r.x == r.x, batch = (a.flags[slot] & FYX_NODE_STATIC_BATCH) != 0u;
+    const float gx = a.G[0][slot].w, gy = a.G[1][slot].w, gz = a.G[2][slot].w; // global_position()
+    for (uint32_t b = 0; b < 32u; ++b) {
+        const uint32_t m = w * 32u + b;
+        if (m >= n_maps) break;
+        if (lod) { // metric_distance: |observer - position|, nalgebra's left-to-right dot, then sqrt
+            const fyx_observer o = observer(m);
+            const float dx = FYX_ADD(o.translation[0], -gx), dy = FYX_ADD(o.translation[1], -gy), dz = FYX_ADD(o.translation[2], -gz);
+            const float dist = __fsqrt_rn(FYX_ADD(FYX_ADD(FYX_MUL(dx, dx), FYX_MUL(dy, dy)), FYX_MUL(dz, dz)));
+            const float normalized = __fdiv_rn(FYX_ADD(dist, -o.z_near), FYX_ADD(o.z_far, -o.z_near));
+            if (!((normalized >= r.x) && (normalized <= r.y))) self |= 1u << b;
+        }
+        if (batch && drawn(m)) rendered |= 1u << b;
+    }
+    pr.rows[((size_t)p * 2u) * W + w] = self;
+    pr.rows[((size_t)p * 2u + 1u) * W + w] = self | rendered;
+}
+
+// The pruner table of a camera cull, one launch per hierarchy level's pruners [p_lo, p_hi) (parents first), one thread per
+// pruner and one word per row (at most FYX_MAX_FRUSTA frusta); drawn in frustum f = bit f of cull_bits, k_cull's predicate.
+// The LOD observers travel by value (pr.range nullptr: no LOD filter, obs unused).
+__global__ void __launch_bounds__(kBlock) k_cull_pruners(const NodeArrays a, const CullParams cp, const MapParams::Prune pr, const Observers obs,
+                                                         const uint32_t p_lo, const uint32_t p_hi)
+{
+    const uint32_t p = p_lo + blockIdx.x * kBlock + threadIdx.x;
+    if (p >= p_hi) return;
+    const uint32_t slot = pr.slot[p];
+    const uint32_t drawn = cull_warp<0>(true, a.flags[slot], a.mask[slot], a.wa[0][slot], a.wa[1][slot], a.wa[2][slot], cp);
+    pruner_step(a, pr, p, slot, 0u, (uint32_t)cp.nf, [&](const uint32_t m) { return obs.o[m]; },
+                [&](const uint32_t m) { return ((drawn >> m) & 1u) != 0u; });
+}
+
+// pr.col != nullptr: a node is hidden for the frusta in which its row of the camera's pruner table (k_cull_pruners, one word
+// per row) says the DFS stopped above it or at it: a LOD object out of range, or a statically batched mesh that is rendered
+// (RdcControlFlow::Break, scene/mesh/mod.rs:725; renderer/bundle.rs:996-1001).
+template <int NFT>
+__global__ void __launch_bounds__(kBlock) k_cull(const NodeArrays a, const CullParams cp, const MapParams::Prune pr)
+{
+    const uint32_t slot = blockIdx.x * kBlock + threadIdx.x;
+    const bool valid = slot < a.cap;
     uint32_t nf = 0u, mask = 0u;
     float2 wx = make_float2(0.f, 0.f), wy = wx, wz = wx;
     if (valid) {
@@ -407,15 +459,9 @@ __global__ void __launch_bounds__(kBlock) k_cull(const NodeArrays a, const CullP
         wz = ld_stream(a.wa[2] + slot);
     }
     uint32_t vis_bits = cull_warp<NFT>(valid, nf, mask, wx, wy, wz, cp);
-    uint32_t hidden = 0u;
-    if (valid && (lodp || prune)) {
-        if (lodp) hidden = lodp[slot]; // frusta whose LOD filter hides the node or one of its ancestors
-        if (prune) {
-            const uint32_t p = a.parent[slot];
-            if (p != FYX_NONE) hidden |= prune[p];
-        }
-        vis_bits &= ~hidden;
-        if (prune) prune[slot] = hidden | ((nf & FYX_NODE_STATIC_BATCH) ? vis_bits : 0u);
+    if (pr.col && vis_bits) {
+        const uint32_t *row = pruner_row(pr.rows, 1u, pr.col[slot]);
+        if (row) vis_bits &= ~*row;
     }
     const uint32_t gi = vis_bits ? a.gidx[slot] : 0u;
     compact_emit<NFT>(vis_bits, gi, slot, cp);
@@ -1279,7 +1325,7 @@ void launch_update_subforest(cudaStream_t s, const NodeArrays &a, const Subfores
 
 // Reflection-probe selection of from_graph (renderer/bundle.rs:918-925): the last ReflectionProbe in pool order whose world box
 // contains the observer (AxisAlignedBoundingBox::is_contains_point, inclusive) — atomicMax over (node index + 1) per observer.
-__global__ void __launch_bounds__(kBlock) k_select_probes(const NodeArrays a, const LodParams obs, uint32_t *best)
+__global__ void __launch_bounds__(kBlock) k_select_probes(const NodeArrays a, const Observers obs, uint32_t *best)
 {
     const uint32_t slot = blockIdx.x * kBlock + threadIdx.x;
     if (slot >= a.cap) return;
@@ -1287,15 +1333,15 @@ __global__ void __launch_bounds__(kBlock) k_select_probes(const NodeArrays a, co
     if ((nf & (FYX_NODE_ALIVE | FYX_NODE_REFLECTION_PROBE)) != (FYX_NODE_ALIVE | FYX_NODE_REFLECTION_PROBE)) return;
     const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
     const uint32_t gi = a.gidx[slot];
-    for (int f = 0; f < obs.nf; ++f) {
-        const float px = obs.ox[f], py = obs.oy[f], pz = obs.oz[f];
+    for (uint32_t f = 0; f < obs.n; ++f) {
+        const float px = obs.o[f].translation[0], py = obs.o[f].translation[1], pz = obs.o[f].translation[2];
         if (px >= wx.x && px <= wx.y && py >= wy.x && py <= wy.y && pz >= wz.x && pz <= wz.y) atomicMax(best + f, gi + 1u);
     }
 }
 
-void launch_select_probes(cudaStream_t s, const NodeArrays &a, const LodParams &obs, uint32_t *best)
+void launch_select_probes(cudaStream_t s, const NodeArrays &a, const Observers &obs, uint32_t *best)
 {
-    if (!a.cap || !obs.nf) return;
+    if (!a.cap || !obs.n) return;
     k_select_probes<<<grid_for(a.cap), kBlock, 0, s>>>(a, obs, best);
 }
 
@@ -1305,21 +1351,28 @@ void launch_cull_lights(cudaStream_t s, const NodeArrays &a, const CullParams &c
     k_cull_lights<<<grid_for(a.cap), kBlock, 0, s>>>(a, cp, d_out_ptrs, counts);
 }
 
-void launch_cull_range(cudaStream_t s, const NodeArrays &a, const CullParams &cp, const uint32_t *lodp, uint32_t lo, uint32_t hi, uint32_t *prune)
+uint32_t launch_cull(cudaStream_t s, const NodeArrays &a, const CullParams &cp, const MapParams::Prune &pr, const Observers &obs,
+                     const uint32_t *pr_level_off, uint32_t n_levels)
 {
-    if (hi <= lo) return;
-    const unsigned g = grid_for(hi - lo);
-    switch (cp.nf) {
-    case 1: k_cull<1><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 2: k_cull<2><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 3: k_cull<3><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 4: k_cull<4><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    case 6: k_cull<6><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
-    default: k_cull<0><<<g, kBlock, 0, s>>>(a, cp, lodp, lo, hi, prune); break;
+    uint32_t n = 0u;
+    for (uint32_t l = 0; l < n_levels; ++l) {
+        const uint32_t lo = pr_level_off[l], hi = pr_level_off[l + 1];
+        if (hi <= lo) continue;
+        k_cull_pruners<<<grid_for(hi - lo), kBlock, 0, s>>>(a, cp, pr, obs, lo, hi);
+        ++n;
     }
+    if (!a.cap) return n;
+    const unsigned g = grid_for(a.cap);
+    switch (cp.nf) {
+    case 1: k_cull<1><<<g, kBlock, 0, s>>>(a, cp, pr); break;
+    case 2: k_cull<2><<<g, kBlock, 0, s>>>(a, cp, pr); break;
+    case 3: k_cull<3><<<g, kBlock, 0, s>>>(a, cp, pr); break;
+    case 4: k_cull<4><<<g, kBlock, 0, s>>>(a, cp, pr); break;
+    case 6: k_cull<6><<<g, kBlock, 0, s>>>(a, cp, pr); break;
+    default: k_cull<0><<<g, kBlock, 0, s>>>(a, cp, pr); break;
+    }
+    return n + 1u;
 }
-
-void launch_cull(cudaStream_t s, const NodeArrays &a, const CullParams &cp, const uint32_t *lodp) { launch_cull_range(s, a, cp, lodp, 0u, a.cap, nullptr); }
 
 void launch_fold_bones(cudaStream_t s, const NodeArrays &a, const FoldArrays &fa, const CullParams *cull)
 {
@@ -1783,18 +1836,8 @@ __device__ __forceinline__ bool shadow_in_map(const FrustumDev *__restrict__ F, 
     return ok;
 }
 
-// the node's row of the pruner table: its own (it is a pruner) or its nearest pruner ancestor's children row
-__device__ __forceinline__ const uint32_t *pruner_row(const MapParams &mp, const uint32_t pc)
-{
-    if (pc == FYX_NONE) return nullptr;
-    return mp.pr.rows + ((size_t)(pc & ~kPrSelf) * 2u + ((pc & kPrSelf) ? 0u : 1u)) * mp.pr.words;
-}
-
 // The pruner table of a shadow cull, one launch per hierarchy level's pruners [p_lo, p_hi) (parents first), one thread per
-// (pruner, word of 32 maps) — renderer/bundle.rs:898-916, 988-1004 with each map's observer, and Mesh::collect_render_data's
-// Break (scene/mesh/mod.rs:691-725):
-//   self_hidden[p]     = children_hidden[anc(p)] | (LOD object outside its range for the map's observer)
-//   children_hidden[p] = self_hidden[p] | (static batch rendered in the map)
+// (pruner, word of 32 maps); drawn in a map = shadow_in_map
 template <int FORM>
 __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, const MapParams mp, const uint32_t p_lo, const uint32_t p_hi)
 {
@@ -1803,33 +1846,21 @@ __global__ void __launch_bounds__(kBlock) k_shadow_pruners(const NodeArrays a, c
     const uint64_t t = (uint64_t)blockIdx.x * kBlock + threadIdx.x;
     if (t >= (uint64_t)(p_hi - p_lo) * W) return;
     const uint32_t p = p_lo + (uint32_t)(t / W), w = (uint32_t)(t % W);
-    const uint32_t slot = mp.pr.slot[p], anc = mp.pr.anc[p];
-    uint32_t self = anc != FYX_NONE ? mp.pr.rows[((size_t)anc * 2u + 1u) * W + w] : 0u, rendered = 0u;
+    const uint32_t slot = mp.pr.slot[p];
     const uint32_t nf = a.flags[slot], mask = a.mask[slot];
-    const float2 r = mp.pr.range ? mp.pr.range[slot] : make_float2(NAN, NAN);
-    const bool lod = r.x == r.x, batch = (nf & FYX_NODE_STATIC_BATCH) != 0u;
     const float2 wx = a.wa[0][slot], wy = a.wa[1][slot], wz = a.wa[2][slot];
-    const float gx = a.G[0][slot].w, gy = a.G[1][slot].w, gz = a.G[2][slot].w; // global_position()
     const PackedConsts kc = packed_consts();
     const bool cand = shadow_candidate<FORM>(nf, mask, mp);
     const bool tame = cand && aabb_is_tame(wx, wy, wz);
     const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
-    const uint32_t n_maps = *mp.n_maps;
     uint32_t unused = 0u;
-    for (uint32_t b = 0; b < 32u; ++b) {
-        const uint32_t m = w * 32u + b;
-        if (m >= n_maps) break;
-        if (lod) { // k_lod_level's arithmetic with the map's observer
+    pruner_step(
+        a, mp.pr, p, slot, w, *mp.n_maps,
+        [&](const uint32_t m) {
             const float *o = mp.pr.obs + (size_t)m * 5;
-            const float dx = FYX_ADD(o[0], -gx), dy = FYX_ADD(o[1], -gy), dz = FYX_ADD(o[2], -gz);
-            const float dist = __fsqrt_rn(FYX_ADD(FYX_ADD(FYX_MUL(dx, dx), FYX_MUL(dy, dy)), FYX_MUL(dz, dz)));
-            const float normalized = __fdiv_rn(FYX_ADD(dist, -o[3]), FYX_ADD(o[4], -o[3]));
-            if (!((normalized >= r.x) && (normalized <= r.y))) self |= 1u << b;
-        }
-        if (batch && shadow_in_map<false, FORM>(mp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused, mask)) rendered |= 1u << b;
-    }
-    mp.pr.rows[((size_t)p * 2u) * W + w] = self;
-    mp.pr.rows[((size_t)p * 2u + 1u) * W + w] = self | rendered;
+            return fyx_observer{{o[0], o[1], o[2]}, o[3], o[4]};
+        },
+        [&](const uint32_t m) { return shadow_in_map<false, FORM>(mp.frusta, m, cand, test, tame, wx, wy, wz, kc, nullptr, unused, mask); });
 }
 
 // pass 2: every node read once (flags, mask, box: 32 B; with PRUNE its pruner id: 4 B more) and tested against every map;
@@ -1859,7 +1890,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_count(const NodeArrays a, con
         const bool test = cand && (nf & FYX_NODE_FRUSTUM_CULLING);
         const FrustumDev *__restrict__ F = mp.frusta;
         const uint32_t n_maps = *mp.n_maps;
-        const uint32_t *hrow = PRUNE && cand ? pruner_row(mp, pc) : nullptr;
+        const uint32_t *hrow = PRUNE && cand ? pruner_row(mp.pr.rows, mp.pr.words, pc) : nullptr;
         uint32_t hword = 0u;
         for (uint32_t m = 0; m < n_maps; ++m) {
             const bool ok = shadow_in_map<PRUNE, FORM>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);
@@ -1919,7 +1950,7 @@ __global__ void __launch_bounds__(kBlock) k_shadow_emit(const NodeArrays a, cons
     const FrustumDev *__restrict__ F = mp.frusta;
     const uint32_t n_maps = *mp.n_maps;
     const uint32_t lt = (1u << lane) - 1u;
-    const uint32_t *hrow = PRUNE && cand ? pruner_row(mp, pc) : nullptr;
+    const uint32_t *hrow = PRUNE && cand ? pruner_row(mp.pr.rows, mp.pr.words, pc) : nullptr;
     uint32_t hword = 0u;
     for (uint32_t m = 0; m < n_maps; ++m) {
         const bool ok = shadow_in_map<PRUNE, FORM>(F, m, cand, test, tame, wx, wy, wz, kc, hrow, hword, mask);

@@ -363,7 +363,8 @@ int32_t fyx_get_shadow_maps_device(fyx_ctx *ctx, const fyx_shadow_map **d_maps, 
  * pool order, levels and objects in order, the last write wins.  Carried over by fyx_set_topology with the node indices.
  * fyx_set_observers: ObserverPosition::{translation, z_near, z_far} of the frusta of the culls that follow, one per
  * frustum (count 0 = no LOD filtering).  While both are set the cull runs un-fused: update, then one small pass per
- * hierarchy level that propagates the filter bits from parents to children, then the cull over all nodes. */
+ * hierarchy level that holds LOD objects or static batches, over those nodes only, that propagates the filter bits from
+ * parents to children, then the cull over all nodes. */
 typedef struct fyx_observer {
     float translation[3];
     float z_near, z_far;

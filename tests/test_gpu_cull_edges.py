@@ -123,7 +123,7 @@ def test_fused_update_and_cull_on_edge_boxes(ctx, n_frusta, update):
     assert_census(census, frusta=frusta)
 
 
-# ---- 2. stand-alone fyx_cull: k_cull<NFT>, flat and level by level with prune / lodp ------------------------------------------
+# ---- 2. stand-alone fyx_cull: k_cull<NFT>, flat and masked by the camera's pruner table ---------------------------------------
 @pytest.mark.parametrize("n_frusta", [1, 2, 3, 4, 5, 6, 7, 8])
 def test_cull_on_edge_boxes(ctx, n_frusta):
     rng = np.random.default_rng(200 + n_frusta)
@@ -141,7 +141,7 @@ def test_cull_on_edge_boxes(ctx, n_frusta):
 @pytest.mark.parametrize("n_frusta", [1, 3, 6, 7])
 def test_cull_with_static_batch_and_lod_group_on_edge_boxes(ctx, n_frusta):
     """A static batch (its sub-tree is pruned where the batch is visible) and LOD objects (hidden where out of range) make k_cull
-    run level by level with prune / lodp; the edge boxes hang under the batch, on the LOD objects and beside them."""
+    run after the camera's pruner table; the edge boxes hang under the batch, on the LOD objects and beside them."""
     rng = np.random.default_rng(300 + n_frusta)
     frusta = pick_frusta(rng, n_frusta)
     cam, pf = masks_for(n_frusta)

@@ -86,7 +86,7 @@ def test_static_batches_prune_the_dfs_like_rdc_control_flow_break(ctx):
     """A statically batched mesh (BatchingMode::Static) that is rendered for a frustum returns RdcControlFlow::Break: its
     children are not visited FOR THAT FRUSTUM (scene/mesh/mod.rs:701-725, renderer/bundle.rs:996-1001); one that is culled
     lets the DFS continue.  Random forest with static batches at every depth, nested ones, six frusta with masks and a shadow
-    pass; fused-capable entry points (they must notice and run level by level), flags set later through fyx_set_flags."""
+    pass; fused-capable entry points (they must notice and run the cull un-fused), flags set later through fyx_set_flags."""
     rng = np.random.default_rng(41)
     parent, flags, mask, local, aabb = random_graph(rng, 5000, p_orphan=0.01, max_depth_bias=0.2)
     renderable = np.nonzero((flags & fb.NODE_RENDERABLE) != 0)[0]
@@ -120,7 +120,7 @@ def test_static_batches_prune_the_dfs_like_rdc_control_flow_break(ctx):
     for f, fo in enumerate(fos):
         pruned_something += og0.from_graph(fo, int(cam[f]), bool(pf[f] & fb.PASS_SHADOW)).size - og.from_graph(fo, int(cam[f]), bool(pf[f] & fb.PASS_SHADOW)).size
     assert pruned_something > 20
-    # flags arriving later through fyx_set_flags switch the level-by-level cull on as well
+    # flags arriving later through fyx_set_flags switch the pruned cull on as well
     with fb.Context() as c2:
         c2.set_topology(parent, flags, mask, aabb)
         c2.set_local_matrices(local)

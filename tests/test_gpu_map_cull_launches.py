@@ -2,7 +2,8 @@
 one sequence: a one-CTA table kernel, the pruner table (one launch per hierarchy level that holds pruners), the count pass,
 the scan, and the emit pass when there is a list to write.  Pins the kernel launches of every call in its steady state (the
 second call: the first also builds the light table and the pruner column), with and without pruners, and with no map and
-no observer at all."""
+no observer at all.  The camera cull (fyx_cull) shares the pruner table's rule: the table (one launch per hierarchy level
+that holds pruners), then one launch over all slots."""
 import numpy as np
 import pytest
 
@@ -84,3 +85,14 @@ def test_kernel_launches_of_every_map_cull(ctx, scene):
     assert launches(ctx, lambda: ctx.cull_scene_shadow_casters(*WIDE)) == 4 + levels
     assert min(n_entries()) > 0 and len(ctx.get_scene_shadow_maps()) > 0
 
+
+
+@pytest.mark.parametrize("n_frusta", [1, 6])
+def test_kernel_launches_of_a_camera_cull(ctx, scene, n_frusta):
+    s, levels = scene
+    _, ff, _, _ = camera()
+    frusta = [ff] * n_frusta
+    ctx.set_observers([((float(k), 0.0, 0.0), 0.1, 150.0) for k in range(n_frusta)])  # the LOD filter is on
+    assert launches(ctx, lambda: ctx.cull(frusta)) == 1 + levels
+    ctx.set_observers([])  # LOD objects without observers still prune nothing, static batches still do
+    assert launches(ctx, lambda: ctx.cull(frusta)) == 1 + levels
