@@ -79,6 +79,59 @@ struct SlotColumn {
     int32_t scatter(fyx_ctx *c, uint32_t count, const uint32_t *idx, const void *values); // the nodes' records, from the host
 };
 
+// One record per node index, for what the setters keep on the host by node: light sources, CSM options, cameras, reflection
+// probes, node surfaces, pruner marks.  `def` is the record of a node that was never given one.  Across fyx_set_topology a
+// record stays with its node index while the node is alive before and after the call; every other index starts again from
+// `def`, as in the slot columns.
+template <class T> struct NodeRecords {
+    T def;
+    std::vector<T> rec; // by node index; the indices past its end hold `def`
+    explicit NodeRecords(const T &v) : def(v) {}
+    const T &operator[](uint32_t node) const { return node < rec.size() ? rec[node] : def; }
+    void set(uint32_t node, const T &v)
+    {
+        if (node >= rec.size()) rec.resize(node + 1, def);
+        rec[node] = v;
+    }
+    int32_t check(fyx_ctx *c, uint32_t count, const uint32_t *idx) const; // every node listed (idx NULL = 0..count-1) is in range
+    // keep(record) trims a record that stays to what it keeps.  Only the records that restart are written.
+    template <class Keep> void topology_changed(const std::vector<uint32_t> &old_slot_of_node, const std::vector<uint32_t> &new_slot_of_node, Keep keep)
+    {
+        if (rec.size() > new_slot_of_node.size()) rec.resize(new_slot_of_node.size());
+        for (size_t i = 0; i < rec.size(); ++i) {
+            if (i < old_slot_of_node.size() && old_slot_of_node[i] != FYX_NONE && new_slot_of_node[i] != FYX_NONE) keep(rec[i]);
+            else rec[i] = def;
+        }
+    }
+    void topology_changed(const std::vector<uint32_t> &old_slot_of_node, const std::vector<uint32_t> &new_slot_of_node)
+    {
+        topology_changed(old_slot_of_node, new_slot_of_node, [](T &) {});
+    }
+    // f(node, slot, record) for the record of every alive node, in pool order
+    template <class F> void for_alive(const std::vector<uint32_t> &slot_of_node, F f)
+    {
+        const size_t n = std::min(rec.size(), slot_of_node.size());
+        for (size_t node = 0; node < n; ++node)
+            if (slot_of_node[node] != FYX_NONE) f((uint32_t)node, slot_of_node[node], rec[node]);
+    }
+};
+
+// The records kept with a value derived from them: the projection's one transcendental, evaluated on the host with the
+// platform's tanf, and whether a probe is due
+struct LightRec {
+    fyx_light_source src;
+    float m22; // 1 / tan(fovy / 2)
+};
+struct CameraRec {
+    fyx_camera cam;
+    float m22_or_vertical_size; // perspective: 1 / tan(fov / 2)
+};
+struct ProbeRec {
+    fyx_reflection_probe probe;
+    bool due; // set or forced since the observer table was built: its rendered bit starts at 0
+};
+constexpr fyx_csm_options kCsmDefault{0u, {5.0f, 25.0f, 64.0f}}; // FrustumSplitOptions::default() (scene/light/directional.rs:83-91)
+
 // page-locked host memory
 struct PinnedBuf {
     void *p = nullptr;
@@ -394,7 +447,7 @@ struct fyx_ctx {
     DevBuf b_vflag;        // one byte per vertex block: raw or coded (fyx_vcode.cuh)
     bool vblk_raw = false; // a palette of more than kSkinRingMaxBones bones was loaded: every block raw from then on
     // surfaces per node (fyx_set_node_surfaces): host CSR by node, device table by slot (rebuilt when dirty)
-    std::vector<uint2> ms_of_node;       // (first, count) into ms_bundle_h / ms_skin_h; count 0 = default single surface
+    NodeRecords<uint2> ms_of_node{make_uint2(0u, 0u)}; // (first, count) into ms_bundle_h / ms_skin_h; count 0 = default single surface
     std::vector<uint32_t> ms_bundle_h, ms_skin_h;
     bool ms_dirty = false, have_ms = false;
     uint32_t ms_max = 0;                 // the most surfaces any node was given (bounds the shadow maps' bundle tables)
@@ -445,9 +498,8 @@ struct fyx_ctx {
     bool lights_valid = false;
 
     // N4 shadow casters (fyx_drawprep.inl): light-source records by node index, their device table by pool order, the maps
-    std::vector<fyx_light_source> light_src; // kind FYX_LIGHT_UNKNOWN = no record
-    std::vector<float> light_m22;
-    std::vector<fyx_csm_options> csm_opts; // by node index; missing = FrustumSplitOptions::default()
+    NodeRecords<LightRec> light_src{LightRec{fyx_light_source{FYX_LIGHT_UNKNOWN, 0.f, 0.f}, 0.f}}; // kind FYX_LIGHT_UNKNOWN = no record
+    NodeRecords<fyx_csm_options> csm_opts{kCsmDefault};
     bool light_table_dirty = false;
     uint32_t n_light_table = 0;
     DevBuf b_light_table;
@@ -455,7 +507,7 @@ struct fyx_ctx {
     // LOD filter and static-batch pruning of the camera culls and the many-map culls.  pr_node: by node index, kPrLod | kPrBatch
     // for a node with a LOD range / FYX_NODE_STATIC_BATCH (kept beside the device columns, so that a change is seen without
     // reading them back).  The pruner column is rebuilt by the first pruned cull after such a change (pr_dirty).
-    std::vector<uint8_t> pr_node;
+    NodeRecords<uint8_t> pr_node{uint8_t(0)};
     bool pr_dirty = true;
     uint32_t n_pruners = 0;
     std::vector<uint32_t> pr_level_off; // pruner ids per hierarchy level (pruners are numbered in slot order)
@@ -463,10 +515,8 @@ struct fyx_ctx {
 
     // N4 scene observers (fyx_drawprep.inl): camera and reflection-probe records by node index, their device table (due
     // probes, then cameras, each in pool order; rebuilt when a record or the topology changes), the observer cull's outputs
-    std::vector<fyx_camera> cam_src;            // projection FYX_PROJECTION_NONE = no record
-    std::vector<float> cam_m22;                 // 1 / tan(fov / 2) or vertical_size
-    std::vector<fyx_reflection_probe> probe_src; // present 0 = no record
-    std::vector<uint8_t> probe_due;             // set or forced since the table was built: its rendered bit starts at 0
+    NodeRecords<CameraRec> cam_src{CameraRec{fyx_camera{0u, FYX_PROJECTION_NONE}, 0.f}}; // projection FYX_PROJECTION_NONE = no record
+    NodeRecords<ProbeRec> probe_src{ProbeRec{fyx_reflection_probe{}, false}};            // present 0 = no record
     std::vector<uint32_t> ob_rec_node;          // node of each record of the device table
     bool obs_table_dirty = false;
     uint32_t n_ob_recs = 0;
@@ -642,6 +692,15 @@ int32_t SlotColumn::scatter(fyx_ctx *c, uint32_t count, const uint32_t *idx, con
     return rc ? rc : scatter_words(c, buf.as<uint32_t>(), def.words, count, idx, values);
 }
 
+template <class T> int32_t NodeRecords<T>::check(fyx_ctx *c, uint32_t count, const uint32_t *idx) const
+{
+    for (uint32_t e = 0; e < count; ++e) {
+        const uint32_t node = idx ? idx[e] : e;
+        if (node >= c->n_nodes) return fail(c, FYX_ERR_INVALID_ARGUMENT, "node %u out of range", node);
+    }
+    return FYX_OK;
+}
+
 int32_t check_device_errors(fyx_ctx *c)
 {
     // called right after a stream synchronisation; h_err was copied before it
@@ -686,10 +745,11 @@ int32_t enter(fyx_ctx *c)
 // a pruner mark (kPrLod / kPrBatch) of an alive node set or cleared; the pruner column is rebuilt when a mark changes
 void pr_mark(fyx_ctx *c, uint32_t node, uint8_t bit, bool on)
 {
-    if (node >= c->n_nodes || node >= c->pr_node.size() || c->slot_of_node[node] == FYX_NONE) return; // skipped by the scatter kernels too
+    if (node >= c->n_nodes || c->slot_of_node[node] == FYX_NONE) return; // skipped by the scatter kernels too
     const uint8_t m = on ? (c->pr_node[node] | bit) : (c->pr_node[node] & ~bit);
-    if (m != c->pr_node[node]) c->pr_dirty = true;
-    c->pr_node[node] = m;
+    if (m == c->pr_node[node]) return;
+    c->pr_node.set(node, m);
+    c->pr_dirty = true;
 }
 
 void rebuild_node_arrays(fyx_ctx *c)
@@ -958,87 +1018,27 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     if (capacity && !parent) return fail(c, FYX_ERR_INVALID_ARGUMENT, "parent is NULL");
     if (capacity == FYX_NONE) return fail(c, FYX_ERR_INVALID_ARGUMENT, "capacity too large");
     CU(cudaSetDevice(c->device));
-    const uint32_t def_flags = FYX_NODE_VISIBILITY | FYX_NODE_ENABLED | FYX_NODE_FRUSTUM_CULLING | FYX_NODE_CAST_SHADOWS | FYX_NODE_ALIVE;
-    auto fl = [&](uint32_t i) { return flags ? (flags[i] & FYX_NODE_INPUT_MASK) : def_flags; };
-    auto alive = [&](uint32_t i) { return i < capacity && (fl(i) & FYX_NODE_ALIVE); };
-
-    // depth of every alive node (parent chains; a dead / out-of-range parent counts as "no parent",
-    // like Pool::try_borrow failing in graph/mod.rs:1210)
-    std::vector<int32_t> depth(capacity, -1);
-    std::vector<uint32_t> path;
-    uint32_t max_depth = 0;
-    for (uint32_t i = 0; i < capacity; ++i) {
-        if (!alive(i) || depth[i] >= 0) continue;
-        path.clear();
-        uint32_t n = i;
-        int32_t base = -1;
-        while (true) {
-            if (depth[n] >= 0) { base = depth[n]; break; }
-            if (depth[n] == -2) return fail(c, FYX_ERR_TOPOLOGY, "cycle in parent[] through node %u", n);
-            depth[n] = -2;
-            path.push_back(n);
-            const uint32_t p = parent[n];
-            if (p == FYX_NONE || !alive(p)) break;
-            n = p;
-        }
-        for (size_t k = path.size(); k-- > 0;) {
-            base += 1;
-            depth[path[k]] = base;
-            max_depth = std::max<uint32_t>(max_depth, (uint32_t)base);
-        }
-    }
-    // counting sort by depth, stable in node index
-    std::vector<uint32_t> level_off(capacity ? max_depth + 2 : 1, 0);
-    uint32_t n_slots = 0;
-    for (uint32_t i = 0; i < capacity; ++i)
-        if (alive(i)) { level_off[depth[i] + 1]++; n_slots++; }
-    for (size_t l = 1; l < level_off.size(); ++l) level_off[l] += level_off[l - 1];
-    std::vector<uint32_t> cursor(level_off.begin(), level_off.end());
-    std::vector<uint32_t> slot_of_node(capacity, FYX_NONE), node_of_slot(n_slots);
-    for (uint32_t i = 0; i < capacity; ++i)
-        if (alive(i)) {
-            const uint32_t s = cursor[depth[i]]++;
-            slot_of_node[i] = s;
-            node_of_slot[s] = i;
-        }
-    // within a level, order by parent slot (counting sort, stable in node index): siblings become
-    // contiguous, so a warp's gather of parent rows touches one or two parents instead of 32
-    {
-        std::vector<uint32_t> tmp, cnt;
-        for (size_t d = 1; d + 1 < level_off.size(); ++d) {
-            const uint32_t plo = level_off[d - 1], phi = level_off[d], lo = level_off[d], hi = level_off[d + 1];
-            if (hi - lo < 2) continue;
-            cnt.assign((size_t)(phi - plo) + 1, 0);
-            for (uint32_t s = lo; s < hi; ++s) cnt[slot_of_node[parent[node_of_slot[s]]] - plo + 1]++;
-            for (size_t k = 1; k < cnt.size(); ++k) cnt[k] += cnt[k - 1];
-            tmp.resize(hi - lo);
-            for (uint32_t s = lo; s < hi; ++s) {
-                const uint32_t i = node_of_slot[s];
-                tmp[cnt[slot_of_node[parent[i]] - plo]++] = i;
-            }
-            for (uint32_t k = 0; k < hi - lo; ++k) {
-                node_of_slot[lo + k] = tmp[k];
-                slot_of_node[tmp[k]] = lo + k;
-            }
-        }
-    }
+    SlotPlan plan = plan_slots(capacity, parent, flags);
+    if (plan.cycle_node != FYX_NONE) return fail(c, FYX_ERR_TOPOLOGY, "cycle in parent[] through node %u", plan.cycle_node);
+    const char *env = getenv("FYX_SUBFOREST"); // 1 forces the sub-forest plan on, 0 off
+    const SubforestLayout sf = plan_subforest(plan, (env && *env) ? atoi(env) : -1);
+    const uint32_t n_slots = plan.n_slots();
 
     // slot-ordered host columns
-    std::vector<uint32_t> h_parent(n_slots), h_flags(n_slots), h_mask(n_slots), h_gidx(n_slots);
+    const uint32_t def_flags = FYX_NODE_VISIBILITY | FYX_NODE_ENABLED | FYX_NODE_FRUSTUM_CULLING | FYX_NODE_CAST_SHADOWS | FYX_NODE_ALIVE;
+    std::vector<uint32_t> h_flags(n_slots), h_mask(n_slots), h_gidx(n_slots);
     std::vector<float2> h_la[3];
     for (auto &v : h_la) v.resize(n_slots);
+    std::vector<uint32_t> static_batch; // nodes with FYX_NODE_STATIC_BATCH
     uint32_t n_renderable = 0;
-    bool any_static = false;
     for (uint32_t s = 0; s < n_slots; ++s) {
-        const uint32_t i = node_of_slot[s];
-        const uint32_t p = parent[i];
-        h_parent[s] = (p != FYX_NONE && alive(p)) ? slot_of_node[p] : FYX_NONE;
-        uint32_t f = fl(i) | F_DIRTY_SELF;
+        const uint32_t i = plan.node_of_slot[s];
+        uint32_t f = (flags ? (flags[i] & FYX_NODE_INPUT_MASK) : def_flags) | F_DIRTY_SELF;
         if (i == root) f |= F_ROOT;
         if (i < c->skinned_node.size() && c->skinned_node[i]) f |= F_SKINNED;
         h_flags[s] = f;
         n_renderable += (f & FYX_NODE_RENDERABLE) ? 1u : 0u;
-        any_static |= (f & FYX_NODE_STATIC_BATCH) != 0;
+        if (f & FYX_NODE_STATIC_BATCH) static_batch.push_back(i);
         h_mask[s] = render_mask ? render_mask[i] : 0xFFFFFFFFu;
         h_gidx[s] = global_index ? global_index[i] : i;
         if (local_aabb) {
@@ -1051,66 +1051,6 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
         }
     }
 
-    // Sub-forest plan: from the first level on whose sub-trees are all small (<= kSfCap nodes) and numerous relative to the
-    // level's width (skeletons under a wide level of meshes), whole sub-trees are grouped so that no level of a group has
-    // more than kSfCap nodes; a group is one CTA of k_update_subforest.  Not worth it for wide deep levels (each launch is
-    // busy by itself): FYX_SUBFOREST=1 forces it on, =0 off.
-    std::vector<uint2> sf_rng;
-    uint32_t sf_first = 0, sf_levels = 0, sf_ctas = 0;
-    {
-        const char *env = getenv("FYX_SUBFOREST");
-        const int mode = (env && *env) ? atoi(env) : -1;
-        const size_t nlev = level_off.size() ? level_off.size() - 1 : 0;
-        if (mode != 0 && nlev >= 4 && n_slots) {
-            std::vector<uint32_t> size(n_slots, 1u);
-            for (uint32_t s2 = n_slots; s2-- > 0;)
-                if (h_parent[s2] != FYX_NONE) size[h_parent[s2]] += size[s2];
-            // widest level at or below l: a wide level keeps a launch of its own busy, only narrow ones are launch-bound
-            std::vector<uint32_t> widest(nlev + 1, 0u);
-            for (size_t l = nlev; l-- > 0;) widest[l] = std::max(widest[l + 1], level_off[l + 1] - level_off[l]);
-            size_t pick = 0;
-            for (size_t l = 1; l + 3 <= nlev; ++l) {
-                uint32_t mx = 0;
-                for (uint32_t s2 = level_off[l]; s2 < level_off[l + 1]; ++s2) mx = std::max(mx, size[s2]);
-                const uint64_t cnt = level_off[l + 1] - level_off[l], deep = n_slots - level_off[l];
-                if (cnt && mx <= kSfCap && deep >= 8 * cnt && (mode == 1 || widest[l] <= 131072u)) { pick = l; break; }
-            }
-            // on by default only where every deep level is narrow (<= 131 072 nodes)
-            if (pick) {
-                sf_first = (uint32_t)pick;
-                sf_levels = (uint32_t)(nlev - pick);
-                // per level, where each sub-tree's nodes start: the sub-trees of level `pick` in slot order own consecutive ranges
-                const uint32_t n_tiles = level_off[pick + 1] - level_off[pick];
-                std::vector<uint32_t> tile_of(n_slots - level_off[pick]);
-                std::vector<uint32_t> cnt((size_t)n_tiles * sf_levels, 0u);
-                for (uint32_t s2 = level_off[pick]; s2 < n_slots; ++s2) {
-                    const uint32_t rel = s2 - level_off[pick];
-                    tile_of[rel] = (s2 < level_off[pick + 1]) ? rel : tile_of[h_parent[s2] - level_off[pick]];
-                }
-                for (size_t l = pick; l < nlev; ++l)
-                    for (uint32_t s2 = level_off[l]; s2 < level_off[l + 1]; ++s2) cnt[(size_t)tile_of[s2 - level_off[pick]] * sf_levels + (l - pick)]++;
-                std::vector<uint32_t> cursor(sf_levels), acc(sf_levels, 0u);
-                for (uint32_t li = 0; li < sf_levels; ++li) cursor[li] = level_off[pick + li];
-                auto close_group = [&]() {
-                    for (uint32_t li = 0; li < sf_levels; ++li) {
-                        sf_rng.push_back(make_uint2(cursor[li], cursor[li] + acc[li]));
-                        cursor[li] += acc[li];
-                        acc[li] = 0;
-                    }
-                    sf_ctas++;
-                };
-                for (uint32_t t = 0; t < n_tiles; ++t) {
-                    bool fits = true;
-                    for (uint32_t li = 0; li < sf_levels; ++li)
-                        if (acc[li] + cnt[(size_t)t * sf_levels + li] > kSfCap) fits = false;
-                    if (!fits) close_group();
-                    for (uint32_t li = 0; li < sf_levels; ++li) acc[li] += cnt[(size_t)t * sf_levels + li];
-                }
-                close_group();
-            }
-        }
-    }
-
     // Per-node data that is NOT an argument of this call survives it: the slot columns (local matrices, TRS records, transform
     // statics, bundle ids and LOD ranges) of every node that was alive before and still is are carried from their old slot to
     // the new one on the device (nodes that were not alive start from the defaults).  old_of_new[s] = the old slot.
@@ -1119,9 +1059,9 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     int32_t rc;
     if (carry) {
         std::vector<uint32_t> old_of_new(n_slots, FYX_NONE);
-        for (uint32_t s2 = 0; s2 < n_slots; ++s2) {
-            const uint32_t i = node_of_slot[s2];
-            if (i < c->n_nodes && c->slot_of_node[i] != FYX_NONE) old_of_new[s2] = c->slot_of_node[i];
+        for (uint32_t s = 0; s < n_slots; ++s) {
+            const uint32_t i = plan.node_of_slot[s];
+            if (i < c->n_nodes && c->slot_of_node[i] != FYX_NONE) old_of_new[s] = c->slot_of_node[i];
         }
         if ((rc = dev_ensure(c, b_map, (size_t)n_slots * 4))) return rc;
         CU(cudaStreamSynchronize(c->stream));
@@ -1132,26 +1072,12 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
         if (!carry) col->live = false; // nothing to carry over (first topology, or one side empty): the column starts afresh
         else if ((rc = col->carry(c, b_map.as<uint32_t>()))) return rc;
     }
-    // the pruner marks: a LOD range stays with a node alive before and after (as the column carries it), static batches come
-    // from the new flags
-    {
-        const size_t old_cap = c->slot_of_node.size();
-        c->pr_node.resize(capacity, 0);
-        for (uint32_t i = 0; i < capacity; ++i) {
-            const bool kept = carry && i < old_cap && c->slot_of_node[i] != FYX_NONE && slot_of_node[i] != FYX_NONE;
-            uint8_t m = kept ? (c->pr_node[i] & kPrLod) : 0;
-            if (slot_of_node[i] != FYX_NONE && (fl(i) & FYX_NODE_STATIC_BATCH)) m |= kPrBatch;
-            c->pr_node[i] = m;
-        }
-        c->pr_dirty = true;
-    }
     if (!carry) c->n_bundle_ids = 1;
 
     // device columns.  Everything is allocated before the fills below are launched: the planes the level kernels stream side by
     // side stay adjacent in allocation order (with a fill launched between them, k_update_level measured ~1% slower on an
     // H100 80GB HBM3 at a 400 W power limit).
     const size_t n = std::max<uint32_t>(n_slots, 1);
-    c->light_table_dirty = true; // the light-source records stay with their node indices; their slots are looked up again
     if ((rc = dev_ensure(c, c->b_parent, n * 4))) return rc;
     if ((rc = dev_ensure(c, c->b_flags, n * 4))) return rc;
     if ((rc = dev_ensure(c, c->b_mask, n * 4))) return rc;
@@ -1165,26 +1091,21 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     }
     CU(cudaStreamSynchronize(c->stream));
     if (n_slots) {
-        CU(cudaMemcpy(c->b_parent.p, h_parent.data(), n_slots * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(c->b_parent.p, plan.parent.data(), n_slots * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(c->b_flags.p, h_flags.data(), n_slots * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(c->b_mask.p, h_mask.data(), n_slots * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(c->b_gidx.p, h_gidx.data(), n_slots * 4, cudaMemcpyHostToDevice));
         for (int k = 0; k < 3; ++k) CU(cudaMemcpy(c->b_la[k].p, h_la[k].data(), n_slots * sizeof(float2), cudaMemcpyHostToDevice));
     }
-    if (capacity) CU(cudaMemcpy(c->b_slot_of_node.p, slot_of_node.data(), (size_t)capacity * 4, cudaMemcpyHostToDevice));
-
-    const bool same_capacity = c->have_topology && capacity == c->n_nodes;
-    c->n_nodes = capacity;
-    c->root = root;
-    c->n_renderable = n_renderable;
-    c->maybe_static_batch = any_static;
+    if (capacity) CU(cudaMemcpy(c->b_slot_of_node.p, plan.slot_of_node.data(), (size_t)capacity * 4, cudaMemcpyHostToDevice));
     c->sf = SubforestPlan{};
-    if (sf_ctas) {
-        if ((rc = dev_ensure(c, c->b_sf_rng, sf_rng.size() * sizeof(uint2)))) return rc;
-        CU(cudaMemcpy(c->b_sf_rng.p, sf_rng.data(), sf_rng.size() * sizeof(uint2), cudaMemcpyHostToDevice));
-        c->sf.n_ctas = sf_ctas;
-        c->sf.n_levels = sf_levels;
-        c->sf.first_level = sf_first;
+    if (sf.n_ctas()) {
+        static_assert(sizeof(SfRange) == sizeof(uint2), "a sub-forest range is the uint2 the kernel reads");
+        if ((rc = dev_ensure(c, c->b_sf_rng, sf.rng.size() * sizeof(uint2)))) return rc;
+        CU(cudaMemcpy(c->b_sf_rng.p, sf.rng.data(), sf.rng.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+        c->sf.n_ctas = sf.n_ctas();
+        c->sf.n_levels = sf.n_levels;
+        c->sf.first_level = sf.first_level;
         c->sf.rng = c->b_sf_rng.as<uint2>();
     }
     // local rows are always there; global matrices start as identity rows (the local rows' default), world boxes as
@@ -1195,28 +1116,44 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
         launch_permute_words(c->stream, c->b_wa[k].p, nullptr, nullptr, n_slots, WordRecord(make_float2(3.402823466e38f, -3.402823466e38f)));
         c->launches += 2;
     }
-    c->slot_of_node.swap(slot_of_node);
-    c->node_of_slot.swap(node_of_slot);
-    c->level_off.swap(level_off);
+
+    const bool same_capacity = c->have_topology && capacity == c->n_nodes;
+    const std::vector<uint32_t> old_slot_of_node = std::move(c->slot_of_node);
+    c->slot_of_node = std::move(plan.slot_of_node);
+    c->node_of_slot = std::move(plan.node_of_slot);
+    c->level_off = std::move(plan.level_off);
+    c->n_nodes = capacity;
+    c->root = root;
+    c->n_renderable = n_renderable;
+    c->maybe_static_batch = !static_batch.empty();
     c->have_topology = true;
     c->updated_once = false;
-    if (!same_capacity) c->dfs_rank.clear(); // indexed by node: stays valid while the pool capacity does
-    c->rank_on_device = false; // re-derived from dfs_rank in the new slot order
+    rebuild_node_arrays(c);
+
+    // the other owners of per-node data
+    const std::vector<uint32_t> &new_slot_of_node = c->slot_of_node;
+    c->light_src.topology_changed(old_slot_of_node, new_slot_of_node);
+    c->csm_opts.topology_changed(old_slot_of_node, new_slot_of_node);
+    c->cam_src.topology_changed(old_slot_of_node, new_slot_of_node);
+    c->probe_src.topology_changed(old_slot_of_node, new_slot_of_node);
+    c->ms_of_node.topology_changed(old_slot_of_node, new_slot_of_node);
+    // a pruner mark keeps its LOD bit (as the LOD range column does); static batches come from the new flags
+    c->pr_node.topology_changed(old_slot_of_node, new_slot_of_node, [](uint8_t &m) { m &= kPrLod; });
+    for (uint32_t i : static_batch) pr_mark(c, i, kPrBatch, true);
     c->shadow_cull.topology_changed();
     c->observer_cull.topology_changed();
-    ++c->hier_epoch;
-    // camera and probe records stay with their node indices; a node that is not alive any more drops its record
-    for (size_t i = 0; i < c->cam_src.size(); ++i)
-        if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->cam_src[i].projection = FYX_PROJECTION_NONE;
-    for (size_t i = 0; i < c->probe_src.size(); ++i)
-        if (i >= capacity || c->slot_of_node[i] == FYX_NONE) c->probe_src[i].present = 0u;
+    c->dyn.topology_changed(c);
+
+    // the tables derived from them, which address nodes by slot
+    c->light_table_dirty = true;
     c->obs_table_dirty = true;
-    c->dyn.topology_changed(c); // dynamic registrations and quad nodes too
-    c->ms_dirty = c->have_ms;  // the per-slot surface table too (the CSR itself is by node)
-    if (c->ms_of_node.size() < capacity) c->ms_of_node.resize(capacity, make_uint2(0u, 0u));
-    c->anim_csr_dirty = true; // animated nodes are addressed by slot
-    c->tables_dirty = true; // bone slots depend on the slot order
-    rebuild_node_arrays(c);
+    c->ms_dirty = c->have_ms;
+    c->pr_dirty = true;
+    c->anim_csr_dirty = true;
+    c->tables_dirty = true; // bone slots
+    if (!same_capacity) c->dfs_rank.clear(); // indexed by node: stays valid while the pool capacity does
+    c->rank_on_device = false;
+    ++c->hier_epoch;
     return FYX_OK;
 }
 

@@ -14,6 +14,7 @@
 
 #include "../../include/fyrox_b200.h"
 #include "fyx_math.cuh"
+#include "fyx_slots.hpp"
 
 namespace fyx {
 
@@ -263,10 +264,9 @@ void launch_bone_block_index(cudaStream_t s, uint32_t n, const uint32_t *inst_sk
 void launch_bone_blocks(cudaStream_t s, uint32_t n, const uint32_t *inst_skin, const uint2 *surf_bones, const float *palette, const uint32_t *block_of_inst,
                         float *blocks);
 
-// Sub-forest plan (fyx_set_topology): the deep levels of the hierarchy — small sub-trees such as skeletons — are cut into groups
-// of whole sub-trees; one CTA walks all levels of its group with CTA-wide barriers instead of one kernel launch per level.
-// Slots are sorted by (depth, parent slot), so the nodes of a group form ONE contiguous slot range in every level.
-constexpr uint32_t kSfCap = 384; // nodes per level and CTA (the previous level's matrices stay in shared memory)
+// Sub-forest plan (plan_subforest, fyx_slots.hpp): the deep levels of the hierarchy — small sub-trees such as skeletons — are
+// cut into groups of whole sub-trees; one CTA walks all levels of its group with CTA-wide barriers instead of one kernel
+// launch per level.
 struct SubforestPlan {
     uint32_t n_ctas = 0, n_levels = 0, first_level = 0; // deep levels = [first_level, first_level + n_levels)
     const uint2 *rng = nullptr;                        // [cta][level] = slot range (begin, end)

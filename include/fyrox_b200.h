@@ -147,9 +147,9 @@ void    fyx_mat4_mul(const float a_m16[16], const float b_m16[16], float out_m16
  * Marks every node changed (like Base::on_connected_to_graph, scene/base.rs:520-540): the next update recomputes
  * every global matrix and world box.
  * What the call keeps: everything that is per node but not an argument here — local matrices, TRS records, transform
- * statics, bundle ids, LOD ranges, skinned surfaces and animations — stays with its node index (the data moves to the
- * node's new place on the device); a node index that was not alive before the call starts from the defaults (identity
- * local matrix ...).  The DFS order is kept while `capacity` is unchanged.  So the add / link / remove sequence of
+ * statics, bundle ids, LOD ranges, light sources, CSM options, cameras, reflection probes, node surfaces, skinned surfaces
+ * and animations — stays with its node index (the data moves to the node's new place on the device); a node index that was
+ * not alive before the call starts from the defaults (identity local matrix ...).  The DFS order is kept while `capacity` is unchanged.  So the add / link / remove sequence of
  * INTEGRATION.md is: fyx_set_topology with the new columns, then upload the matrices of the NEW or changed nodes only. */
 int32_t fyx_set_topology(fyx_ctx *ctx, uint32_t capacity, uint32_t root, const uint32_t *parent,
                          const uint32_t *flags, const uint32_t *render_mask, const float *local_aabb_minmax,
@@ -246,7 +246,8 @@ int32_t fyx_get_visible_lights(fyx_ctx *ctx, uint32_t frustum, const uint32_t **
  *
  * fyx_set_light_sources: the LightSource data of `count` light nodes (idx NULL = nodes 0..count-1) that the world
  * transform does not give: kind, SpotLight::full_cone_angle (spot only) and SpotLight::distance / PointLight::radius.
- * FYX_LIGHT_UNKNOWN removes the node's record.  Carried over by fyx_set_topology with the node indices.  The projection's
+ * FYX_LIGHT_UNKNOWN removes the node's record.  fyx_set_topology keeps a record with its node index while the node is alive
+ * before and after the call; any other node index starts again without a record.  The projection's
  * one transcendental, m22 = 1 / tan(fovy / 2) (fovy = full_cone_angle, or FRAC_PI_2 for a point light), is evaluated here
  * with the platform's tanf; everything the device does with the record is + − × ÷ √.
  *
@@ -271,8 +272,9 @@ int32_t fyx_get_visible_lights(fyx_ctx *ctx, uint32_t frustum, const uint32_t **
  * camera_frustum is not a frustum of the last cull.
  *
  * fyx_set_csm_options: the FrustumSplitOptions (scene/light/directional.rs:60-91) of `count` directional light nodes (idx
- * NULL = nodes 0..count-1).  A node without a record uses the reference's default, Absolute {5, 25, 64}.  Carried over by
- * fyx_set_topology with the node indices.  FYX_ERR_INVALID_ARGUMENT for a node out of range or `relative` other than 0 / 1.
+ * NULL = nodes 0..count-1).  A node without a record uses the reference's default, Absolute {5, 25, 64}.  fyx_set_topology
+ * keeps a record with its node index while the node is alive before and after the call; any other node index starts again
+ * from the default.  FYX_ERR_INVALID_ARGUMENT for a node out of range or `relative` other than 0 / 1.
  *
  * fyx_cull_shadow_casters_csm: fyx_cull_shadow_casters plus the cascaded shadow maps of the directional lights
  * (renderer/shadow/csm.rs:165-277).  A directional light in the camera's light list gets maps when its node has
@@ -377,8 +379,8 @@ int32_t fyx_set_observers(fyx_ctx *ctx, uint32_t count, const fyx_observer *obse
  *
  * fyx_set_cameras / fyx_set_reflection_probes: the Camera / ReflectionProbe data of `count` nodes (idx NULL = nodes
  * 0..count-1) that the global transform does not give.  A record with projection FYX_PROJECTION_NONE (camera) or present 0
- * (probe) removes the node's record.  Records are kept by node index, carried over by fyx_set_topology; a node that a
- * topology removes drops its record.  The perspective's one transcendental, 1 / tan(fov / 2), is evaluated here with the
+ * (probe) removes the node's record.  Records are kept by node index: fyx_set_topology keeps a record while the node is
+ * alive before and after the call; any other node index starts again without a record.  The perspective's one transcendental, 1 / tan(fov / 2), is evaluated here with the
  * platform's tanf (a probe's fov is 90f32.to_radians() = FRAC_PI_2, the point lights' value).  Setting a probe's record
  * makes it due, as does fyx_force_reflection_probe_update (ReflectionProbe::force_update, scene/probe.rs:215-218).
  *
@@ -646,7 +648,9 @@ int32_t fyx_animate(fyx_ctx *ctx, float dt);
  * For node idx[i] the surfaces are entries [first[i], first[i+1]) of bundle_ids / skin_surface (first has count + 1 entries):
  * bundle_ids[k] = the dense bundle id of surface k, skin_surface[k] = the fyx surface id (fyx_add_skinned_surface) whose
  * palette skins it, FYX_NONE (or skin_surface == NULL) = unskinned.  Nodes never listed keep the default: one surface in the
- * node's bundle id (fyx_set_bundle_ids), skinned iff the node has a skinned surface.  A count of 0 surfaces restores the default. */
+ * node's bundle id (fyx_set_bundle_ids), skinned iff the node has a skinned surface.  A count of 0 surfaces restores the default.
+ * fyx_set_topology keeps a node's surfaces with its node index while the node is alive before and after the call; any other
+ * node index starts again from the default. */
 int32_t fyx_set_node_surfaces(fyx_ctx *ctx, uint32_t count, const uint32_t *idx, const uint32_t *first, const uint32_t *bundle_ids,
                               const uint32_t *skin_surface);
 /* Per-node bundle id = the host's dense id for the (material, surface data, render path) key that push()

@@ -1,8 +1,9 @@
 """Dynamic batching on the device: each pack's dynamic batches (bundles, instances, transformed vertex streams, shifted
 triangles) against tests/dynamic_batch_oracle.py run over the same pass in DFS order, for a camera frustum (with and without
 fyx_set_dfs_order) and every shadow map; registered surfaces leave the ordinary instances; register-then-clear changes nothing;
-registrations follow their nodes across fyx_set_topology; a registered surface that fyx_set_node_surfaces later removes or
-names skinned is pushed again; the device getters equal the host getters."""
+registrations follow their nodes across fyx_set_topology, and a node removed and brought back has neither its registrations
+nor its surfaces; a registered surface that fyx_set_node_surfaces later removes or names skinned is pushed again; the device
+getters equal the host getters."""
 import numpy as np
 import pytest
 
@@ -186,7 +187,7 @@ def test_register_then_clear_changes_nothing(ctx):
     assert run(ctx, True) == want
 
 
-def test_registrations_follow_their_nodes_across_topology(ctx):
+def test_registrations_and_surfaces_follow_their_nodes_across_topology(ctx):
     _, sc, og, dyn, n_surf = build(ctx, 60)
     parents = set(sc.parent.tolist())
     dyn_nodes = sorted({n for n, _ in dyn} - parents)  # leaves: removing them leaves every other node's path as it was
@@ -201,12 +202,14 @@ def test_registrations_follow_their_nodes_across_topology(ctx):
     og2.update_hierarchical_data()
     kept = {k: v for k, v in dyn.items() if k[0] not in set(gone)}
     check_frustum(ctx, og2, kept, n_surf)
-    # and back: the removed nodes come back (with their local matrices sent again) without registrations
+    # and back: the removed nodes come back (with their local matrices sent again) without registrations, and with the
+    # default single surface instead of the surfaces they had
     ctx.set_topology(sc.parent, sc.flags, sc.mask, sc.aabb)
     back = np.array(gone, np.uint32)
     ctx.set_local_matrices(sc.local[back], back)
     ctx.update_transforms(fb.UPDATE_ALL)
-    check_frustum(ctx, og, kept, n_surf)
+    assert any(n_surf.get(n, 1) > 1 for n in gone)
+    check_frustum(ctx, og, kept, {**n_surf, **{n: 1 for n in gone}})
 
 
 def test_node_surfaces_changed_after_a_pack(ctx):

@@ -117,6 +117,47 @@ def test_random_scenes_across_calls(ctx, seed):
     observe_and_shadow(ctx, s.pr.oracle(), s)
 
 
+def test_records_of_a_node_removed_and_back_start_from_the_defaults(ctx):
+    """A light record, CSM options and node surfaces stay with their node index across fyx_set_topology only while the node is
+    alive before and after it: a node that one topology removes and the next brings back starts from the defaults, as a
+    camera does in test_records_carried_across_topology."""
+    rng = np.random.default_rng(6600)
+    s = ObserverScene(rng, 3000, 6, 4)
+    shadowy(s)
+    sc = s.sc
+    ctx.enable_instances(True)
+    og = s.load(ctx)
+    want, (maps, _, _) = observe_and_shadow(ctx, og, s, settings=WIDE)
+    lit = {int(m["light"]) for m in maps}
+    spot = min(n for n in lit if sc.sources[n][0] == fb.LIGHT_SPOT)
+    dirl = min(n for n in lit if sc.sources[n][0] == DIR)
+    special = set(sc.lights.tolist()) | set(s.cam_nodes.tolist()) | set(s.probe_nodes.tolist()) | {0}
+    mesh = min(set(np.concatenate([w["visible"] for w in want]).tolist()) - special)
+    opt = np.zeros(1, fb.Context.CSM_OPTIONS_DTYPE)
+    opt[0] = (1, (0.1, 0.5, 1.0))
+    ctx.set_csm_options(opt, np.array([dirl], np.uint32))
+    ctx.set_node_surfaces([mesh], [[(3, None), (4, None)]])
+    # removed by one topology, back with the next; the spot light's record is not sent again, the directional light's is
+    flags = sc.flags.copy()
+    sc.flags[[spot, dirl, mesh]] &= ~np.uint32(fb.NODE_ALIVE)
+    ctx.set_topology(sc.parent, sc.flags, sc.mask, sc.aabb)
+    sc.flags = flags
+    del sc.sources[spot]
+    og = s.load(ctx)
+    # no spot maps, the default cascades (the oracle's), one surface in bundle 0
+    want, (maps, _, _) = observe_and_shadow(ctx, og, s, settings=WIDE)
+    lit = {int(m["light"]) for m in maps}
+    assert dirl in lit and spot not in lit
+    ctx.pack_scene_observer_instances()
+    n_mesh = 0
+    for o, w in enumerate(want):
+        got = ctx.get_scene_observer_instances(o)
+        k = int(np.count_nonzero(got["node"] == mesh))
+        assert k == int(np.count_nonzero(w["visible"] == mesh)) and not got["surface"][got["node"] == mesh].any()
+        n_mesh += k
+    assert n_mesh
+
+
 def test_distinct_masks_are_not_merged(ctx):
     rng = np.random.default_rng(6200)
     s = ObserverScene(rng, 2500, 4, 2)
