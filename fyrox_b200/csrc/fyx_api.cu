@@ -221,19 +221,6 @@ struct Stream {
     operator cudaStream_t() const { return h; }
 };
 
-struct Surface {
-    uint32_t mesh_node;
-    uint32_t n_bones;
-    uint32_t bone_off;  // first palette entry
-    uint32_t n_verts;
-    uint64_t vert_off;  // first vertex (multiple of 4)
-    std::vector<uint32_t> bones; // node indices
-    // N4 blend shapes
-    uint32_t n_shapes = 0, bs_blocks = 0, bs_cap = 0; // shapes, 128-vertex blocks per shape, capacity of the region in shape blocks
-    uint64_t bs_off = 0;                               // first shape block of the region
-    uint32_t w_off = 0, w_cap = 0;
-};
-
 enum { EV_START = 0, EV_UPLOAD, EV_UPDATE, EV_CULL, EV_PALETTE, EV_SKIN, EV_READBACK, EV_COUNT };
 
 // Output of one cull: per-frustum visible lists + counters, device and (pinned) host side.  Two slots
@@ -377,6 +364,35 @@ struct DynBatches {
                  bool shadow);
 };
 
+// The skinned surfaces (fyx_add_skinned_surface) and what the frame kernels read of them: the vertex store, the bone tables,
+// the blend-shape pools, and the tables plan_skin (fyx_skin_plan.hpp) derives from the surfaces and the topology, which
+// commit rebuilds when `dirty`.  Surfaces and skinned_node stay with their node index across topology calls.
+struct Skinning {
+    std::vector<SkinSurface> surfaces;
+    std::vector<uint8_t> skinned_node; // per node: has a skinned surface
+    // vertex store: 128-vertex blocks with one flag byte each (raw or coded, fyx_vcode.cuh), the skinned output streams
+    uint64_t n_verts = 0, vert_cap = 0; // padded
+    DevBuf b_vblk, b_vflag, b_opos, b_onrm;
+    bool vblk_raw = false; // a palette of more than kSkinRingMaxBones bones was loaded: every block raw from then on
+    uint32_t n_entries = 0, entry_cap = 0; // bone tables: one entry per (surface, bone)
+    DevBuf b_ib[3], b_palette;
+    DevBuf b_bs, b_bs_w;  // blend-shape offsets (blocked f16) and weights
+    uint64_t bs_used = 0; // shape blocks handed out
+    uint32_t bs_w_used = 0;
+    bool dirty = false; // the derived tables (SkinPlan) below are out of date
+    DevBuf b_bone_slot, b_tiles, b_fold_node, b_fold_begin, b_fold_bone, b_fold_stale_idx, b_late_slot, b_stale_pos;
+    DevBuf b_surf_of_slot, b_surf_bones; // per slot: the node's first skinned surface (FYX_NONE = none); per surface: its palette range
+    uint32_t n_tiles = 0, n_fold = 0, n_late = 0, max_bones = 0;
+    bool any_blend_shapes = false;
+
+    bool is_skinned(uint32_t node) const { return node < skinned_node.size() && skinned_node[node]; }
+    int32_t grow(fyx_ctx *c, uint32_t entries, uint64_t verts); // room for this many palette entries and (padded) vertices
+    int32_t commit(fyx_ctx *c); // plan_skin, then the upload of the derived tables
+    void topology_changed() { dirty = true; } // bone and mesh slots
+    SkinArrays arrays() const;  // what the kernels read, from the buffers as they are now
+    FoldArrays fold() const;
+};
+
 } // namespace
 
 struct PeerState {
@@ -437,33 +453,14 @@ struct fyx_ctx {
     cudaEvent_t ev_levels_prev = nullptr; // the previous frame's "level kernels + fold + cull are done" event (its ev_cull), if it recorded one
     uint64_t launches_at_frame_end = ~0ull;
 
-    // skinning
-    std::vector<Surface> surfaces;
-    bool tables_dirty = false;
-    uint64_t n_verts_total = 0; // padded
-    uint64_t vert_cap = 0;
-    uint32_t n_entries = 0, entry_cap = 0;
-    DevBuf b_vblk, b_opos, b_onrm, b_ib[3], b_palette, b_bone_slot, b_tiles;
-    DevBuf b_vflag;        // one byte per vertex block: raw or coded (fyx_vcode.cuh)
-    bool vblk_raw = false; // a palette of more than kSkinRingMaxBones bones was loaded: every block raw from then on
+    Skinning skin;
+    std::vector<uint32_t> dfs_rank; // optional: pre-order rank of every node in the reference's DFS (fyx_set_dfs_order); read through dfs_rank_of
     // surfaces per node (fyx_set_node_surfaces): host CSR by node, device table by slot (rebuilt when dirty)
     NodeRecords<uint2> ms_of_node{make_uint2(0u, 0u)}; // (first, count) into ms_bundle_h / ms_skin_h; count 0 = default single surface
     std::vector<uint32_t> ms_bundle_h, ms_skin_h;
     bool ms_dirty = false, have_ms = false;
     uint32_t ms_max = 0;                 // the most surfaces any node was given (bounds the shadow maps' bundle tables)
     DevBuf b_ms_range, b_ms_bundle, b_ms_skin;
-    DevBuf b_surf_of_slot, b_surf_bones; // per slot: the node's first skinned surface (FYX_NONE = none); per surface: (first palette entry, n_bones)
-    DevBuf b_bs, b_bs_w;          // blend-shape offsets (blocked f16) and weights
-    uint64_t bs_used = 0;         // shape blocks handed out
-    uint32_t bs_w_used = 0;
-    bool any_blend_shapes = false;
-    DevBuf b_fold_node, b_fold_begin, b_fold_bone, b_fold_stale_idx, b_late_slot, b_stale_pos;
-    std::vector<uint32_t> dfs_rank; // optional: pre-order rank of every node in the reference's DFS (fyx_set_dfs_order)
-    uint32_t n_late = 0;
-    uint32_t n_tiles = 0, max_bones = 0;
-    FoldArrays fold{};
-    SkinArrays sk{};
-    std::vector<uint8_t> skinned_node; // per node: has a skinned surface
 
     // timing
     Event ev[EV_COUNT];
@@ -742,6 +739,8 @@ int32_t enter(fyx_ctx *c)
     return FYX_OK;
 }
 
+const uint32_t *dfs_rank_of(const fyx_ctx *c) { return valid_dfs_rank(c->dfs_rank, c->n_nodes); }
+
 // a pruner mark (kPrLod / kPrBatch) of an alive node set or cleared; the pruner column is rebuilt when a mark changes
 void pr_mark(fyx_ctx *c, uint32_t node, uint8_t bit, bool on)
 {
@@ -814,8 +813,9 @@ int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cu
     const bool all = (update_flags & FYX_UPDATE_ALL) || !c->updated_once;
     const size_t nl = c->level_off.size() ? c->level_off.size() - 1 : 0;
     ++c->hier_epoch;
-    if (c->n_late) {
-        launch_snapshot_bones(c->stream, c->a, c->n_late, c->b_late_slot.as<uint32_t>(), c->b_stale_pos.as<float4>());
+    const Skinning &sk = c->skin;
+    if (sk.n_late) {
+        launch_snapshot_bones(c->stream, c->a, sk.n_late, sk.b_late_slot.as<uint32_t>(), sk.b_stale_pos.as<float4>());
         c->launches++;
     }
     const size_t nl_wide = c->sf.n_ctas ? std::min<size_t>(nl, c->sf.first_level) : nl;
@@ -827,12 +827,12 @@ int32_t run_update(fyx_ctx *c, uint32_t update_flags, const CullParams *cull, cu
         launch_update_subforest(c->stream, c->a, c->sf, all, cull);
         c->launches++;
     }
-    if (c->fold.n) {
+    if (sk.n_fold) {
         if (fold_on) {
             CU(cudaEventRecord(c->ev_levels_done, c->stream));
             CU(cudaStreamWaitEvent(fold_on, c->ev_levels_done, 0));
         }
-        launch_fold_bones(fold_on ? fold_on : c->stream, c->a, c->fold, cull);
+        launch_fold_bones(fold_on ? fold_on : c->stream, c->a, sk.fold(), cull);
         c->launches++;
         if (fold_on) CU(cudaEventRecord(c->ev_fold_done, fold_on));
     }
@@ -1035,7 +1035,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
         const uint32_t i = plan.node_of_slot[s];
         uint32_t f = (flags ? (flags[i] & FYX_NODE_INPUT_MASK) : def_flags) | F_DIRTY_SELF;
         if (i == root) f |= F_ROOT;
-        if (i < c->skinned_node.size() && c->skinned_node[i]) f |= F_SKINNED;
+        if (c->skin.is_skinned(i)) f |= F_SKINNED;
         h_flags[s] = f;
         n_renderable += (f & FYX_NODE_RENDERABLE) ? 1u : 0u;
         if (f & FYX_NODE_STATIC_BATCH) static_batch.push_back(i);
@@ -1143,6 +1143,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     c->shadow_cull.topology_changed();
     c->observer_cull.topology_changed();
     c->dyn.topology_changed(c);
+    c->skin.topology_changed();
 
     // the tables derived from them, which address nodes by slot
     c->light_table_dirty = true;
@@ -1150,7 +1151,6 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     c->ms_dirty = c->have_ms;
     c->pr_dirty = true;
     c->anim_csr_dirty = true;
-    c->tables_dirty = true; // bone slots
     if (!same_capacity) c->dfs_rank.clear(); // indexed by node: stays valid while the pool capacity does
     c->rank_on_device = false;
     ++c->hier_epoch;
@@ -1164,7 +1164,7 @@ extern "C" int32_t fyx_set_dfs_order(fyx_ctx *c, uint32_t capacity, const uint32
     if (preorder_rank) c->dfs_rank.assign(preorder_rank, preorder_rank + capacity);
     else c->dfs_rank.clear();
     c->rank_on_device = false;
-    c->tables_dirty = true;
+    c->skin.dirty = true; // late bones
     c->dyn.invalidate();
     return FYX_OK;
 }
@@ -1283,170 +1283,70 @@ extern "C" int32_t fyx_set_local_aabbs(fyx_ctx *c, uint32_t count, const uint32_
 // --------------------------------------------------------------------------------------------
 namespace {
 
-int32_t grow_vertex_streams(fyx_ctx *c, uint64_t need)
+int32_t Skinning::grow(fyx_ctx *c, uint32_t entries, uint64_t verts)
 {
-    if (need <= c->vert_cap) return FYX_OK;
     int32_t rc;
-    const uint64_t blocks = (need + 127) / 128 + 1; // 128-vertex blocks of 11 x 512 B
-    if ((rc = dev_ensure(c, c->b_vblk, blocks * kVblkStride * sizeof(float4), true))) return rc;
-    if ((rc = dev_ensure(c, c->b_vflag, blocks, true))) return rc;
-    if ((rc = dev_ensure(c, c->b_opos, need * 12, true))) return rc;
-    if ((rc = dev_ensure(c, c->b_onrm, need * 12, true))) return rc;
-    c->vert_cap = std::min<uint64_t>({(c->b_vblk.bytes / (kVblkStride * sizeof(float4)) - 1) * 128, (c->b_vflag.bytes - 1) * 128,
-                                      c->b_opos.bytes / 12, c->b_onrm.bytes / 12});
+    if (entries > entry_cap) {
+        for (int k = 0; k < 3; ++k)
+            if ((rc = dev_ensure(c, b_ib[k], (size_t)entries * 16, true))) return rc;
+        if ((rc = dev_ensure(c, b_palette, (size_t)entries * 64, true))) return rc;
+        entry_cap = (uint32_t)std::min<size_t>({b_ib[0].bytes / 16, b_ib[1].bytes / 16, b_ib[2].bytes / 16, b_palette.bytes / 64});
+    }
+    if (verts > vert_cap) {
+        const uint64_t blocks = (verts + 127) / 128 + 1; // 128-vertex blocks of 11 x 512 B
+        if ((rc = dev_ensure(c, b_vblk, blocks * kVblkStride * sizeof(float4), true))) return rc;
+        if ((rc = dev_ensure(c, b_vflag, blocks, true))) return rc;
+        if ((rc = dev_ensure(c, b_opos, verts * 12, true))) return rc;
+        if ((rc = dev_ensure(c, b_onrm, verts * 12, true))) return rc;
+        vert_cap = std::min<uint64_t>({(b_vblk.bytes / (kVblkStride * sizeof(float4)) - 1) * 128, (b_vflag.bytes - 1) * 128, b_opos.bytes / 12,
+                                       b_onrm.bytes / 12});
+    }
     return FYX_OK;
 }
 
-int32_t grow_bone_tables(fyx_ctx *c, uint32_t need)
+SkinArrays Skinning::arrays() const
 {
-    if (need <= c->entry_cap) return FYX_OK;
-    int32_t rc;
-    for (int k = 0; k < 3; ++k)
-        if ((rc = dev_ensure(c, c->b_ib[k], (size_t)need * 16, true))) return rc;
-    if ((rc = dev_ensure(c, c->b_palette, (size_t)need * 64, true))) return rc;
-    c->entry_cap = (uint32_t)std::min<size_t>({c->b_ib[0].bytes / 16, c->b_ib[1].bytes / 16, c->b_ib[2].bytes / 16, c->b_palette.bytes / 64});
+    return SkinArrays{n_entries, b_bone_slot.as<uint32_t>(), {b_ib[0].as<float4>(), b_ib[1].as<float4>(), b_ib[2].as<float4>()}, b_palette.as<float>(),
+                      b_vblk.as<float4>(), b_opos.as<float>(), b_onrm.as<float>(), b_bs.as<uint2>(), b_bs_w.as<float>()};
+}
+
+FoldArrays Skinning::fold() const
+{
+    return FoldArrays{n_fold, b_fold_node.as<uint32_t>(), b_fold_begin.as<uint32_t>(), b_fold_bone.as<uint32_t>(),
+                      n_late ? b_fold_stale_idx.as<uint32_t>() : nullptr, n_late ? b_stale_pos.as<float4>() : nullptr};
+}
+
+// `v` into `b`, sized for at least one element; the stream has finished reading `b`
+template <class T> int32_t upload(fyx_ctx *c, DevBuf &b, const std::vector<T> &v)
+{
+    if (int32_t rc = dev_ensure(c, b, std::max<size_t>(v.size(), 1) * sizeof(T))) return rc;
+    if (!v.empty()) CU(cudaMemcpy(b.p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
     return FYX_OK;
 }
 
-void rebuild_skin_arrays(fyx_ctx *c)
+int32_t Skinning::commit(fyx_ctx *c)
 {
-    SkinArrays &sk = c->sk;
-    sk.n_entries = c->n_entries;
-    sk.bone_slot = c->b_bone_slot.as<uint32_t>();
-    for (int k = 0; k < 3; ++k) sk.ib[k] = c->b_ib[k].as<float4>();
-    sk.palette = c->b_palette.as<float>();
-    sk.vblk = c->b_vblk.as<float4>();
-    sk.opos = c->b_opos.as<float>();
-    sk.onrm = c->b_onrm.as<float>();
-    sk.bs = c->b_bs.as<uint2>();
-    sk.bs_w = c->b_bs_w.as<float>();
-}
-
-constexpr uint32_t kTileQuads = 2048; // up to 8192 vertices per tile (a 5k-vertex surface is one tile)
-
-// (re)build bone-slot, fold and tile tables from the host-side surface list
-int32_t commit_surfaces(fyx_ctx *c)
-{
-    if (!c->tables_dirty) return FYX_OK;
+    if (!dirty) return FYX_OK;
     if (int32_t rc = topology_check(c)) return rc;
-    const size_t ns = c->surfaces.size();
-    std::vector<uint32_t> bone_slot(c->n_entries);
-    std::vector<SkinTile> tiles;
-    // per skinned node: bones of all its surfaces in surface order
-    std::vector<uint32_t> fold_node, fold_begin, fold_bone;
-    std::vector<int64_t> fold_of_node; // node → index in fold_node, built in first-surface order
-    std::vector<std::vector<uint32_t>> per_node_bones, per_node_bone_nodes;
-    std::vector<uint32_t> fold_mesh_node;
-    fold_of_node.assign(c->n_nodes, -1);
-    for (size_t s = 0; s < ns; ++s) {
-        const Surface &sf = c->surfaces[s];
-        for (uint32_t b = 0; b < sf.n_bones; ++b) {
-            const uint32_t bn = sf.bones[b];
-            bone_slot[sf.bone_off + b] = (bn < c->n_nodes) ? c->slot_of_node[bn] : FYX_NONE;
-        }
-        if (sf.n_verts) {
-            const uint32_t quads = (sf.n_verts + 3) / 4;
-            const uint32_t nt = (quads + kTileQuads - 1) / kTileQuads;
-            const uint32_t per = (quads + nt - 1) / nt;
-            for (uint32_t t = 0; t < nt; ++t) {
-                SkinTile tl{};
-                tl.bone_off = sf.bone_off;
-                tl.n_bones = sf.n_bones;
-                tl.quad_start = (uint32_t)(sf.vert_off / 4 + (uint64_t)t * per);
-                tl.n_quads = std::min(per, quads - t * per);
-                tl.n_shapes = sf.n_shapes;
-                tl.bs_off = (uint32_t)sf.bs_off;
-                tl.bs_blocks = sf.bs_blocks;
-                tl.w_off = sf.w_off;
-                tl.local_quad0 = t * per;
-                tiles.push_back(tl);
-            }
-        }
-        if (sf.n_bones && sf.mesh_node < c->n_nodes && c->slot_of_node[sf.mesh_node] != FYX_NONE) {
-            int64_t &fi = fold_of_node[sf.mesh_node];
-            if (fi < 0) {
-                fi = (int64_t)per_node_bones.size();
-                per_node_bones.emplace_back();
-                per_node_bone_nodes.emplace_back();
-                fold_node.push_back(c->slot_of_node[sf.mesh_node]);
-                fold_mesh_node.push_back(sf.mesh_node);
-            }
-            for (uint32_t b = 0; b < sf.n_bones; ++b) {
-                per_node_bones[fi].push_back(bone_slot[sf.bone_off + b]);
-                per_node_bone_nodes[fi].push_back(sf.bones[b]);
-            }
-        }
-    }
-    fold_begin.push_back(0);
-    // bones visited after their mesh by the reference's DFS (needs fyx_set_dfs_order) keep their pre-update position
-    std::vector<uint32_t> stale_idx, late_slot;
-    const bool have_rank = c->dfs_rank.size() == c->n_nodes && c->n_nodes > 0;
-    for (size_t m = 0; m < per_node_bones.size(); ++m) {
-        const auto &v = per_node_bones[m];
-        for (size_t k = 0; k < v.size(); ++k) {
-            uint32_t si = FYX_NONE;
-            const uint32_t bn = per_node_bone_nodes[m][k];
-            if (have_rank && v[k] != FYX_NONE && c->dfs_rank[bn] > c->dfs_rank[fold_mesh_node[m]]) {
-                si = (uint32_t)late_slot.size();
-                late_slot.push_back(v[k]);
-            }
-            stale_idx.push_back(si);
-        }
-        fold_bone.insert(fold_bone.end(), v.begin(), v.end());
-        fold_begin.push_back((uint32_t)fold_bone.size());
-    }
-    int32_t rc;
-    if ((rc = dev_ensure(c, c->b_bone_slot, std::max<size_t>(bone_slot.size(), 1) * 4))) return rc;
-    if ((rc = dev_ensure(c, c->b_tiles, std::max<size_t>(tiles.size(), 1) * sizeof(SkinTile)))) return rc;
-    if ((rc = dev_ensure(c, c->b_fold_node, std::max<size_t>(fold_node.size(), 1) * 4))) return rc;
-    if ((rc = dev_ensure(c, c->b_fold_begin, fold_begin.size() * 4))) return rc;
-    if ((rc = dev_ensure(c, c->b_fold_bone, std::max<size_t>(fold_bone.size(), 1) * 4))) return rc;
+    const SkinPlan p = plan_skin(surfaces, c->slot_of_node, c->n_slots, dfs_rank_of(c));
+    static_assert(sizeof(SurfBones) == sizeof(uint2), "a palette range is the uint2 the bone-block kernels read");
     CU(cudaStreamSynchronize(c->stream));
-    if (!bone_slot.empty()) CU(cudaMemcpy(c->b_bone_slot.p, bone_slot.data(), bone_slot.size() * 4, cudaMemcpyHostToDevice));
-    if (!tiles.empty()) CU(cudaMemcpy(c->b_tiles.p, tiles.data(), tiles.size() * sizeof(SkinTile), cudaMemcpyHostToDevice));
-    launch_tile_vcode(c->stream, c->b_tiles.as<SkinTile>(), (uint32_t)tiles.size(), c->b_vflag.as<uint8_t>());
-    if (!fold_node.empty()) CU(cudaMemcpy(c->b_fold_node.p, fold_node.data(), fold_node.size() * 4, cudaMemcpyHostToDevice));
-    CU(cudaMemcpy(c->b_fold_begin.p, fold_begin.data(), fold_begin.size() * 4, cudaMemcpyHostToDevice));
-    if (!fold_bone.empty()) CU(cudaMemcpy(c->b_fold_bone.p, fold_bone.data(), fold_bone.size() * 4, cudaMemcpyHostToDevice));
-    {   // node -> its first skinned surface, surface -> its palette range (fyx_pack_bone_matrices)
-        std::vector<uint32_t> surf_of_slot(std::max<uint32_t>(c->n_slots, 1), FYX_NONE);
-        std::vector<uint2> surf_bones(std::max<size_t>(ns, 1));
-        for (size_t si = 0; si < ns; ++si) {
-            const Surface &sf = c->surfaces[si];
-            surf_bones[si] = make_uint2(sf.bone_off, sf.n_bones);
-            if (!sf.n_bones || sf.mesh_node >= c->n_nodes) continue;
-            const uint32_t sl = c->slot_of_node[sf.mesh_node];
-            if (sl != FYX_NONE && surf_of_slot[sl] == FYX_NONE) surf_of_slot[sl] = (uint32_t)si;
-        }
-        if ((rc = dev_ensure(c, c->b_surf_of_slot, surf_of_slot.size() * 4))) return rc;
-        if ((rc = dev_ensure(c, c->b_surf_bones, surf_bones.size() * sizeof(uint2)))) return rc;
-        CU(cudaMemcpy(c->b_surf_of_slot.p, surf_of_slot.data(), surf_of_slot.size() * 4, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(c->b_surf_bones.p, surf_bones.data(), surf_bones.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+    int32_t rc;
+    if ((rc = upload(c, b_bone_slot, p.bone_slot)) || (rc = upload(c, b_tiles, p.tiles)) || (rc = upload(c, b_fold_node, p.fold_node)) ||
+        (rc = upload(c, b_fold_begin, p.fold_begin)) || (rc = upload(c, b_fold_bone, p.fold_bone)) ||
+        (rc = upload(c, b_surf_of_slot, p.surf_of_slot)) || (rc = upload(c, b_surf_bones, p.surf_bones)))
+        return rc;
+    if (!p.late_slot.empty()) {
+        if ((rc = upload(c, b_fold_stale_idx, p.stale_idx)) || (rc = upload(c, b_late_slot, p.late_slot))) return rc;
+        if ((rc = dev_ensure(c, b_stale_pos, p.late_slot.size() * sizeof(float4)))) return rc;
     }
-    c->n_tiles = (uint32_t)tiles.size();
-    c->any_blend_shapes = false;
-    for (const Surface &sf : c->surfaces) c->any_blend_shapes |= sf.n_shapes != 0 && sf.n_verts != 0;
-    c->max_bones = 0;
-    for (const Surface &sf : c->surfaces)
-        if (sf.n_verts) c->max_bones = std::max(c->max_bones, sf.n_bones);
-    c->fold.n = (uint32_t)fold_node.size();
-    c->fold.node_slot = c->b_fold_node.as<uint32_t>();
-    c->fold.bone_begin = c->b_fold_begin.as<uint32_t>();
-    c->fold.bone_slot = c->b_fold_bone.as<uint32_t>();
-    c->n_late = (uint32_t)late_slot.size();
-    c->fold.stale_idx = nullptr;
-    c->fold.stale_pos = nullptr;
-    if (c->n_late) {
-        if ((rc = dev_ensure(c, c->b_fold_stale_idx, stale_idx.size() * 4))) return rc;
-        if ((rc = dev_ensure(c, c->b_late_slot, late_slot.size() * 4))) return rc;
-        if ((rc = dev_ensure(c, c->b_stale_pos, late_slot.size() * sizeof(float4)))) return rc;
-        CU(cudaMemcpy(c->b_fold_stale_idx.p, stale_idx.data(), stale_idx.size() * 4, cudaMemcpyHostToDevice));
-        CU(cudaMemcpy(c->b_late_slot.p, late_slot.data(), late_slot.size() * 4, cudaMemcpyHostToDevice));
-        c->fold.stale_idx = c->b_fold_stale_idx.as<uint32_t>();
-        c->fold.stale_pos = c->b_stale_pos.as<float4>();
-    }
-    rebuild_skin_arrays(c);
-    c->tables_dirty = false;
+    launch_tile_vcode(c->stream, b_tiles.as<SkinTile>(), (uint32_t)p.tiles.size(), b_vflag.as<uint8_t>());
+    n_tiles = (uint32_t)p.tiles.size();
+    n_fold = (uint32_t)p.fold_node.size();
+    n_late = (uint32_t)p.late_slot.size();
+    max_bones = p.max_bones;
+    any_blend_shapes = p.any_blend_shapes;
+    dirty = false;
     return FYX_OK;
 }
 
@@ -1470,53 +1370,49 @@ extern "C" int32_t fyx_add_skinned_surface(fyx_ctx *c, uint32_t mesh_node, uint3
             return fail(c, FYX_ERR_INVALID_ARGUMENT, "vertex attribute outside the vertex");
     }
     CU(cudaSetDevice(c->device));
-    Surface sf;
+    Skinning &sk = c->skin;
+    SkinSurface sf;
     sf.mesh_node = mesh_node;
-    sf.n_bones = n_bones;
-    sf.bone_off = c->n_entries;
-    sf.n_verts = n_verts;
-    sf.vert_off = c->n_verts_total;
     sf.bones.assign(bone_nodes, bone_nodes + n_bones);
-    int32_t rc;
-    if ((rc = grow_bone_tables(c, c->n_entries + n_bones))) return rc;
+    sf.bone_off = sk.n_entries;
+    sf.n_verts = n_verts;
+    sf.vert_off = sk.n_verts;
     const uint64_t padded = ((uint64_t)n_verts + 3) & ~uint64_t(3);
-    if ((rc = grow_vertex_streams(c, c->n_verts_total + padded))) return rc;
-    rebuild_skin_arrays(c);
+    int32_t rc;
+    if ((rc = sk.grow(c, sk.n_entries + n_bones, sk.n_verts + padded))) return rc;
     if (n_bones) {
         void *d_m = nullptr;
         if ((rc = stage_to_device(c, inv_bind, (size_t)n_bones * 64, nullptr, 0, false, &d_m, nullptr))) return rc;
-        launch_ib_rows(c->stream, n_bones, static_cast<const float *>(d_m), c->b_ib[0].as<float4>() + sf.bone_off,
-                       c->b_ib[1].as<float4>() + sf.bone_off, c->b_ib[2].as<float4>() + sf.bone_off, c->d_err.as<uint32_t>());
+        launch_ib_rows(c->stream, n_bones, static_cast<const float *>(d_m), sk.b_ib[0].as<float4>() + sf.bone_off,
+                       sk.b_ib[1].as<float4>() + sf.bone_off, sk.b_ib[2].as<float4>() + sf.bone_off, c->d_err.as<uint32_t>());
         c->launches++;
     }
     if (n_verts) {
         void *d_v = nullptr;
         if ((rc = stage_to_device(c, verts, (size_t)n_verts * layout->stride, nullptr, 0, false, &d_v, nullptr))) return rc;
-        if (n_bones > kSkinRingMaxBones && !c->vblk_raw) { // k_skin's register-load form reads raw blocks
-            launch_vdecode_all(c->stream, c->b_vblk.as<float4>(), c->b_vflag.as<uint8_t>(), (c->n_verts_total + 127) / 128);
-            c->vblk_raw = true;
+        if (n_bones > kSkinRingMaxBones && !sk.vblk_raw) { // k_skin's register-load form reads raw blocks
+            launch_vdecode_all(c->stream, sk.b_vblk.as<float4>(), sk.b_vflag.as<uint8_t>(), (sk.n_verts + 127) / 128);
+            sk.vblk_raw = true;
         }
-        launch_deinterleave(c->stream, n_verts, static_cast<const unsigned char *>(d_v), *layout, n_bones, c->b_vblk.as<float4>(),
-                            c->b_vflag.as<uint8_t>(), !c->vblk_raw, sf.vert_off, c->d_err.as<uint32_t>());
+        launch_deinterleave(c->stream, n_verts, static_cast<const unsigned char *>(d_v), *layout, n_bones, sk.b_vblk.as<float4>(),
+                            sk.b_vflag.as<uint8_t>(), !sk.vblk_raw, sf.vert_off, c->d_err.as<uint32_t>());
         c->launches++;
     }
     CU(cudaGetLastError());
-    c->n_entries += n_bones;
-    c->n_verts_total += padded;
-    if (n_bones && mesh_node < c->n_nodes) {
-        if (c->skinned_node.size() < c->n_nodes) c->skinned_node.resize(c->n_nodes, 0);
-        if (!c->skinned_node[mesh_node]) {
-            c->skinned_node[mesh_node] = 1;
-            const uint32_t slot = c->slot_of_node[mesh_node];
-            if (slot != FYX_NONE) {
-                launch_or_u32(c->stream, c->a.flags + slot, F_SKINNED | F_DIRTY_SELF);
-                c->launches++;
-            }
+    sk.n_entries += n_bones;
+    sk.n_verts += padded;
+    if (n_bones && mesh_node < c->n_nodes && !sk.is_skinned(mesh_node)) {
+        if (sk.skinned_node.size() < c->n_nodes) sk.skinned_node.resize(c->n_nodes, 0);
+        sk.skinned_node[mesh_node] = 1;
+        const uint32_t slot = c->slot_of_node[mesh_node];
+        if (slot != FYX_NONE) {
+            launch_or_u32(c->stream, c->a.flags + slot, F_SKINNED | F_DIRTY_SELF);
+            c->launches++;
         }
     }
-    if (out_id) *out_id = (uint32_t)c->surfaces.size();
-    c->surfaces.push_back(std::move(sf));
-    c->tables_dirty = true;
+    if (out_id) *out_id = (uint32_t)sk.surfaces.size();
+    sk.surfaces.push_back(std::move(sf));
+    sk.dirty = true;
     return FYX_OK;
 }
 
@@ -1525,13 +1421,14 @@ extern "C" int32_t fyx_add_skinned_surface(fyx_ctx *c, uint32_t mesh_node, uint3
 extern "C" int32_t fyx_set_blend_shapes(fyx_ctx *c, uint32_t sid, uint32_t n_shapes, const void *records, uint32_t layer_stride, const float *weights)
 {
     if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (sid >= c->surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
+    Skinning &sk = c->skin;
+    if (sid >= sk.surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
     if (n_shapes > FYX_MAX_BLEND_SHAPES) return fail(c, FYX_ERR_INVALID_ARGUMENT, "n_shapes %u > %u", n_shapes, FYX_MAX_BLEND_SHAPES);
-    Surface &sf = c->surfaces[sid];
+    SkinSurface &sf = sk.surfaces[sid];
     if (n_shapes && !records) return fail(c, FYX_ERR_INVALID_ARGUMENT, "records are NULL");
     if (n_shapes && layer_stride < sf.n_verts) return fail(c, FYX_ERR_INVALID_ARGUMENT, "layer_stride %u < the surface's %u vertices", layer_stride, sf.n_verts);
     CU(cudaSetDevice(c->device));
-    c->tables_dirty = true;
+    sk.dirty = true;
     if (!n_shapes || !sf.n_verts) {
         sf.n_shapes = 0;
         return FYX_OK;
@@ -1541,28 +1438,27 @@ extern "C" int32_t fyx_set_blend_shapes(fyx_ctx *c, uint32_t sid, uint32_t n_sha
     if (need > 0xFFFFFFFFull) return fail(c, FYX_ERR_INVALID_ARGUMENT, "too much blend-shape data");
     int32_t rc;
     if (need > sf.bs_cap) { // a new region at the end (an earlier, smaller region of this surface is abandoned)
-        if (c->bs_used + need > 0xFFFFFFFFull) return fail(c, FYX_ERR_OUT_OF_MEMORY, "blend-shape storage exhausted");
-        if ((rc = dev_ensure(c, c->b_bs, (c->bs_used + need) * kBsBlockU2 * sizeof(uint2), true))) return rc;
-        sf.bs_off = c->bs_used;
+        if (sk.bs_used + need > 0xFFFFFFFFull) return fail(c, FYX_ERR_OUT_OF_MEMORY, "blend-shape storage exhausted");
+        if ((rc = dev_ensure(c, sk.b_bs, (sk.bs_used + need) * kBsBlockU2 * sizeof(uint2), true))) return rc;
+        sf.bs_off = sk.bs_used;
         sf.bs_cap = (uint32_t)need;
-        c->bs_used += need;
+        sk.bs_used += need;
     }
     if (n_shapes > sf.w_cap) {
-        if ((rc = dev_ensure(c, c->b_bs_w, (size_t)(c->bs_w_used + n_shapes) * sizeof(float), true))) return rc;
-        sf.w_off = c->bs_w_used;
+        if ((rc = dev_ensure(c, sk.b_bs_w, (size_t)(sk.bs_w_used + n_shapes) * sizeof(float), true))) return rc;
+        sf.w_off = sk.bs_w_used;
         sf.w_cap = n_shapes;
-        c->bs_w_used += n_shapes;
+        sk.bs_w_used += n_shapes;
     }
     sf.n_shapes = n_shapes;
     sf.bs_blocks = bs_blocks;
-    rebuild_skin_arrays(c);
     std::vector<float> w(n_shapes);
     for (uint32_t i = 0; i < n_shapes; ++i) w[i] = (weights ? weights[i] : 100.0f) / 100.0f; // bs.weight / 100.0 (mesh/mod.rs:797)
     void *d_rec = nullptr, *d_w = nullptr;
     if ((rc = stage_to_device(c, records, (size_t)n_shapes * layer_stride * 18, w.data(), (size_t)n_shapes * 4, false, &d_rec, &d_w))) return rc;
-    launch_bs_layout(c->stream, sf.n_verts, n_shapes, layer_stride, static_cast<const uint16_t *>(d_rec), c->b_bs.as<uint2>() + sf.bs_off * kBsBlockU2, bs_blocks);
+    launch_bs_layout(c->stream, sf.n_verts, n_shapes, layer_stride, static_cast<const uint16_t *>(d_rec), sk.b_bs.as<uint2>() + sf.bs_off * kBsBlockU2, bs_blocks);
     c->launches++;
-    CU(cudaMemcpyAsync(c->b_bs_w.as<float>() + sf.w_off, d_w, (size_t)n_shapes * 4, cudaMemcpyDeviceToDevice, c->stream));
+    CU(cudaMemcpyAsync(sk.b_bs_w.as<float>() + sf.w_off, d_w, (size_t)n_shapes * 4, cudaMemcpyDeviceToDevice, c->stream));
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(c->stream)); // `w` and the staging buffer are free again
     return FYX_OK;
@@ -1571,8 +1467,9 @@ extern "C" int32_t fyx_set_blend_shapes(fyx_ctx *c, uint32_t sid, uint32_t n_sha
 extern "C" int32_t fyx_set_blend_shape_weights(fyx_ctx *c, uint32_t sid, uint32_t n, const float *weights)
 {
     if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (sid >= c->surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
-    Surface &sf = c->surfaces[sid];
+    Skinning &sk = c->skin;
+    if (sid >= sk.surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
+    SkinSurface &sf = sk.surfaces[sid];
     if (n != sf.n_shapes) return fail(c, FYX_ERR_INVALID_ARGUMENT, "the surface has %u blend shapes, %u weights given", sf.n_shapes, n);
     if (!n) return FYX_OK;
     if (!weights) return fail(c, FYX_ERR_INVALID_ARGUMENT, "weights are NULL");
@@ -1582,7 +1479,7 @@ extern "C" int32_t fyx_set_blend_shape_weights(fyx_ctx *c, uint32_t sid, uint32_
     void *d_w = nullptr;
     int32_t rc = stage_to_device(c, w.data(), (size_t)n * 4, nullptr, 0, false, &d_w, nullptr);
     if (rc) return rc;
-    CU(cudaMemcpyAsync(c->b_bs_w.as<float>() + sf.w_off, d_w, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
+    CU(cudaMemcpyAsync(sk.b_bs_w.as<float>() + sf.w_off, d_w, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return FYX_OK;
 }
@@ -1592,20 +1489,15 @@ extern "C" int32_t fyx_reserve_skinning(fyx_ctx *c, uint64_t total_bones, uint64
     if (!c) return FYX_ERR_INVALID_ARGUMENT;
     if (total_bones > 0xFFFFFFFFull) return fail(c, FYX_ERR_INVALID_ARGUMENT, "too many bones");
     CU(cudaSetDevice(c->device));
-    int32_t rc = grow_bone_tables(c, (uint32_t)total_bones);
-    if (rc) return rc;
     // every surface is padded to a multiple of 4 vertices: leave room for 3 per surface (bounded by bones)
-    rc = grow_vertex_streams(c, total_verts + 4 * total_bones + 4);
-    if (rc) return rc;
-    rebuild_skin_arrays(c);
-    return FYX_OK;
+    return c->skin.grow(c, (uint32_t)total_bones, total_verts + 4 * total_bones + 4);
 }
 
 extern "C" int32_t fyx_commit_surfaces(fyx_ctx *c)
 {
     if (!c) return FYX_ERR_INVALID_ARGUMENT;
     CU(cudaSetDevice(c->device));
-    int32_t rc = commit_surfaces(c);
+    int32_t rc = c->skin.commit(c);
     if (rc) return rc;
     return sync_and_check(c);
 }
@@ -1627,7 +1519,7 @@ int32_t update_cull_enqueue(fyx_ctx *c, uint32_t update_flags, uint32_t nf, bool
         return !(e && *e == '0');
     }();
     const bool unf = unfused_cull(c, nf);
-    const bool side = side_fold_wanted && side_fold_allowed && !unf && c->fold.n;
+    const bool side = side_fold_wanted && side_fold_allowed && !unf && c->skin.n_fold;
     if (side_fold) *side_fold = side;
     int32_t rc = run_update(c, update_flags, (nf && !unf) ? &c->cp : nullptr, side ? c->fold_stream.h : nullptr);
     if (rc) return rc;
@@ -1637,16 +1529,17 @@ int32_t update_cull_enqueue(fyx_ctx *c, uint32_t update_flags, uint32_t nf, bool
 // the bones' skinning matrices (palettes)
 void palette_enqueue(fyx_ctx *c, cudaStream_t s)
 {
-    if (c->sk.n_entries) {
-        launch_palette(s, c->a, c->sk);
+    if (c->skin.n_entries) {
+        launch_palette(s, c->a, c->skin.arrays());
         c->launches++;
     }
 }
 
 void skin_enqueue(fyx_ctx *c, cudaStream_t s)
 {
-    if (c->n_tiles) {
-        launch_skin(s, c->sk, c->b_tiles.as<SkinTile>(), c->n_tiles, c->max_bones, c->any_blend_shapes);
+    const Skinning &sk = c->skin;
+    if (sk.n_tiles) {
+        launch_skin(s, sk.arrays(), sk.b_tiles.as<SkinTile>(), sk.n_tiles, sk.max_bones, sk.any_blend_shapes);
         c->launches++;
     }
 }
@@ -1668,7 +1561,7 @@ template <class Enqueue> int32_t run_timed(fyx_ctx *c, int ev_end, float &ms, En
 extern "C" int32_t fyx_update_transforms(fyx_ctx *c, uint32_t update_flags)
 {
     int32_t rc;
-    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    if ((rc = enter(c)) || (rc = c->skin.commit(c))) return rc;
     return run_timed(c, EV_UPDATE, c->timings.update_ms, [&] { return update_cull_enqueue(c, update_flags, 0); });
 }
 
@@ -1687,7 +1580,7 @@ extern "C" int32_t fyx_update_and_cull(fyx_ctx *c, uint32_t update_flags, uint32
                                        const uint32_t *cam_mask, const uint32_t *pass_flags)
 {
     int32_t rc;
-    if ((rc = enter(c)) || (rc = commit_surfaces(c)) || (rc = cull_prune_prepare(c, nf))) return rc;
+    if ((rc = enter(c)) || (rc = c->skin.commit(c)) || (rc = cull_prune_prepare(c, nf))) return rc;
     return run_timed(c, EV_UPDATE, c->timings.update_ms, [&] {
         return (rc = prepare_cull(c, nf, fr, cam_mask, pass_flags)) ? rc : update_cull_enqueue(c, update_flags, nf);
     });
@@ -1720,7 +1613,7 @@ extern "C" int32_t fyx_get_visible_device(fyx_ctx *c, uint32_t f, const uint32_t
 extern "C" int32_t fyx_build_palettes(fyx_ctx *c)
 {
     int32_t rc;
-    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    if ((rc = enter(c)) || (rc = c->skin.commit(c))) return rc;
     return run_timed(c, EV_PALETTE, c->timings.palette_ms, [&] {
         palette_enqueue(c, c->stream);
         return FYX_OK;
@@ -1730,7 +1623,7 @@ extern "C" int32_t fyx_build_palettes(fyx_ctx *c)
 extern "C" int32_t fyx_skin(fyx_ctx *c)
 {
     int32_t rc;
-    if ((rc = enter(c)) || (rc = commit_surfaces(c))) return rc;
+    if ((rc = enter(c)) || (rc = c->skin.commit(c))) return rc;
     return run_timed(c, EV_SKIN, c->timings.skin_ms, [&] {
         skin_enqueue(c, c->stream);
         return FYX_OK;
@@ -1813,7 +1706,7 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
     if (!c || !fr) return FYX_ERR_INVALID_ARGUMENT;
     if (fr->struct_size < offsetof(fyx_frame_desc, do_animate)) return fail(c, FYX_ERR_INVALID_ARGUMENT, "fyx_frame_desc.struct_size too small");
     int32_t rc;
-    if ((rc = enter(c)) || (rc = commit_surfaces(c)) || (rc = cull_prune_prepare(c, fr->n_frusta))) return rc;
+    if ((rc = enter(c)) || (rc = c->skin.commit(c)) || (rc = cull_prune_prepare(c, fr->n_frusta))) return rc;
     cudaStream_t s = c->stream;
     CU(cudaEventRecord(c->ev[EV_START], s));
     // 0. animation players tick before Graph::update (N2): curves are device-resident, nothing to upload
@@ -1837,7 +1730,7 @@ extern "C" int32_t fyx_render_prep(fyx_ctx *c, const fyx_frame_desc *fr)
         if (rc) return rc;
     }
     bool side_fold = false;
-    if ((rc = update_cull_enqueue(c, fr->update_flags, fr->n_frusta, async && fr->do_skin && c->n_tiles, &side_fold))) return rc;
+    if ((rc = update_cull_enqueue(c, fr->update_flags, fr->n_frusta, async && fr->do_skin && c->skin.n_tiles, &side_fold))) return rc;
     if (stage_events) CU(cudaEventRecord(c->ev[EV_UPDATE], s));
     c->ev_levels_prev = nullptr;
     if (fr->n_frusta && (async || (fr->flags & FYX_FRAME_ALLGATHER))) {
@@ -2001,11 +1894,11 @@ extern "C" int32_t fyx_get_global_flags(fyx_ctx *c, uint32_t count, const uint32
 extern "C" int32_t fyx_get_palette(fyx_ctx *c, uint32_t sid, float *out)
 {
     if (!c || !out) return FYX_ERR_INVALID_ARGUMENT;
-    if (sid >= c->surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
+    if (sid >= c->skin.surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
     CU(cudaSetDevice(c->device));
-    const Surface &sf = c->surfaces[sid];
-    if (!sf.n_bones) return FYX_OK;
-    CU(cudaMemcpyAsync(out, c->b_palette.as<float>() + 16 * (size_t)sf.bone_off, (size_t)sf.n_bones * 64, cudaMemcpyDeviceToHost, c->stream));
+    const SkinSurface &sf = c->skin.surfaces[sid];
+    if (!sf.n_bones()) return FYX_OK;
+    CU(cudaMemcpyAsync(out, c->skin.b_palette.as<float>() + 16 * (size_t)sf.bone_off, (size_t)sf.n_bones() * 64, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return FYX_OK;
 }
@@ -2013,12 +1906,12 @@ extern "C" int32_t fyx_get_palette(fyx_ctx *c, uint32_t sid, float *out)
 extern "C" int32_t fyx_get_skinned(fyx_ctx *c, uint32_t sid, float *out_pos, float *out_nrm)
 {
     if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (sid >= c->surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
+    if (sid >= c->skin.surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
     CU(cudaSetDevice(c->device));
-    const Surface &sf = c->surfaces[sid];
+    const SkinSurface &sf = c->skin.surfaces[sid];
     if (!sf.n_verts) return FYX_OK;
-    if (out_pos) CU(cudaMemcpyAsync(out_pos, c->b_opos.as<float>() + 3 * sf.vert_off, (size_t)sf.n_verts * 12, cudaMemcpyDeviceToHost, c->stream));
-    if (out_nrm) CU(cudaMemcpyAsync(out_nrm, c->b_onrm.as<float>() + 3 * sf.vert_off, (size_t)sf.n_verts * 12, cudaMemcpyDeviceToHost, c->stream));
+    if (out_pos) CU(cudaMemcpyAsync(out_pos, c->skin.b_opos.as<float>() + 3 * sf.vert_off, (size_t)sf.n_verts * 12, cudaMemcpyDeviceToHost, c->stream));
+    if (out_nrm) CU(cudaMemcpyAsync(out_nrm, c->skin.b_onrm.as<float>() + 3 * sf.vert_off, (size_t)sf.n_verts * 12, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return FYX_OK;
 }
@@ -2026,10 +1919,10 @@ extern "C" int32_t fyx_get_skinned(fyx_ctx *c, uint32_t sid, float *out_pos, flo
 extern "C" int32_t fyx_get_skinned_device(fyx_ctx *c, uint32_t sid, const float **d_pos, const float **d_nrm)
 {
     if (!c) return FYX_ERR_INVALID_ARGUMENT;
-    if (sid >= c->surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
-    const Surface &sf = c->surfaces[sid];
-    if (d_pos) *d_pos = c->b_opos.as<float>() + 3 * sf.vert_off;
-    if (d_nrm) *d_nrm = c->b_onrm.as<float>() + 3 * sf.vert_off;
+    if (sid >= c->skin.surfaces.size()) return fail(c, FYX_ERR_INVALID_ARGUMENT, "surface id %u out of range", sid);
+    const SkinSurface &sf = c->skin.surfaces[sid];
+    if (d_pos) *d_pos = c->skin.b_opos.as<float>() + 3 * sf.vert_off;
+    if (d_nrm) *d_nrm = c->skin.b_onrm.as<float>() + 3 * sf.vert_off;
     return FYX_OK;
 }
 

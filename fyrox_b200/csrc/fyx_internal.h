@@ -14,6 +14,7 @@
 
 #include "../../include/fyrox_b200.h"
 #include "fyx_math.cuh"
+#include "fyx_skin_plan.hpp"
 #include "fyx_slots.hpp"
 
 namespace fyx {
@@ -93,19 +94,6 @@ struct SkinArrays {
     const float *bs_w;
 };
 
-struct SkinTile {
-    uint32_t bone_off; // first palette entry of the surface
-    uint32_t n_bones;
-    uint32_t quad_start; // absolute index of the first 4-vertex group
-    uint32_t n_quads;
-    // blend shapes of the surface (n_shapes = 0: none)
-    uint32_t n_shapes;
-    uint32_t bs_off;      // index of (shape 0, block 0) of the surface in units of 192 uint2 (one 1536-byte shape block)
-    uint32_t bs_blocks;   // 128-vertex blocks per shape
-    uint32_t w_off;       // first weight in bs_w
-    uint32_t local_quad0; // the tile's first group relative to the surface's first group
-    uint32_t vcoded[3];   // bit s: block quad_start / 32 + s is coded (fyx_vcode.cuh); a tile spans at most 65 blocks
-};
 constexpr uint32_t kBsBlockU2 = 6 * 32; // uint2 per (shape, block)
 void launch_bs_layout(cudaStream_t s, uint32_t n_verts, uint32_t n_shapes, uint32_t layer_stride, const uint16_t *d_records, uint2 *d_dst, uint32_t bs_blocks);
 

@@ -35,7 +35,7 @@ LAYOUTS = {
 }
 
 MAX_BLEND_SHAPES = 128  # FYX_MAX_BLEND_SHAPES
-TILE_QUADS = 2048  # four-vertex groups per skinning tile (commit_surfaces)
+TILE_QUADS = 2048  # four-vertex groups per skinning tile (kTileQuads, fyx_skin_plan.hpp)
 
 
 @dataclass
@@ -309,7 +309,7 @@ def oracle_skin(pal, sd: SurfaceData, weights_w100=None, verts=None):
 
 
 def tile_starts(specs):
-    """First four-vertex group of every skinning tile when the surfaces are added in this order (commit_surfaces:
+    """First four-vertex group of every skinning tile when the surfaces are added in this order (plan_skin:
     each surface starts at a multiple of 4 vertices, a surface of q groups makes ceil(q / 2048) tiles of
     ceil(q / tiles) groups).  Returns (absolute group, group within the surface) per tile."""
     out, off = [], 0
