@@ -324,8 +324,8 @@ __global__ void __launch_bounds__(kBlock) k_anim_tick(const AnimArrays an, const
 
 } // namespace
 
-void launch_animate(cudaStream_t s, const NodeArrays &a, const AnimArrays &an, fyx_trs *trs_by_slot,
-                    const fyx_transform_statics *st_by_slot, float dt, uint32_t *d_err)
+uint32_t launch_animate(cudaStream_t s, const NodeArrays &a, const AnimArrays &an, fyx_trs *trs_by_slot,
+                        const fyx_transform_statics *st_by_slot, float dt, uint32_t *d_err)
 {
     if (an.n_tracks) k_anim_sample<<<(an.n_tracks + kBlock - 1) / kBlock, kBlock, 0, s>>>(an);
     if (an.n_nodes) {
@@ -334,6 +334,7 @@ void launch_animate(cudaStream_t s, const NodeArrays &a, const AnimArrays &an, f
         else k_anim_apply<false><<<g, kBlock, 0, s>>>(a, an, trs_by_slot, st_by_slot, d_err);
     }
     if (an.n_anims) k_anim_tick<<<(an.n_anims + kBlock - 1) / kBlock, kBlock, 0, s>>>(an, dt);
+    return (an.n_tracks ? 1 : 0) + (an.n_nodes ? 1 : 0) + (an.n_anims ? 1 : 0);
 }
 
 } // namespace fyx

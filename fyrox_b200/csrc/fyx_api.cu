@@ -255,12 +255,6 @@ struct VisSlot {
     Event ev_cull, ev_counts, ev_done;
 };
 
-// N2: one animation on the host side (fyx_anim.inl)
-struct AnimHost {
-    uint32_t first_track = 0, n_tracks = 0, pos_in_group = 0;
-    AnimStateDev st{};
-};
-
 // N3: packed instances in segments, segment after segment (fyx_drawprep.inl): one segment for a camera frustum, one per
 // map for the shadow maps
 struct InstPack {
@@ -393,6 +387,32 @@ struct Skinning {
     FoldArrays fold() const;
 };
 
+// The animations (fyx_anim_add, fyx_anim.inl): what the host reads of each animation and track, the blend groups, the
+// records added since the last flush, and the device tables with the node CSR that plan_anim_nodes (fyx_anim_plan.hpp)
+// derives from the tracks and the topology, which commit rebuilds when `dirty`.  Uploads wait for the first call that needs
+// the device tables: thousands of animations (one per skeleton) arrive back to back at load time.
+struct Animations {
+    std::vector<AnimInfo> anims;
+    std::vector<uint32_t> track_node, track_bk;      // per track, animation after animation: target node, binding | value_kind << 8
+    std::vector<std::vector<uint32_t>> groups;       // sources of blend group g at [g - 1]
+    uint32_t n_keys = 0;
+    std::vector<fyx_curve_key> pend_keys;            // added since the last flush
+    std::vector<AnimTrackDev> pend_tracks;
+    std::vector<AnimStateDev> pend_state;
+    DevBuf b_keys, b_tracks, b_state, b_hints, b_values, b_ok, b_bk, b_node_slot, b_node_begin, b_node_tracks;
+    uint32_t n_nodes = 0; // of the node CSR
+    bool dirty = true;    // the node CSR is out of date
+
+    int32_t add(fyx_ctx *c, const fyx_animation_desc &d, uint32_t *out_id); // checks, then queues
+    int32_t flush(fyx_ctx *c); // uploads the queue (the device tables grow, keeping the older animations' hints and time)
+    int32_t commit(fyx_ctx *c); // flush, then plan_anim_nodes and its upload when dirty
+    int32_t blend_group(fyx_ctx *c, uint32_t n, const uint32_t *ids, const float *weights, uint32_t *out_group);
+    // v into `field` of device record i: the state of animation i, or track i
+    template <class R, class F> int32_t write(fyx_ctx *c, uint32_t i, F R::*field, F v) const;
+    void topology_changed() { dirty = true; } // target slots
+    AnimArrays arrays() const; // what the kernels read, from the buffers as they are now
+};
+
 } // namespace
 
 struct PeerState {
@@ -468,19 +488,7 @@ struct fyx_ctx {
     bool timings_pending = false; // an async frame's events have not been read yet
     bool stage_events_valid = false; // the last frame recorded the per-stage events (synchronous frames only)
 
-    // N2 animation sampling (fyx_anim.inl)
-    std::vector<AnimHost> anims;
-    std::vector<fyx_anim_track> anim_tracks; // all tracks, animation after animation
-    uint32_t n_anim_keys = 0, n_blend_groups = 0;
-    std::vector<std::vector<uint32_t>> blend_groups; // sources of group g at [g - 1]
-    bool anim_csr_dirty = true;
-    std::vector<fyx_curve_key> pend_keys; // queued by fyx_anim_add, uploaded by anim_flush
-    std::vector<AnimTrackDev> pend_tracks;
-    std::vector<uint32_t> pend_bk;
-    std::vector<AnimStateDev> pend_state;
-    AnimArrays an{};
-    DevBuf b_anim_keys, b_anim_tracks, b_anim_state, b_anim_hints, b_anim_values, b_anim_ok, b_anim_bk, b_anim_node_slot,
-        b_anim_node_begin, b_anim_node_tracks;
+    Animations anim; // N2 animation sampling
 
     // N4 LOD filter (fyx_drawprep.inl)
     SlotColumn lod_range{make_float2(NAN, NAN)}; // (begin, end); begin NaN = not a LOD object
@@ -1144,13 +1152,13 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     c->observer_cull.topology_changed();
     c->dyn.topology_changed(c);
     c->skin.topology_changed();
+    c->anim.topology_changed();
 
     // the tables derived from them, which address nodes by slot
     c->light_table_dirty = true;
     c->obs_table_dirty = true;
     c->ms_dirty = c->have_ms;
     c->pr_dirty = true;
-    c->anim_csr_dirty = true;
     if (!same_capacity) c->dfs_rank.clear(); // indexed by node: stays valid while the pool capacity does
     c->rank_on_device = false;
     ++c->hier_epoch;

@@ -14,6 +14,7 @@
 
 #include "../../include/fyrox_b200.h"
 #include "fyx_math.cuh"
+#include "fyx_anim_plan.hpp"
 #include "fyx_skin_plan.hpp"
 #include "fyx_slots.hpp"
 
@@ -108,23 +109,7 @@ struct FoldArrays {
     const float4 *stale_pos;
 };
 
-// N2 animation sampling (fyx_anim.cu)
-struct AnimTrackDev {
-    uint32_t anim;       // owning animation
-    uint32_t value_kind; // FYX_TV_*
-    uint32_t enabled;
-    uint32_t n_curves;
-    uint32_t first_key[4]; // offsets into the context-wide key array
-    uint32_t n_keys[4];
-    float first_loc[4], last_loc[4]; // location of each curve's first / last key (keys are immutable once added): the
-                                     // common in-range fetch touches only the remembered span, not the curve's ends
-};
-struct AnimStateDev {
-    float time, speed, slice_start, slice_end;
-    uint32_t looped, enabled;
-    uint32_t group; // 0 = applied directly (AnimationPlayer, auto_apply); g > 0 = source of blend group g
-    float weight;   // its PoseWeight::Constant inside that group
-};
+// N2 animation sampling (fyx_anim.cu; AnimTrackDev / AnimStateDev in fyx_anim_plan.hpp); launch_animate returns its launches
 struct AnimArrays {
     uint32_t n_tracks, n_anims, n_nodes;
     const fyx_curve_key *keys;
@@ -139,8 +124,8 @@ struct AnimArrays {
     const uint32_t *node_begin;
     const uint32_t *node_tracks;
 };
-void launch_animate(cudaStream_t s, const NodeArrays &a, const AnimArrays &an, fyx_trs *trs_by_slot,
-                    const fyx_transform_statics *st_by_slot, float dt, uint32_t *d_err);
+uint32_t launch_animate(cudaStream_t s, const NodeArrays &a, const AnimArrays &an, fyx_trs *trs_by_slot,
+                        const fyx_transform_statics *st_by_slot, float dt, uint32_t *d_err);
 
 // N3 draw-prep (fyx_drawprep.cu): one frustum's visible list -> instances grouped by bundle
 struct InstParams {
