@@ -79,43 +79,6 @@ struct SlotColumn {
     int32_t scatter(fyx_ctx *c, uint32_t count, const uint32_t *idx, const void *values); // the nodes' records, from the host
 };
 
-// One record per node index, for what the setters keep on the host by node: light sources, CSM options, cameras, reflection
-// probes, node surfaces, pruner marks.  `def` is the record of a node that was never given one.  Across fyx_set_topology a
-// record stays with its node index while the node is alive before and after the call; every other index starts again from
-// `def`, as in the slot columns.
-template <class T> struct NodeRecords {
-    T def;
-    std::vector<T> rec; // by node index; the indices past its end hold `def`
-    explicit NodeRecords(const T &v) : def(v) {}
-    const T &operator[](uint32_t node) const { return node < rec.size() ? rec[node] : def; }
-    void set(uint32_t node, const T &v)
-    {
-        if (node >= rec.size()) rec.resize(node + 1, def);
-        rec[node] = v;
-    }
-    int32_t check(fyx_ctx *c, uint32_t count, const uint32_t *idx) const; // every node listed (idx NULL = 0..count-1) is in range
-    // keep(record) trims a record that stays to what it keeps.  Only the records that restart are written.
-    template <class Keep> void topology_changed(const std::vector<uint32_t> &old_slot_of_node, const std::vector<uint32_t> &new_slot_of_node, Keep keep)
-    {
-        if (rec.size() > new_slot_of_node.size()) rec.resize(new_slot_of_node.size());
-        for (size_t i = 0; i < rec.size(); ++i) {
-            if (i < old_slot_of_node.size() && old_slot_of_node[i] != FYX_NONE && new_slot_of_node[i] != FYX_NONE) keep(rec[i]);
-            else rec[i] = def;
-        }
-    }
-    void topology_changed(const std::vector<uint32_t> &old_slot_of_node, const std::vector<uint32_t> &new_slot_of_node)
-    {
-        topology_changed(old_slot_of_node, new_slot_of_node, [](T &) {});
-    }
-    // f(node, slot, record) for the record of every alive node, in pool order
-    template <class F> void for_alive(const std::vector<uint32_t> &slot_of_node, F f)
-    {
-        const size_t n = std::min(rec.size(), slot_of_node.size());
-        for (size_t node = 0; node < n; ++node)
-            if (slot_of_node[node] != FYX_NONE) f((uint32_t)node, slot_of_node[node], rec[node]);
-    }
-};
-
 // The records kept with a value derived from them: the projection's one transcendental, evaluated on the host with the
 // platform's tanf, and whether a probe is due
 struct LightRec {
@@ -268,11 +231,11 @@ struct InstPack {
     uint32_t h_seg = FYX_NONE, h_surf_seg = FYX_NONE;
     bool valid = false, blocks_valid = false;
     uint32_t segments() const { return (uint32_t)inst_first.size() - 1; }
-    // the dynamic batches of every segment (fyx_dynamic_batches): bundles and instances at dyn_item0[seg], each segment's
-    // streams (one per layout it uses, ascending layout id) at dyn_stream0[seg] of dyn_streams with device pointers
+    // the dynamic batches of every segment (fyx_dynamic_batches): bundles and instances at dyn.item0[seg], each segment's
+    // streams at dyn.stream0[seg] of dyn.streams with device pointers
     DevBuf b_dyn_bundles, b_dyn_inst, b_dyn_vtx, b_dyn_tri;
-    std::vector<uint32_t> dyn_item0, dyn_counts, dyn_stream0; // [segments + 1], [segments * 2] bundles / instances, [segments + 1]
-    std::vector<fyx_dynamic_stream> dyn_streams;
+    DynPlacement dyn;
+    std::vector<uint32_t> dyn_counts; // [segments * 2] bundles / instances
     PinnedBuf h_dyn[4];                     // bundles, instances, vertices, triangles of segment h_dyn_seg
     std::vector<fyx_dynamic_stream> dyn_out_host, dyn_out_dev; // the streams handed out by the last host / device getter
     uint32_t h_dyn_seg = FYX_NONE;
@@ -310,48 +273,24 @@ struct PackScratch {
     PinnedBuf h_dyn_counts;
 };
 
-// Dynamic batching: one registered surface (fyx_add_dynamic_surface)
-struct DynReg {
-    uint32_t id, node, ordinal, batch_key, layout, n_verts, n_tris, tri_src;
-    uint64_t vtx_src;
-};
-
-// Dynamic batching (fyx_drawprep.inl): what push_triangles batches, the registered surfaces of Dynamic meshes and the quad
-// nodes (fyx_set_sprites), with the layout ids and batch keys they share, the pools, and the device tables in push order
-// (DynItemDev).  The tables are rebuilt by the first pack after invalidate(), which every input of the flush calls: the
-// registrations, the quad nodes, the topology, the DFS order and the node surfaces.
+// Dynamic batching (fyx_drawprep.inl): what push_triangles batches, the registrations of Dynamic meshes and the quad nodes
+// (fyx_set_sprites) with the rules of fyx_dyn_plan.hpp, the quad nodes' full records by slot, which the quad kernel reads, the
+// pools, and the device tables in push order (DynItemDev).  The tables are rebuilt by the first pack after invalidate(), which
+// every input of the flush calls: the registrations, the quad nodes, the topology, the DFS order and the node surfaces.
 struct DynBatches {
-    enum Use { kNeither, kRegistrations, kQuad }; // what a node holds
-    // this call's claims of layout ids (with their layouts) and batch keys (with their layout ids), not yet committed
-    struct Claims {
-        std::unordered_map<uint32_t, fyx_dynamic_layout> layout;
-        std::unordered_map<uint32_t, uint32_t> key;
-    };
-    std::vector<DynReg> regs;
-    std::set<uint64_t> pairs; // node << 32 | ordinal of every registration
-    uint32_t next_id = 0;
-    // quad nodes: kind, batch key and layout id by node index (kind 0 = not a quad node); the full records by slot, which the
-    // quad kernel reads
-    std::vector<uint3> quad_of_node;
-    std::vector<uint32_t> quad_seen; // by node index: the fyx_set_sprites call that last listed it (duplicate check)
-    uint32_t quad_call = 0;
+    DynRegistry reg;
     SlotColumn quads{fyx_sprite{}};
-    std::vector<fyx_dynamic_layout> layouts; // by layout id; stride FYX_NONE = nothing uses it
-    std::vector<uint32_t> key_layout;        // by batch key; FYX_NONE = nothing uses it
-    DevBuf b_vtx, b_tri;                     // pools: vertex bytes (each surface 16-byte aligned), triangles
-    uint64_t vtx_used = 0, tri_used = 0;
+    DevBuf b_vtx, b_tri; // pools: vertex bytes, triangles (reg.vtx_used / reg.tri_used)
     bool stale = false;
     uint32_t n_nodes = 0, n_items = 0, n_quads = 0, n_layouts = 0; // of the device tables
     DevBuf b_of_slot, b_item_first, b_ordinal, b_items, b_layouts;
 
     void invalidate() { stale = true; }
-    Use use_of(uint32_t node) const;
-    // a claim of `layout_id` for `ly` and of `batch_key` for `layout_id`: refused when the committed tables or `staged` give
-    // either to another, else added to `staged`
-    int32_t check_claim(fyx_ctx *c, uint32_t layout_id, const fyx_dynamic_layout &ly, uint32_t batch_key, Claims &staged) const;
-    void commit(const Claims &staged);
-    void release(); // after registrations or quad nodes went: their pairs, and the layout ids and batch keys nothing uses, go
-    void topology_changed(const fyx_ctx *c); // a node that is not alive any more drops its registrations and quad
+    void topology_changed(const std::vector<uint32_t> &old_slot_of_node, const std::vector<uint32_t> &new_slot_of_node)
+    {
+        reg.topology_changed(old_slot_of_node, new_slot_of_node);
+        invalidate();
+    }
     int32_t compact(fyx_ctx *c);
     int32_t flush(fyx_ctx *c);
     int32_t pack(fyx_ctx *c, InstPack &o, const uint32_t *vis_slot, const float *views, const float *view, const std::vector<uint32_t> &first,
@@ -584,6 +523,12 @@ int32_t fail(fyx_ctx *c, int32_t code, const char *fmt, ...)
     return code;
 }
 
+// the context's error message, for the checks of the planner headers
+auto fail_of(fyx_ctx *c)
+{
+    return [c](int32_t code, const char *fmt, auto... args) { return fail(c, code, fmt, args...); };
+}
+
 #define CU(call)                                                                                         \
     do {                                                                                                 \
         cudaError_t e__ = (call);                                                                        \
@@ -697,7 +642,9 @@ int32_t SlotColumn::scatter(fyx_ctx *c, uint32_t count, const uint32_t *idx, con
     return rc ? rc : scatter_words(c, buf.as<uint32_t>(), def.words, count, idx, values);
 }
 
-template <class T> int32_t NodeRecords<T>::check(fyx_ctx *c, uint32_t count, const uint32_t *idx) const
+} // namespace
+
+template <class T> int32_t fyx::NodeRecords<T>::check(fyx_ctx *c, uint32_t count, const uint32_t *idx) const
 {
     for (uint32_t e = 0; e < count; ++e) {
         const uint32_t node = idx ? idx[e] : e;
@@ -705,6 +652,8 @@ template <class T> int32_t NodeRecords<T>::check(fyx_ctx *c, uint32_t count, con
     }
     return FYX_OK;
 }
+
+namespace {
 
 int32_t check_device_errors(fyx_ctx *c)
 {
@@ -1150,7 +1099,7 @@ extern "C" int32_t fyx_set_topology(fyx_ctx *c, uint32_t capacity, uint32_t root
     for (uint32_t i : static_batch) pr_mark(c, i, kPrBatch, true);
     c->shadow_cull.topology_changed();
     c->observer_cull.topology_changed();
-    c->dyn.topology_changed(c);
+    c->dyn.topology_changed(old_slot_of_node, new_slot_of_node);
     c->skin.topology_changed();
     c->anim.topology_changed();
 

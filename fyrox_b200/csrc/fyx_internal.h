@@ -15,6 +15,7 @@
 #include "../../include/fyrox_b200.h"
 #include "fyx_math.cuh"
 #include "fyx_anim_plan.hpp"
+#include "fyx_dyn_plan.hpp"
 #include "fyx_skin_plan.hpp"
 #include "fyx_slots.hpp"
 
@@ -171,22 +172,9 @@ struct InstParams {
     const uint32_t *dyn_of_slot, *dyn_item_first, *dyn_ordinal;
 };
 
-// Dynamic batching (scene/mesh/mod.rs:739-753, 804-833; renderer/bundle.rs:1177-1243).  The registered surfaces and the quad
-// nodes (fyx_set_sprites: one item of 4 vertices and 2 triangles each), in the reference's push order: dynamic nodes ordered by
-// DFS rank (else node index), each node's surfaces by ordinal.
-constexpr uint32_t kDynMesh = 0u; // DynItemDev::kind of a registered surface; else FYX_SPRITE_3D / FYX_SPRITE_RECTANGLE
-struct DynItemDev {
-    uint32_t node, slot, batch_key, layout;
-    uint32_t n_verts, n_tris;
-    uint32_t tri_src;   // first u32 of its triangles in the registration pool
-    uint32_t kind;
-    uint64_t vtx_src;   // first byte of its vertices in the registration pool (16-byte aligned)
-};
-struct DynLayoutDev {
-    uint32_t stride, pos, nrm, tan; // attribute offsets, FYX_NONE = not transformed
-};
-// One pack's dynamic pass over its segments: mark (the segments' dynamic nodes and counts), then, once the host has placed
-// every segment's items, hash tables and (segment, layout) streams, order + bundles (one CTA per segment) and geometry.
+// One pack's dynamic pass over its segments (DynItemDev / DynLayoutDev in fyx_dyn_plan.hpp): mark (the segments' dynamic nodes
+// and counts), then, once the host has placed every segment's items, hash tables and (segment, layout) streams, order + bundles
+// (one CTA per segment) and geometry.
 struct DynParams {
     // registrations
     const uint32_t *dyn_of_slot, *item_first; // [slots], [D + 1]

@@ -100,6 +100,43 @@ inline SlotPlan plan_slots(uint32_t capacity, const uint32_t *parent, const uint
     return p;
 }
 
+// One record per node index, for what the setters keep on the host by node: light sources, CSM options, cameras, reflection
+// probes, node surfaces, pruner marks, quad nodes.  `def` is the record of a node that was never given one.  Across
+// fyx_set_topology a record stays with its node index while the node is alive before and after the call; every other index
+// starts again from `def`, as in the slot columns.
+template <class T> struct NodeRecords {
+    T def;
+    std::vector<T> rec; // by node index; the indices past its end hold `def`
+    explicit NodeRecords(const T &v) : def(v) {}
+    const T &operator[](uint32_t node) const { return node < rec.size() ? rec[node] : def; }
+    void set(uint32_t node, const T &v)
+    {
+        if (node >= rec.size()) rec.resize(node + 1, def);
+        rec[node] = v;
+    }
+    int32_t check(fyx_ctx *c, uint32_t count, const uint32_t *idx) const; // every node listed (idx NULL = 0..count-1) is in range
+    // keep(record) trims a record that stays to what it keeps.  Only the records that restart are written.
+    template <class Keep> void topology_changed(const std::vector<uint32_t> &old_slot_of_node, const std::vector<uint32_t> &new_slot_of_node, Keep keep)
+    {
+        if (rec.size() > new_slot_of_node.size()) rec.resize(new_slot_of_node.size());
+        for (size_t i = 0; i < rec.size(); ++i) {
+            if (i < old_slot_of_node.size() && old_slot_of_node[i] != FYX_NONE && new_slot_of_node[i] != FYX_NONE) keep(rec[i]);
+            else rec[i] = def;
+        }
+    }
+    void topology_changed(const std::vector<uint32_t> &old_slot_of_node, const std::vector<uint32_t> &new_slot_of_node)
+    {
+        topology_changed(old_slot_of_node, new_slot_of_node, [](T &) {});
+    }
+    // f(node, slot, record) for the record of every alive node, in pool order
+    template <class F> void for_alive(const std::vector<uint32_t> &slot_of_node, F f)
+    {
+        const size_t n = std::min(rec.size(), slot_of_node.size());
+        for (size_t node = 0; node < n; ++node)
+            if (slot_of_node[node] != FYX_NONE) f((uint32_t)node, slot_of_node[node], rec[node]);
+    }
+};
+
 struct SfRange {
     uint32_t begin, end; // slots [begin, end) of one level of one group
 };

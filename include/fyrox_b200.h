@@ -775,7 +775,9 @@ typedef struct fyx_dynamic_layout { /* the VertexBuffer layout, as transform_ver
  * the shared surface.  verts = n_verts records of layout->stride bytes; triangles = 3 u32 per triangle.  FYX_ERR_INVALID_ARGUMENT
  * for n_verts >= 256 (the reference pushes such a surface), a surface that fyx_set_node_surfaces names as skinned, an ordinal
  * the node does not have, a (node, ordinal) already registered, a layout_id given before with another layout, and a
- * batch_key given before with another layout_id (the reference's push_vertex_raw would panic, scene/mesh/buffer.rs:506-517).
+ * batch_key given before with another layout_id (the reference's push_vertex_raw would panic, scene/mesh/buffer.rs:506-517),
+ * and triangles that would not end below 2^32 u32 words of the context's triangle pool (dropped registrations keep their words
+ * until the next pack reuses the space).
  * Registrations stay with their node index across fyx_set_topology; a node it removes drops them.  A surface that a later
  * fyx_set_node_surfaces removes or names skinned is pushed again (its registration is kept but not used).  The call copies the
  * data before it returns.  out_id may be NULL. */
