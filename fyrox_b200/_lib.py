@@ -123,6 +123,11 @@ class fyx_anim_track(C.Structure):
                 ("n_curves", C.c_uint32), ("first_key", C.c_uint32 * 4), ("n_keys", C.c_uint32 * 4)]
 
 
+class fyx_root_motion_settings(C.Structure):
+    _fields_ = [("node", C.c_uint32), ("ignore_x_movement", C.c_uint32), ("ignore_y_movement", C.c_uint32), ("ignore_z_movement", C.c_uint32),
+                ("ignore_rotations", C.c_uint32)]
+
+
 class fyx_animation_desc(C.Structure):
     _fields_ = [
         ("struct_size", C.c_uint32),
@@ -299,6 +304,13 @@ SYMBOLS = {
     "fyx_anim_blend_group": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p, u32p]),
     "fyx_anim_set_blend_weights": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "fyx_animate": (C.c_int32, [ctx_p, C.c_float]),
+    "fyx_anim_set_signals": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "fyx_anim_set_signal_enabled": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_uint32]),
+    "fyx_anim_set_max_event_capacity": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32]),
+    "fyx_anim_take_events": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, u32p, u32p]),
+    "fyx_anim_set_root_motion": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p]),
+    "fyx_anim_get_root_motions": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "fyx_anim_get_group_root_motions": (C.c_int32, [ctx_p, C.c_uint32, C.c_uint32, C.c_void_p]),
     "fyx_set_bundle_ids": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),
     "fyx_enable_instances": (C.c_int32, [ctx_p, C.c_uint32]),
     "fyx_pack_instances": (C.c_int32, [ctx_p, C.c_uint32, C.c_void_p, C.c_void_p]),

@@ -173,6 +173,43 @@ class TrackBinding:
     enabled: bool = True
 
 
+@dataclass
+class AnimationSignal:
+    """fyrox-animation/src/signal.rs:44-74: `id` stands for the Uuid; events name the signal by it."""
+
+    id: int = 0
+    name: str = ""
+    time: float = 0.0
+    enabled: bool = True
+
+
+@dataclass
+class AnimationEvent:
+    """lib.rs: the signal_id and name of the signal that fired."""
+
+    signal_id: int
+    name: str
+
+
+@dataclass
+class RootMotionSettings:
+    """lib.rs:305-319"""
+
+    node: int = 0
+    ignore_x_movement: bool = False
+    ignore_y_movement: bool = False
+    ignore_z_movement: bool = False
+    ignore_rotations: bool = False
+
+
+@dataclass
+class RootMotion:
+    """lib.rs:324-336, the public part: what Animation::root_motion() shows a game."""
+
+    delta_position: Tuple[float, float, float] = (0.0, 0.0, 0.0)
+    delta_rotation: Tuple[float, float, float, float] = (0.0, 0.0, 0.0, 1.0)  # (i, j, k, w)
+
+
 class Animation:
     """fyrox-animation/src/lib.rs:269-496, 755-790, 922-945 — the data and switches of one animation; defaults as
     Animation::default (speed 1, looped, enabled, empty time slice)."""
@@ -186,6 +223,34 @@ class Animation:
         self.enabled = True
         self.looped = True
         self.time_slice: Tuple[float, float] = (0.0, 0.0)
+        self.signals: List[AnimationSignal] = []
+        self.max_event_capacity = 32
+        self.events: List[AnimationEvent] = []  # filled by AnimationContainer.fetch_events from the device
+        self.root_motion_settings: Optional[RootMotionSettings] = None
+        self._root_motion: Optional[RootMotion] = None  # set by AnimationContainer.fetch_root_motions
+
+    def add_signal(self, signal: AnimationSignal) -> AnimationSignal:
+        self.signals.append(signal)
+        return signal
+
+    def set_max_event_capacity(self, capacity: int):
+        self.max_event_capacity = int(capacity)
+
+    def pop_event(self) -> Optional[AnimationEvent]:
+        return self.events.pop(0) if self.events else None
+
+    def take_events(self) -> List[AnimationEvent]:
+        ev, self.events = self.events, []
+        return ev
+
+    def set_root_motion_settings(self, settings: Optional[RootMotionSettings]):
+        self.root_motion_settings = settings
+
+    def root_motion_settings_ref(self) -> Optional[RootMotionSettings]:
+        return self.root_motion_settings
+
+    def root_motion(self) -> Optional[RootMotion]:
+        return self._root_motion
 
     def add_track_with_binding(self, binding: TrackBinding, track: Track):
         self.tracks.append(track)
@@ -249,8 +314,41 @@ class AnimationContainer:
         return len(self.animations) - 1
 
     def upload(self, ctx) -> List[int]:
+        """Also hands each animation's signals, event capacity and root-motion settings to the device."""
         ids = []
         for a in self.animations:
             t, k, kw = a.flatten()
-            ids.append(ctx.anim_add(t, k, **kw))
+            i = ctx.anim_add(t, k, **kw)
+            if a.signals:
+                ctx.anim_set_signals(i, [(s.time, s.enabled) for s in a.signals])
+            if a.max_event_capacity != 32:
+                ctx.anim_set_max_event_capacity(i, a.max_event_capacity)
+            s = a.root_motion_settings
+            if s is not None:
+                ctx.anim_set_root_motion(i, s.node, s.ignore_x_movement, s.ignore_y_movement, s.ignore_z_movement, s.ignore_rotations)
+            ids.append(i)
         return ids
+
+    def fetch_events(self, ctx, ids: List[int]):
+        """Drain the device's events into each animation's queue (then pop_event / take_events), mapping the signal index
+        back to the signal's id and name.  The drain covers every animation of the context: events of animations that are
+        not in `ids` (another container's) are dropped.  Returns the number of events the device dropped because a store
+        was full."""
+        by_id = {d: a for d, a in zip(ids, self.animations)}
+        ev, lost = ctx.anim_take_events()
+        for anim, sig in ev.tolist():
+            a = by_id.get(anim)
+            if a is not None:
+                s = a.signals[sig]
+                a.events.append(AnimationEvent(s.id, s.name))
+        return lost
+
+    def fetch_root_motions(self, ctx, ids: List[int]):
+        """Animation::root_motion() of every animation, read back from the device."""
+        if not ids:
+            return
+        rm = ctx.anim_root_motions(min(ids), max(ids) - min(ids) + 1)
+        for d, a in zip(ids, self.animations):
+            r = rm[d - min(ids)]
+            a._root_motion = RootMotion(tuple(float(x) for x in r["delta_position"]), tuple(float(x) for x in r["delta_rotation"])) \
+                if r["present"] else None

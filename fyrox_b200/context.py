@@ -558,6 +558,58 @@ class Context:
         """AnimationContainer::update_animations(dt) for every animation (scene/animation/mod.rs:83-88)."""
         self._chk(self._lib.fyx_animate(self._h, float(dt)))
 
+    SIGNAL_DTYPE = np.dtype([("time", "<f4"), ("enabled", "<u4")])
+    EVENT_DTYPE = np.dtype([("anim", "<u4"), ("signal", "<u4")])
+    ROOT_MOTION_DTYPE = np.dtype([("delta_position", "<f4", 3), ("delta_rotation", "<f4", 4), ("present", "<u4")])
+
+    def anim_set_signals(self, anim: int, signals):
+        """Replace animation `anim`'s signals: a sequence of (time, enabled) or a SIGNAL_DTYPE array.  Events name a
+        signal by its index in this list."""
+        s = np.array([tuple(x) for x in signals], self.SIGNAL_DTYPE) if not isinstance(signals, np.ndarray) else signals
+        s = np.ascontiguousarray(s, dtype=self.SIGNAL_DTYPE)
+        self._chk(self._lib.fyx_anim_set_signals(self._h, anim, len(s), s.ctypes.data_as(C.c_void_p) if len(s) else None))
+
+    def anim_set_signal_enabled(self, anim: int, signal: int, enabled: bool):
+        self._chk(self._lib.fyx_anim_set_signal_enabled(self._h, anim, signal, int(bool(enabled))))
+
+    def anim_set_max_event_capacity(self, anim: int, capacity: int):
+        self._chk(self._lib.fyx_anim_set_max_event_capacity(self._h, anim, int(capacity)))
+
+    def anim_take_events(self, max_events: Optional[int] = None):
+        """(EVENT_DTYPE array, lost): Animation::take_events of every animation, grouped by animation in ascending order;
+        `lost` counts the events dropped because a store was full since the last call.  max_events None = every queued
+        event; otherwise the rest stays queued."""
+        chunk = 4096 if max_events is None else int(max_events)
+        parts, lost_total = [], 0
+        while True:
+            out = np.zeros(max(chunk, 1), self.EVENT_DTYPE)
+            n, lost = C.c_uint32(), C.c_uint32()
+            self._chk(self._lib.fyx_anim_take_events(self._h, chunk, out.ctypes.data_as(C.c_void_p), C.byref(n), C.byref(lost)))
+            parts.append(out[:n.value])
+            lost_total += lost.value
+            if max_events is not None or n.value < chunk:
+                return np.concatenate(parts), lost_total
+
+    def anim_set_root_motion(self, anim: int, node=None, ignore_x=False, ignore_y=False, ignore_z=False, ignore_rotations=False):
+        """Animation::set_root_motion_settings: node None = settings None."""
+        if node is None:
+            self._chk(self._lib.fyx_anim_set_root_motion(self._h, anim, None))
+            return
+        s = L.fyx_root_motion_settings(int(node), int(bool(ignore_x)), int(bool(ignore_y)), int(bool(ignore_z)), int(bool(ignore_rotations)))
+        self._chk(self._lib.fyx_anim_set_root_motion(self._h, anim, C.byref(s)))
+
+    def anim_root_motions(self, first: int, count: int) -> np.ndarray:
+        """Animation::root_motion() of `count` animations from `first` (ROOT_MOTION_DTYPE; present = 0 is None)."""
+        out = np.zeros(count, self.ROOT_MOTION_DTYPE)
+        self._chk(self._lib.fyx_anim_get_root_motions(self._h, first, count, out.ctypes.data_as(C.c_void_p)))
+        return out
+
+    def anim_group_root_motions(self, first_group: int, count: int) -> np.ndarray:
+        """The final pose's root_motion() of blend groups first_group .. first_group + count (groups count from 1)."""
+        out = np.zeros(count, self.ROOT_MOTION_DTYPE)
+        self._chk(self._lib.fyx_anim_get_group_root_motions(self._h, first_group, count, out.ctypes.data_as(C.c_void_p)))
+        return out
+
     # ---- N3: draw-prep after the cull ----
     def set_bundle_ids(self, ids, idx=None):
         """Per-node bundle id = dense id of the (material, surface data, render path) key of

@@ -183,4 +183,119 @@ inline AnimNodePlan plan_anim_nodes(const std::vector<AnimInfo> &anims, const st
     return p;
 }
 
+// ---- signals and root motion ----
+
+constexpr uint32_t kDefaultMaxEventCapacity = 32; // Animation::default (lib.rs:941)
+
+// One animation's signals and event queue as k_anim_tick reads them: a ring of `storage` signal indices
+struct AnimSigDev {
+    uint32_t first_signal, n_signals; // in the context-wide signal array
+    uint32_t ev_off, storage;         // its ring in the context-wide event array
+    uint32_t cap;                     // max_event_capacity
+    uint32_t head, count;             // undrained events: ring[(head + k) % storage], k < count
+    uint32_t lost;                    // speed >= 0 events that found the ring full, since the last drain
+};
+
+// What the host keeps of one animation's signals
+struct AnimSignals {
+    std::vector<fyx_anim_signal> list;
+    uint32_t cap = kDefaultMaxEventCapacity;
+};
+
+// The device tables of every animation's signals; `queued[a]` = its undrained events in queue order, which the new ring
+// keeps (a ring never shrinks below them, so relaying loses nothing); `lost[a]` carries over
+struct EventPlan {
+    std::vector<AnimSigDev> sig;
+    std::vector<fyx_anim_signal> signals;
+    std::vector<uint32_t> events; // the rings, queued events first
+};
+inline EventPlan plan_events(const std::vector<AnimSignals> &s, const std::vector<std::vector<uint32_t>> &queued,
+                             const std::vector<uint32_t> &lost)
+{
+    EventPlan p;
+    p.sig.resize(s.size());
+    for (size_t a = 0; a < s.size(); ++a) {
+        const std::vector<uint32_t> &q = queued[a];
+        AnimSigDev &d = p.sig[a];
+        d.first_signal = (uint32_t)p.signals.size();
+        d.n_signals = (uint32_t)s[a].list.size();
+        d.ev_off = (uint32_t)p.events.size();
+        d.storage = std::max<uint32_t>(std::max<uint32_t>(s[a].cap, d.n_signals), (uint32_t)q.size());
+        d.cap = s[a].cap;
+        d.head = 0;
+        d.count = (uint32_t)q.size();
+        d.lost = lost[a];
+        p.signals.insert(p.signals.end(), s[a].list.begin(), s[a].list.end());
+        p.events.insert(p.events.end(), q.begin(), q.end());
+        p.events.resize(p.events.size() + (d.storage - d.count), 0u);
+    }
+    return p;
+}
+
+// One animation with root-motion settings as k_anim_root_motion reads it
+constexpr uint32_t kIgnoreX = 1u, kIgnoreY = 2u, kIgnoreZ = 4u, kIgnoreRotations = 8u;
+struct AnimRootDev {
+    uint32_t anim;
+    uint32_t pos_track, rot_track;             // the root node's Vector3 Position / quaternion Rotation track, or FYX_NONE
+    uint32_t first_pos_track, first_rot_track; // the animation's first Position / Rotation track of any target, or FYX_NONE
+    uint32_t ignore;                           // kIgnore* bits
+};
+// RootMotion (lib.rs:324-336) on the device; `m` is what Animation::root_motion() returns
+struct RootMotionDev {
+    fyx_root_motion m;
+    float prev_position[3], position_remainder[3];
+    float prev_rotation[4], rotation_remainder[4];
+    uint32_t has_position_remainder, has_rotation_remainder;
+};
+
+// fyx_anim_set_root_motion's check of the settings of animation `a`
+template <class Fail>
+int32_t check_root_motion(const AnimInfo &a, const fyx_root_motion_settings &s, const std::vector<uint32_t> &track_node,
+                          const std::vector<uint32_t> &track_bind_kind, Fail fail)
+{
+    uint32_t n_pos = 0, n_rot = 0;
+    for (uint32_t t = a.first_track; t < a.first_track + a.n_tracks; ++t) {
+        if (track_node[t] != s.node) continue;
+        const uint32_t b = track_bind_kind[t] & 0xFFu;
+        n_pos += (b == FYX_BIND_POSITION);
+        n_rot += (b == FYX_BIND_ROTATION);
+    }
+    if (n_pos > 1 || n_rot > 1) return fail(FYX_ERR_UNSUPPORTED, "root node %u has two tracks of one property", s.node);
+    return FYX_OK;
+}
+
+// The record of animation `id` (checked settings)
+inline AnimRootDev plan_root_motion(uint32_t id, const AnimInfo &a, const fyx_root_motion_settings &s,
+                                    const std::vector<uint32_t> &track_node, const std::vector<uint32_t> &track_bind_kind)
+{
+    AnimRootDev r{id, FYX_NONE, FYX_NONE, FYX_NONE, FYX_NONE, 0u};
+    r.ignore = (s.ignore_x_movement ? kIgnoreX : 0u) | (s.ignore_y_movement ? kIgnoreY : 0u) | (s.ignore_z_movement ? kIgnoreZ : 0u) |
+               (s.ignore_rotations ? kIgnoreRotations : 0u);
+    for (uint32_t t = a.first_track; t < a.first_track + a.n_tracks; ++t) {
+        const uint32_t b = track_bind_kind[t] & 0xFFu, kind = track_bind_kind[t] >> 8;
+        const bool quat = (kind == FYX_TV_QUAT || kind == FYX_TV_QUAT_EULER);
+        if (b == FYX_BIND_POSITION && r.first_pos_track == FYX_NONE) r.first_pos_track = t;
+        if (b == FYX_BIND_ROTATION && r.first_rot_track == FYX_NONE) r.first_rot_track = t;
+        if (track_node[t] != s.node) continue;
+        if (b == FYX_BIND_POSITION && kind == FYX_TV_VECTOR3) r.pos_track = t; // another kind never matches TrackValue::Vector3
+        if (b == FYX_BIND_ROTATION && quat) r.rot_track = t;
+    }
+    return r;
+}
+
+// The blend groups' sources for k_anim_group_root_motion: group g (from 1) has src[begin[g - 1] .. begin[g])
+struct GroupSourcePlan {
+    std::vector<uint32_t> begin, src;
+};
+inline GroupSourcePlan plan_group_sources(const std::vector<std::vector<uint32_t>> &groups)
+{
+    GroupSourcePlan p;
+    p.begin.push_back(0u);
+    for (const std::vector<uint32_t> &g : groups) {
+        p.src.insert(p.src.end(), g.begin(), g.end());
+        p.begin.push_back((uint32_t)p.src.size());
+    }
+    return p;
+}
+
 } // namespace fyx

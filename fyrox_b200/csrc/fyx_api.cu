@@ -342,6 +342,19 @@ struct Animations {
     uint32_t n_nodes = 0; // of the node CSR
     bool dirty = true;    // the node CSR is out of date
 
+    // Signals: the lists and capacities here; rings, queue heads and counts on the device once any animation has a signal
+    std::vector<AnimSignals> sig;                   // per animation once signals_on
+    bool signals_on = false, events_dirty = false;  // events_dirty: the device tables need relaying (commit)
+    DevBuf b_sig, b_signals, b_events, b_drain; // b_drain: fyx_anim_take_events' header (2 words), then its events
+    // Root motion: the settings per animation; the device records once any animation has had settings (they outlive them)
+    std::vector<uint8_t> has_root;                  // per animation
+    std::vector<fyx_root_motion_settings> root;     // per animation
+    bool root_on = false, roots_dirty = false;
+    uint32_t n_roots = 0, n_sig = 0, n_event_words = 0; // records in b_roots / b_sig, words in b_events
+    DevBuf b_roots, b_rm, b_grm, b_group_begin, b_group_src; // b_grm: per group, BlendAnimations' output, then the final pose's
+    uint64_t frames = 0;                            // fyx_animate calls that launched (a group is evaluated once one has)
+    std::vector<uint64_t> group_born;               // `frames` when group g was made, at [g - 1]
+
     int32_t add(fyx_ctx *c, const fyx_animation_desc &d, uint32_t *out_id); // checks, then queues
     int32_t flush(fyx_ctx *c); // uploads the queue (the device tables grow, keeping the older animations' hints and time)
     int32_t commit(fyx_ctx *c); // flush, then plan_anim_nodes and its upload when dirty
@@ -350,6 +363,9 @@ struct Animations {
     template <class R, class F> int32_t write(fyx_ctx *c, uint32_t i, F R::*field, F v) const;
     void topology_changed() { dirty = true; } // target slots
     AnimArrays arrays() const; // what the kernels read, from the buffers as they are now
+    int32_t download_events(fyx_ctx *c, std::vector<AnimSigDev> &d, std::vector<uint32_t> &ev) const;
+    int32_t commit_events(fyx_ctx *c); // relays the signal tables (commit, when events_dirty)
+    int32_t commit_roots(fyx_ctx *c);  // the root-motion tables (commit, when roots_dirty)
 };
 
 } // namespace

@@ -124,9 +124,22 @@ struct AnimArrays {
     const uint32_t *node_slot;
     const uint32_t *node_begin;
     const uint32_t *node_tracks;
+    // signals: every animation's ring (nullptr = no animation has signals)
+    AnimSigDev *sig;
+    const fyx_anim_signal *signals;
+    uint32_t *events;
+    // root motion: the animations with settings, every animation's record, and the blend groups' (n_groups = 0: none)
+    uint32_t n_roots, n_groups;
+    const AnimRootDev *roots;
+    RootMotionDev *rm;
+    fyx_root_motion *grm; // per group: BlendAnimations' output, then the machine's final pose
+    const uint32_t *group_begin, *group_src;
 };
 uint32_t launch_animate(cudaStream_t s, const NodeArrays &a, const AnimArrays &an, fyx_trs *trs_by_slot,
                         const fyx_transform_statics *st_by_slot, float dt, uint32_t *d_err);
+// Animation::take_events of n animations' rings into out[0 .. header[0]); header[1] = the lost events (cleared)
+uint32_t launch_drain_events(cudaStream_t s, AnimSigDev *sig, uint32_t n, const uint32_t *events, uint32_t max, fyx_anim_event *out,
+                             uint32_t *header);
 
 // N3 draw-prep (fyx_drawprep.cu): one frustum's visible list -> instances grouped by bundle
 struct InstParams {

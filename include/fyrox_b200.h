@@ -570,8 +570,8 @@ uint64_t fyx_kernel_launch_count(const fyx_ctx *ctx);
  * Properties no track writes keep the value of the node's last fyx_set_local_trs record (identity if none);
  * pivots / offsets / pre- and post-rotation come from fyx_set_transform_statics.
  * Parity: Vector3 and UnitQuaternion tracks bit-exact; UnitQuaternionEuler tracks use sin/cos (platform libm in the
- * reference): ~1e-7 absolute on the quaternion.  Signals, root motion, property bindings and the blend-machine
- * (ABSM) layers are not modelled. */
+ * reference): ~1e-7 absolute on the quaternion.  Signals and root motion: fyx_anim_set_signals / fyx_anim_set_root_motion
+ * below.  Property bindings and the blend-machine (ABSM) layers are not modelled. */
 #define FYX_KEY_CONSTANT 0u /* CurveKeyKind (fyrox-math/src/curve.rs:33-45) */
 #define FYX_KEY_LINEAR 1u
 #define FYX_KEY_CUBIC 2u
@@ -636,6 +636,56 @@ int32_t fyx_anim_set_blend_weights(fyx_ctx *ctx, uint32_t group, uint32_t n, con
 /* AnimationContainer::update_animations(dt) for every animation of the context.  The touched nodes are marked
  * changed exactly like fyx_set_local_trs; follow with fyx_update_transforms / fyx_render_prep. */
 int32_t fyx_animate(fyx_ctx *ctx, float dt);
+
+/* Signals (fyrox-animation/src/lib.rs:477-489, signal.rs).  An enabled signal of a ticking animation fires when
+ * speed >= 0 && time < signal.time && time + dt * speed >= signal.time, or when speed < 0 && time > signal.time &&
+ * time + dt * speed <= signal.time && (undrained events of that animation) < max_event_capacity (default 32) — the
+ * capacity binds to the negative-speed branch only, as in the reference.  The time compared is the unwrapped new time,
+ * so a signal past the slice end still fires on the tick that wraps.  An event names the signal by its index in the
+ * animation's list; the host maps it to the signal's Uuid and name.  Each animation stores max(max_event_capacity,
+ * number of its signals) undrained events, so a host that drains after every tick loses none; a speed >= 0 event that
+ * finds the store full is dropped and counted in out_lost (the reference's queue would grow: the one divergence). */
+typedef struct fyx_anim_signal {
+    float time;
+    uint32_t enabled;
+} fyx_anim_signal;
+typedef struct fyx_anim_event {
+    uint32_t anim, signal;
+} fyx_anim_event;
+int32_t fyx_anim_set_signals(fyx_ctx *ctx, uint32_t anim, uint32_t n, const fyx_anim_signal *signals); /* replaces the list */
+int32_t fyx_anim_set_signal_enabled(fyx_ctx *ctx, uint32_t anim, uint32_t signal, uint32_t enabled);
+int32_t fyx_anim_set_max_event_capacity(fyx_ctx *ctx, uint32_t anim, uint32_t capacity);
+/* Animation::take_events of every animation: events grouped by animation (ascending), each animation's in queue order;
+ * what does not fit in `max` stays queued.  out_lost = events dropped since the last call.  The events are gathered on
+ * the device: only they and a two-word count cross PCIe.  Waits for every frame enqueued so far. */
+int32_t fyx_anim_take_events(fyx_ctx *ctx, uint32_t max, fyx_anim_event *out, uint32_t *out_n, uint32_t *out_lost);
+
+/* Root motion (lib.rs:302-344, 498-661): after the pose is sampled and the time advanced, the root node's Position and
+ * Rotation values become a relative motion (re-based on a new loop cycle with the remainder to the cycle's end) and are
+ * reset to the time slice's start, so the root stays in place.  The cycle-start / end values come from the FIRST
+ * Position / Rotation track of the animation whatever its target and enabled flag (zero / identity if it has none or it
+ * is of another kind).  Refused: a root node with two Position or two Rotation tracks in the animation.  Settings NULL =
+ * None; the last root motion then stays as it was. */
+typedef struct fyx_root_motion_settings {
+    uint32_t node;
+    uint32_t ignore_x_movement, ignore_y_movement, ignore_z_movement, ignore_rotations;
+} fyx_root_motion_settings;
+typedef struct fyx_root_motion {
+    float delta_position[3];
+    float delta_rotation[4]; /* (i, j, k, w) */
+    uint32_t present;        /* 0 = None (then zero / identity) */
+} fyx_root_motion;
+int32_t fyx_anim_set_root_motion(fyx_ctx *ctx, uint32_t anim, const fyx_root_motion_settings *settings);
+/* Animation::root_motion() of animations first .. first + count */
+int32_t fyx_anim_get_root_motions(fyx_ctx *ctx, uint32_t first, uint32_t count, fyx_root_motion *out);
+/* The machine's final pose().root_motion() of blend groups first_group .. first_group + count (groups count from 1):
+ * BlendAnimations folds its sources' root motions into its output with RootMotion::blend_with (pose.rs:89-101; lerp and
+ * shortest-way nlerp) starting from last frame's value (AnimationPose::reset keeps it), and the machine blends that into
+ * its own final pose with the layer weight 1 (machine/mod.rs:344-385).  A source without root motion adds the default.
+ * The groups' blends run from the first frame on which any animation of the context has root-motion settings; before it,
+ * a group that has been evaluated reports zero motion and the identity rotation, the fold of default motions for finite
+ * weights (with an infinite or NaN weight the reference's fold would already be NaN there). */
+int32_t fyx_anim_get_group_root_motions(fyx_ctx *ctx, uint32_t first_group, uint32_t count, fyx_root_motion *out);
 
 /* ---- N3: draw-prep after the cull (SURVEY §8f) ------------------------------------------------ */
 /* What RenderDataBundleStorage::push and RenderDataBundle::write_uniforms do per visible surface on the CPU
